@@ -2,7 +2,7 @@
 `--label_nc 35 --loadSize 2048 --n_scales_spatial 3 --use_instance --fg --use_single_G`,
 scripts/street/test_2048.sh) on synthetic 35-label sequences with random-init weights.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg4|cfg2|tiny]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload cfg4|cfg2|tiny] [--dump-outputs DIR]
 
 A step = one steady-state generated frame (all three scales).  One process per GPU; N > 1 runs N
 independent clips (inference has no exchange step: "replicas only", weak scaling) and reports the
@@ -15,12 +15,18 @@ measured in the same run and reported beside it under `fast`.
   value        device-resident inputs, CUDA-event timed (what the kernels can do)
   e2e          the public streaming API with HOST buffers: one pinned uint8 label frame -> H2D -> ... -> uint8 RGB frame
                (util.tensor2im on the device) -> D2H into pinned memory, every step inside the timed region
-  roofline     the tcgen05 conv kernel: algorithmic conv FLOPs of a frame / summed device time of its launches
-               (per-launch CUDA events, v2v_plan_profile) against MEASURED_PEAKS.json dense bf16 (burst)
+  roofline     the wgmma conv kernel: algorithmic conv FLOPs of a frame / summed device time of its launches
+               (per-launch CUDA events, v2v_plan_profile) against the H100 SXM data-sheet dense bf16 rate
   cpu_baseline the reference's own Vid2VidModelG.inference (unmodified, vendored into the git-ignored oracle/_ref by
                oracle/make_ref.py; CPU shims of oracle/ref_shim.py) timed on the host cores on a band of one steady-state
                frame of the same workload (kind "reference"; the oracle port, kind "port", only if no reference travelled)
 `--impl reference` times the same CPU arm as the reference line.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step returned to its caller as DIR/<name>.npy (float32;
+loss values float64): per arithmetic mode the generated frame of Vid2VidModelG.inference and the uint8 frame of the streaming
+API (inference workloads), the loss values (training), flow and confidence (flownet2).  An array of more than 2^21 elements
+is stored as a fixed sample of its flattened values (seeded, the same indices for the same shape), so that DIR stays under
+64 MB.  Inputs and weights are seeded: two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -67,8 +73,33 @@ def frame_macs(wl):
     return total
 
 
+DUMP_MAX_ELEMS = 1 << 21
+
+
+def dump_outputs(dirname, arrays):
+    """{name: tensor or array} -> dirname/<name>.npy (see the module docstring)."""
+    import numpy as np
+    import torch
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in arrays.items():
+        a = a.detach().cpu().double().numpy() if isinstance(a, torch.Tensor) else np.asarray(a, dtype=np.float64)
+        if not name.startswith('loss'):
+            a = a.astype(np.float32)
+        if a.size > DUMP_MAX_ELEMS:
+            idx = np.sort(np.random.default_rng(a.size).choice(a.size, DUMP_MAX_ELEMS, replace=False, shuffle=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(dirname, name + '.npy'), a)
+
+
+def loss_arrays(losses, losses_T):
+    """The (loss dict, [temporal loss dicts]) of Trainer.step -> {'loss_<name>': value, 'loss_T<scale>_<name>': value}."""
+    out = {'loss_' + k: v for k, v in losses.items()}
+    out.update({'loss_T%d_%s' % (i, k): v for i, d in enumerate(losses_T) for k, v in d.items()})
+    return out
+
+
 class ClockSampler(threading.Thread):
-    """SM clock and throttle reasons during the timed region (B200_PROFILING.md): NVML every 50 ms, nvidia-smi fallback."""
+    """SM clock and throttle reasons during the timed region: NVML every 50 ms, nvidia-smi fallback."""
 
     REASONS = {'hw_slowdown': 0x8, 'sw_thermal_slowdown': 0x20, 'hw_thermal_slowdown': 0x40, 'sw_power_cap': 0x4}
 
@@ -131,7 +162,7 @@ class ClockSampler(threading.Thread):
 
 def reduce_times(times_ms, world, device='cpu'):
     """Device-timed durations -> the slowest rank's (replicas finish when the last one does).  One all-reduce(MAX) on the
-    job's process group (NCCL on the GPU box, gloo in the CPU tests); the data path itself has no collective."""
+    job's process group (NCCL on the GPUs, gloo in the CPU tests); the data path itself has no collective."""
     import torch
     t = torch.tensor(list(times_ms), device=device, dtype=torch.float64)
     if world > 1:
@@ -141,17 +172,14 @@ def reduce_times(times_ms, world, device='cpu'):
 
 
 def peaks():
-    """(dense bf16 burst TFLOP/s, sustained TFLOP/s, HBM GB/s, source)."""
-    p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get('bf16_tflops', 1665.0), d.get('bf16_tflops_sustained', 1381.2), d.get('hbm_gbs', 6570.9), 'measured (MEASURED_PEAKS.json)'
-    return 1665.0, 1400.0, 6650.0, 'fallback (B200_PROFILING.md)'
+    """(dense bf16 TFLOP/s, HBM GB/s, source): NVIDIA's H100 SXM data sheet (700 W).  A card run at a lower power limit, or
+    one that lowers its clocks under sustained load, does not reach them."""
+    return 989.0, 3350.0, 'H100 SXM data sheet (700 W), dense bf16'
 
 
 # ----------------------------------------------------------------------------------------------- ours
 MODES = ('precise', 'fast')
-DTYPE = {'precise': 'bf16x3 (split-bf16 hi/lo operands, 3 tcgen05.mma per K block, fp32 accumulate: fp32-class)',
+DTYPE = {'precise': 'bf16x3 (split-bf16 hi/lo operands, 3 wgmma per K block, fp32 accumulate: fp32-class)',
          'fast': 'bf16 (bf16 operands, fp32 accumulate)'}
 
 
@@ -188,7 +216,7 @@ def run_ours(args, rank, world, local_rank):
     modes = [m for m in MODES if args.modes in ('both', m)]
     sampler = ClockSampler(local_rank)
     sampler.start()
-    res = {}
+    res, dumps = {}, {}
     t = 0
     gc.collect()
     for mode in modes:
@@ -210,11 +238,13 @@ def run_ours(args, rank, world, local_rank):
         e0.record()
         for _ in range(K):
             A = seq_dev[:, t:t + tG]
-            model.inference(A, None, A)
+            last = model.inference(A, None, A)
             t += 1
         e1.record()
         barrier()
         ms_dev = e0.elapsed_time(e1)
+        if args.dump_outputs:
+            dumps[mode + '_fake_B'] = last[0].cpu()
         launches = L.LAUNCHES[0] - l0
         # ---- timed: end to end through the public streaming API with HOST buffers: one pinned uint8 label frame (and the
         # instance-id frame: the same synthetic map) -> H2D -> window push -> inference -> tensor2im on device -> D2H uint8
@@ -232,6 +262,8 @@ def run_ours(args, rank, world, local_rank):
         barrier()
         gc.enable()
         ms_e2e = e2.elapsed_time(e3)
+        if args.dump_outputs:
+            dumps[mode + '_stream_frame_u8'] = out_u8.clone()
         ms_dev, ms_e2e = reduce_times([ms_dev, ms_e2e], world, dev)
         res[mode] = dict(ms_dev=ms_dev, ms_e2e=ms_e2e, launches=launches)
     sampler.stop_flag = True
@@ -239,6 +271,8 @@ def run_ours(args, rank, world, local_rank):
     d2h = 3 * H * Wd             # uint8 RGB frame
     if rank != 0:
         return
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dumps)
 
     # ---- first-frame generator (--use_single_G; runs tG - 1 times per clip, not per frame): timed separately (SURVEY 8d)
     first_ms = None
@@ -256,13 +290,8 @@ def run_ours(args, rank, world, local_rank):
         first_ms = f0.elapsed_time(f1) / 3
 
     # ---- roofline of the conv kernel per mode (per-launch CUDA events over one more frame, v2v_plan_profile)
-    peak_burst, peak_sust, peak_gbs, peak_src = peaks()
+    peak_burst, peak_gbs, peak_src = peaks()
     fmacs = frame_macs(args.workload)
-    traffic_db = {}
-    try:
-        traffic_db = json.load(open(os.path.join(ROOT, 'profiles', 'conv_dram_traffic.json')))
-    except Exception:
-        pass
 
     def roofline(mode):
         conv_ms, conv_macs, other_ms, conv_launches, kind_ms = 0.0, 0.0, 0.0, 0, {}
@@ -280,16 +309,13 @@ def run_ours(args, rank, world, local_rank):
                     else:
                         other_ms += ms
         achieved = 2.0 * conv_macs / (conv_ms * 1e-3) / 1e12 if conv_ms > 0 else 0.0
-        tj = traffic_db.get('%s_%s' % (args.workload, mode)) or (traffic_db.get(args.workload) if mode == 'fast' else None) or {}
         passes = 3 if mode == 'precise' else 1
         return {'bound': 'tensor', 'kernel': 'conv_umma_kernel (all launches of one frame)', 'achieved': achieved, 'peak': peak_burst,
                 'unit': 'TFLOP/s', 'frac': achieved / peak_burst,
-                'peak_source': peak_src + ': dense bf16 burst (kernels are timed one launch at a time); sustained %.1f' % peak_sust,
+                'peak_source': peak_src + ' (kernels are timed one launch at a time)',
                 'mma_passes_per_k_block': passes,
                 'issued_tensor_tflops': achieved * passes, 'frac_of_issued_mma_work': achieved * passes / peak_burst,
-                'traffic': tj.get('dram_bytes_per_launch_avg'),
-                'traffic_unit': 'bytes per launch (dram read + write, ncu, mean over the launches of a frame)',
-                'traffic_source': tj.get('source'), 'launches_per_frame': conv_launches,
+                'traffic': None, 'launches_per_frame': conv_launches,
                 'algorithmic_flops_per_launch_avg': 2.0 * conv_macs / max(conv_launches, 1),
                 'avg_launch_us': 1e3 * conv_ms / max(conv_launches, 1),
                 'conv_kernel_ms_per_frame': conv_ms, 'other_kernels_ms_per_frame': other_ms,
@@ -312,7 +338,7 @@ def run_ours(args, rank, world, local_rank):
         'dtype': head['dtype'], 'data': 'synthetic 35-label blocky sequences, random-init weights (N(0,0.02))',
         'config': {'workload': wl['desc'], 'parallelism': 'replicas x%d (independent clips, no collective)' % world,
                    'frames_per_step': 1, 'conv_flops_per_frame': 2 * fmacs, 'precision_mode': modes[0],
-                   'l2_policy': 'per-frame working set (weights 0.8 GB + activations) is far larger than the 126 MB L2'},
+                   'l2_policy': 'per-frame working set (weights 0.8 GB + activations) is far larger than the 50 MB L2'},
         'e2e': head['e2e'], 'gpu_launches': head['gpu_launches'], 'clocks': sampler.summary(), 'roofline': head['roofline'],
         'first_frame_generator_ms': first_ms,
     }
@@ -326,7 +352,7 @@ def run_ours(args, rank, world, local_rank):
 # ----------------------------------------------------------------------------------------------- CPU arm
 def _cpu_model(workload, threads):
     """(step(H, n, seed) -> seconds per frame, kind).  kind 'reference': the UNMODIFIED reference Vid2VidModelG.inference
-    (/root/reference here, its vendored copy oracle/_ref on the GPU box) under the CPU shims of oracle/ref_shim.py;
+    (its copy in oracle/_ref, made by oracle/make_ref.py where the reference tree is available) under the CPU shims of oracle/ref_shim.py;
     kind 'port': the oracle restatement, only when no reference tree travelled."""
     import torch
     from vid2vid_b200.utils import synth_label_sequence
@@ -434,7 +460,7 @@ def run_reference(args, rank, world):
 # ----------------------------------------------------------------------------------------------- training step (cfg3)
 def run_train(args, rank, world, local_rank):
     """BASELINE config 3: `python bench.py --workload cfg3 [--gpus N]`.  A step = one iteration of train.py's inner loop on one
-    clip per GPU (n_frames_load = 1 generated frame): generator forward (tcgen05, precise mode), FlowNet2 (no grad), image and
+    clip per GPU (n_frames_load = 1 generated frame): generator forward (wgmma, precise mode), FlowNet2 (no grad), image and
     temporal discriminator losses, the three backward passes (data gradients as forward convs on conv_umma_kernel, weight
     gradients on wgrad_umma_kernel, both in the split-bf16 precise arithmetic; norm / head / composite / loss backward on CUDA
     cores), ONE flat NCCL all-reduce over [G | D | D_T] and the Adam steps.  value = clips
@@ -505,7 +531,7 @@ def run_train(args, rank, world, local_rank):
     for _ in range(K):
         t_wall = time.perf_counter()
         a, b = A[:, t:t + tG].to(dev, non_blocking=True), B[:, t:t + tG].to(dev, non_blocking=True)     # H2D of the step's inputs
-        losses, _ = tr.step(a, b, a)           # ... and the D2H read of its loss values (one stacked copy to pinned host memory)
+        losses, losses_T = tr.step(a, b, a)    # ... and the D2H read of its loss values (one stacked copy to pinned host memory)
         t += 1
         step_wall.append((time.perf_counter() - t_wall) * 1e3)
     e1.record()
@@ -514,6 +540,8 @@ def run_train(args, rank, world, local_rank):
     sampler.stop_flag = True
     ms = e0.elapsed_time(e1)
     launches = L.LAUNCHES[0] - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss_arrays(losses, losses_T))
     ar = sum(x.elapsed_time(y) for x, y in ar_ms) / max(len(ar_ms), 1)
     ms, ar = reduce_times([ms, ar], world, dev)
     if rank != 0:
@@ -523,7 +551,7 @@ def run_train(args, rank, world, local_rank):
         for key, ent in getattr(G, 'netG%d' % s)._plans().items():
             if 'train' in key:
                 gmacs += ent['plan'].conv_macs
-    peak_burst, peak_sust, peak_gbs, peak_src = peaks()
+    peak_burst, peak_gbs, peak_src = peaks()
     step_ms = ms / K
     fl = 3 * 2 * gmacs                    # forward + data gradient + weight gradient of every generator convolution
     out = {'metric': 'training clips/sec (%s)' % args.workload, 'value': world * K / (ms * 1e-3), 'unit': 'clips/s', 'n_gpus': world, 'steps': K,
@@ -589,10 +617,12 @@ def run_flownet2(args, rank, world, local_rank):
     e0, e1, e2, e3 = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
     e0.record()
     for t in range(Wm, Wm + K):
-        F(frames_dev[t + 1:t + 2], frames_dev[t:t + 1])
+        flow, conf = F(frames_dev[t + 1:t + 2], frames_dev[t:t + 1])
     e1.record()
     barrier()
     launches = L.LAUNCHES[0] - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {'flow': flow, 'conf': conf})
     e2.record()
     for t in range(Wm, Wm + K):
         a, b = frames[t + 1:t + 2].to(dev, non_blocking=True), frames[t:t + 1].to(dev, non_blocking=True)
@@ -612,7 +642,7 @@ def run_flownet2(args, rank, world, local_rank):
                 conv_ms += ms; conv_macs += macs; n_conv += 1
             else:
                 other_ms += ms
-    peak_burst, peak_sust, peak_gbs, peak_src = peaks()
+    peak_burst, peak_gbs, peak_src = peaks()
     ach = 2.0 * conv_macs / (conv_ms * 1e-3) / 1e12 if conv_ms else 0.0
     out = {'metric': 'frame pairs/sec (FlowNet2 1024x512)', 'value': world * K / (ms_dev * 1e-3), 'unit': 'pairs/s', 'n_gpus': world, 'steps': K,
            'warmup': Wm, 'ms_per_step': ms_dev / K, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': DTYPE['precise'],
@@ -656,7 +686,11 @@ def main():
     ap.add_argument('--workload', default='cfg4', choices=list(WORKLOADS))
     ap.add_argument('--no-cpu-baseline', dest='no_cpu_baseline', action='store_true')
     ap.add_argument('--modes', default='both', choices=['both', 'precise', 'fast'])
+    ap.add_argument('--dump-outputs', dest='dump_outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step to DIR/<name>.npy')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
     rank = int(os.environ.get('RANK', '0'))
     world = int(os.environ.get('WORLD_SIZE', '1'))
     local_rank = int(os.environ.get('LOCAL_RANK', '0'))

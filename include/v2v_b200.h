@@ -1,4 +1,4 @@
-/* vid2vid-b200 -- C ABI of the sm_100a frame-synthesis engine (libv2v_b200.so).
+/* vid2vid-b200 -- C ABI of the sm_90a (H100) frame-synthesis engine (libv2v_b200.so).
  *
  * Plain pointers and sizes only: no torch / ATen types cross this boundary.  Every function returns
  * 0 on success and a non-zero code on failure (cudaError_t value, or V2V_ERR_* below);
@@ -36,7 +36,7 @@ enum { V2V_ACT_NONE = 0, V2V_ACT_RELU = 1, V2V_ACT_LRELU = 2, V2V_ACT_TANH = 3, 
 enum { V2V_NORM_NONE = 0, V2V_NORM_BATCH = 1, V2V_NORM_INSTANCE = 2 };
 enum { V2V_IMPL_UMMA = 0, V2V_IMPL_SIMT = 1 };
 /* Arithmetic of the convolution stack (accumulation is fp32 in both):
- *   V2V_PREC_BF16    operands rounded to bf16, one tcgen05.mma per K block ("fast"; ~2^-9 relative operand error)
+ *   V2V_PREC_BF16    operands rounded to bf16, one wgmma per K block ("fast"; ~2^-9 relative operand error)
  *   V2V_PREC_BF16X3  fp32-class: every operand x is carried as hi = bf16(x), lo = bf16(x - hi) and the kernel accumulates
  *                    A_hi*B_hi + A_lo*B_hi + A_hi*B_lo (three MMAs per K block, ~2^-17 relative); raw conv outputs and
  *                    norm statistics stay fp32.  This is the mode whose results are compared with the fp32 reference

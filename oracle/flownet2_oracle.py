@@ -189,7 +189,7 @@ def flow_and_conf(sd, im1, im2):
 
 def det_state_dict(keys_shapes, seed=0):
     """Weights that depend only on (seed, key, shape): Xavier-uniform filters, as the reference initialises them
-    (models.py:68-77), and small positive biases.  Lets the GPU box rebuild the exact 162 M parameters the golden fixture
+    (models.py:68-77), and small positive biases.  Lets a machine without the reference rebuild the exact 162 M parameters the golden fixture
     was produced with from the 220-entry key list in tests/golden/flownet2_keys.json."""
     import zlib
     sd = {}

@@ -8,10 +8,9 @@ Parameters come from a state_dict with the reference's own key names, so the sam
 dict drives the reference modules (oracle/ref_shim.py), this restatement and the CUDA path.
 
 Parity pin: there are no reference tests / golden vectors (SURVEY.md 4) -> the pin is the
-reference itself, imported in the build container: tests/test_oracle_vs_reference.py checks
-every function here against the reference modules (bit-exact or <=1e-5), and
-oracle/make_golden.py writes the outputs to tests/golden/ so the GPU box (no /root/reference)
-can re-check this file against them.
+reference itself: oracle/make_golden.py runs the reference modules on seeded inputs and stores their
+outputs in tests/golden/, and tests/test_oracle_vs_reference.py / tests/test_oracle_vs_golden.py check
+every function here against them (bit-exact or <=1e-5).
 """
 import torch
 import torch.nn.functional as F

@@ -1,9 +1,9 @@
 """TEST INFRASTRUCTURE.  Generates tests/golden/*.npz by running the UNMODIFIED reference
-(imported from /root/reference through oracle/ref_shim.py) on the seeded cases of
-tests/cases.py.  Run in the build container:   python -m oracle.make_golden [case ...]
+(imported through oracle/ref_shim.py, V2V_REFERENCE_ROOT) on the seeded cases of
+tests/cases.py.  Run where the reference tree is available:   python -m oracle.make_golden [case ...]
 
-The fixtures are what pins oracle/generator_oracle.py and the CUDA path on the GPU box,
-where the reference tree does not exist.
+The fixtures are what pins oracle/generator_oracle.py, oracle/losses_oracle.py, the host helpers
+and the CUDA path: the tests regenerate the weights and inputs from the seeds and compare with them.
 """
 import os
 import sys
@@ -102,10 +102,27 @@ def run_case(name, c):
     finally:
         if c.get('align_corners'):
             F.grid_sample = orig
+    save_fixture(name, out)
+
+
+PART_BYTES = 900 * 1024
+
+
+def save_fixture(name, arrays):
+    """tests/golden/<name>.npz, continued in <name>_2.npz, ... so that no file exceeds 1 MB (tests/cases.load_golden)."""
     os.makedirs(OUT, exist_ok=True)
-    path = os.path.join(OUT, name + '.npz')
-    np.savez_compressed(path, **out)
-    print('%-14s %7.1f KB  %s' % (name, os.path.getsize(path) / 1024, sorted(out)))
+    parts, cur, size = [], {}, 0
+    for k, v in arrays.items():
+        if cur and size + v.nbytes > PART_BYTES:
+            parts.append(cur)
+            cur, size = {}, 0
+        cur[k] = v
+        size += v.nbytes
+    parts.append(cur)
+    for i, part in enumerate(parts):
+        path = os.path.join(OUT, name + ('.npz' if i == 0 else '_%d.npz' % (i + 1)))
+        np.savez_compressed(path, **part)
+        print('%-14s %7.1f KB  %s' % (os.path.basename(path), os.path.getsize(path) / 1024, sorted(part)))
 
 
 def dump_keys():
@@ -161,6 +178,141 @@ def flownet2_golden():
         os.path.getsize(path) / 1024, float(flow.pow(2).mean().sqrt()), float(wflow.pow(2).mean().sqrt()), float(wconf.mean())))
 
 
+def reference_checks():
+    """Reference outputs (and gradients) on the seeded inputs of tests/test_oracle_vs_reference.py,
+    tests/test_losses_oracle.py, tests/test_flownet2_oracle.py and tests/test_gpu_integration.py -> tests/golden/reference*.npz,
+    and the reference BaseModel's schedule / checkpoint behaviour of tests/test_host_schedule.py -> host_schedule.json.
+    Every module is filled with det_fill_ (FlowNet2: flownet2_oracle.det_state_dict), so the tests rebuild the same
+    weights on their own modules."""
+    import json
+    import tempfile
+    import types
+    from oracle import generator_oracle as GO
+    import reference_inputs as RI
+    N = ref_shim.networks()
+    out = {}
+
+    def put(prefix, tensors):
+        for k, t in tensors.items():
+            if t is not None:
+                out[prefix + '/' + k] = _np(t)
+
+    with torch.no_grad():
+        for fg, no_flow, nd in RI.COMPOSITE_VARIANTS:
+            opt = make_opt(ngf=8, n_blocks=3, fg=fg, no_flow=no_flow, n_downsample_G=nd, gpu_ids=[])
+            net = det_fill_(N.define_G(18, 3, 6, 8, 'composite', nd, 'batch', 0, [], opt), seed=1)
+            inp, img_prev, mask = RI.gen_inputs(6, 16, 32)
+            put(RI.composite_key(fg, no_flow, nd), dict(zip(C.GEN_OUT_NAMES, net(inp, img_prev, mask, None, None, None, False))))
+        opt = make_opt(ngf=8, n_blocks_local=2, fg=True, gpu_ids=[])
+        net = det_fill_(N.define_G(18, 3, 6, 4, 'compositeLocal', 3, 'batch', 1, [], opt), seed=2)
+        inp, img_prev, mask = RI.gen_inputs(6, 16, 32)
+        put('composite_local', dict(zip(C.GEN_OUT_NAMES, net(inp, img_prev, mask, *RI.local_coarse(), False))))
+        opt = make_opt(n_blocks=2, n_blocks_local=2, gpu_ids=[])
+        x = RI.single_image_input()
+        put('single', {'global': det_fill_(N.define_G(5, 3, 0, 8, 'global', 2, 'instance', 0, [], opt), seed=3)(x),
+                       'local': det_fill_(N.define_G(5, 3, 0, 4, 'local', 2, 'instance', 0, [], opt), seed=4)(x)})
+        net = det_fill_(N.define_D(9, 8, 3, 'batch', 2, True, []), seed=5)
+        put('D', {'t%d_l%d' % (i, j): t for i, tower in enumerate(net(RI.discriminator_input())) for j, t in enumerate(tower)})
+        # Vid2VidModelG.inference, two scales, --fg --use_single_G
+        opt = RI.inference_opt()
+        single = det_fill_(N.define_G(5, 3, 0, 8, 'global', 2, 'instance', 0, [], opt), seed=9)
+        m = ref_shim.make_model_G(opt, single)
+        det_fill_(m.netG0, seed=10)
+        det_fill_(m.netG1, seed=11)
+        seq = RI.inference_sequence()
+        for t in range(3):
+            A = seq[:, t:t + 3]
+            fake_B, real_A = m.inference(A, None, A)
+            put('inference/%d' % t, {'fake_B': fake_B, 'real_A': real_A})
+        # Vid2VidModelG.forward (training), two calls continuing from the returned fake_B_prev pyramid
+        for no_first_img in (False, True):
+            opt = RI.train_opt(no_first_img)
+            m = ref_shim.make_model_G(opt)
+            det_fill_(m.netG0, seed=20)
+            det_fill_(m.netG1, seed=21)
+            C.condition_flow_heads(m.netG0, 0.05)
+            C.condition_flow_heads(m.netG1, 0.05)
+            seq, real = RI.train_clip(opt)
+            prev = None
+            for call in range(2):
+                A, B = RI.train_call_inputs(seq, real, opt, call)
+                r = m.forward(A, B, A, prev)
+                put('train_forward/%d/%d' % (int(no_first_img), call), dict(zip(RI.TRAIN_OUT_NAMES, r[:6])))
+                put('train_forward/%d/%d' % (int(no_first_img), call), {'prev_%d' % i: t for i, t in enumerate(r[6])})
+                prev = r[6]
+    # gradients of one scalar objective over every output of a coarse generator
+    opt = make_opt(ngf=8, n_blocks=2, fg=True, n_downsample_G=2, gpu_ids=[])
+    net = det_fill_(N.define_G(18, 3, 6, 8, 'composite', 2, 'batch', 0, [], opt), seed=31)
+    C.condition_flow_heads(net, 0.05)
+    inp, img_prev, mask = RI.gen_inputs(6, 16, 32, seed=2)
+    x_r, p_r = inp.clone().requires_grad_(True), img_prev.clone().requires_grad_(True)
+    outs = net(x_r, p_r, mask, None, None, None, False)
+    RI.objective(outs, RI.cotangents(outs)).backward()
+    put('grad', {k: v.grad for k, v in net.named_parameters()})
+    put('grad', {'input': x_r.grad, 'img_prev': p_r.grad})
+    # training losses of Vid2VidModelD.forward (--no_vgg)
+    ref_shim.install()
+    from models.vid2vid_model_D import Vid2VidModelD          # noqa (reference module)
+    for tag, kw in RI.LOSS_MODELS.items():
+        opt = RI.loss_opt(**kw)
+        opt.add_face_disc = False
+        m = Vid2VidModelD()
+        m.initialize(opt)
+        det_fill_(m.netD, seed=RI.D_SEED)
+        det_fill_(m.netD_T0, seed=RI.D_T_SEED)
+        with torch.no_grad():
+            if tag == 'temporal':
+                put('losses/' + tag, dict(zip(RI.LOSS_NAMES_T, m.forward(1, RI.temporal_loss_inputs(opt)))))
+            else:
+                put('losses/' + tag, dict(zip(RI.LOSS_NAMES, m.forward(0, RI.spatial_loss_inputs(opt, kw['no_first_img'], tag == 'raw')))))
+    # FlowNet2: the network, its sub-networks and the vid2vid wrapper on deterministic weights
+    from oracle import flownet2_oracle as FO
+    F2 = ref_shim.flownet2_class()
+    fnet = F2().eval()
+    fnet.load_state_dict(FO.det_state_dict([[k, list(v.shape)] for k, v in fnet.state_dict().items()], seed=RI.FLOWNET_SEED))
+    from models.flownet import FlowNet                                                        # noqa (reference module)
+    from models.flownet2_pytorch.networks.resample2d_package.resample2d import Resample2d     # noqa
+    stub = types.SimpleNamespace(flowNet=fnet, resample=Resample2d())
+    stub.norm = lambda t: FlowNet.norm(stub, t)
+    fi = RI.flownet_inputs()
+    with torch.no_grad():
+        put('flownet2', {'pair': fnet(fi['pair']), 'c': fnet.flownetc(fi['x6'])[0], 's': fnet.flownets_1(fi['x12'])[0],
+                         'sd': fnet.flownets_d(fi['x6'])[0], 'fusion': fnet.flownetfusion(fi['xf'])})
+        for h, w in RI.FLOWNET_WRAPPER_SIZES:
+            f, c = FlowNet.compute_flow_and_conf(stub, *RI.flownet_wrapper_inputs(h, w))
+            put('flownet2', {'wrapper_flow_%dx%d' % (h, w): f, 'wrapper_conf_%dx%d' % (h, w): c})
+        fnet.load_state_dict(FO.det_state_dict([[k, list(v.shape)] for k, v in fnet.state_dict().items()], seed=7))
+        put('flownet2', {'pair_128x192': fnet(RI.flownet_pair_128x192())})
+    save_fixture('reference', out)
+
+    # BaseModel: learning-rate schedule, frame-count schedule, fixed-parameter release, checkpoint file
+    ref_shim.install()
+    from models.base_model import BaseModel                   # noqa (reference module)
+    with tempfile.TemporaryDirectory() as tmp:
+        opt = RI.schedule_opt(tmp)
+        ref = RI.schedule_state(opt, BaseModel)
+        ref.save_dir = os.path.join(tmp, 'ref')
+        os.makedirs(ref.save_dir)
+        rec = {'lr': [], 'batch': []}
+        for epoch in RI.SCHEDULE_EPOCHS:
+            ref.update_learning_rate(epoch, 'G')
+            rec['lr'].append([ref.old_lr, [g['lr'] for g in ref.optimizer_G.param_groups]])
+        for ratio in RI.SCHEDULE_RATIOS:
+            ref.update_training_batch(ratio)
+            rec['batch'].append([ref.n_frames_bp, ref.n_frames_per_gpu, ref.n_frames_load])
+        ref.update_fixed_params()
+        rec['finetune_all'] = bool(ref.finetune_all)
+        rec['n_params_after_release'] = sum(p.numel() for g in ref.optimizer_G.param_groups for p in g['params'])
+        rec['lr_after_release'] = ref.optimizer_G.param_groups[0]['lr']
+        ref.save_network(ref.netG1, 'G1', 'latest', [])
+        rec['checkpoint_files'] = sorted(os.listdir(ref.save_dir))
+        saved = torch.load(os.path.join(ref.save_dir, 'latest_net_G1.pth'))
+        rec['checkpoint'] = {k: {'shape': list(v.shape), 'values': v.flatten().tolist()} for k, v in saved.items()}
+    with open(os.path.join(OUT, 'host_schedule.json'), 'w') as f:
+        json.dump(rec, f, indent=1)
+    print('host_schedule.json', rec)
+
+
 if __name__ == '__main__':
     names = sys.argv[1:] or (list(C.CASES) + ['keys'])
     for n in names:
@@ -168,5 +320,7 @@ if __name__ == '__main__':
             dump_keys()
         elif n == 'flownet2':
             flownet2_golden()
+        elif n == 'reference_checks':
+            reference_checks()
         else:
             run_case(n, C.CASES[n])

@@ -1,10 +1,10 @@
 """TEST INFRASTRUCTURE -- not product code.
 
-Imports the *unmodified* reference (NVIDIA/vid2vid at /root/reference, or its vendored copy
-oracle/_ref/ made by oracle/make_ref.py where /root/reference does not exist) on CPU under the
-installed PyTorch with the harness-level shims of SURVEY.md 8(c).  Used by oracle/make_golden.py to
-produce the committed fixtures in tests/golden/, by the `not gpu` tests that pin oracle/*.py against
-the reference itself, and by bench.py's reference arm (the reference's own modules on the host cores).
+Imports the *unmodified* reference (NVIDIA/vid2vid: the tree named by V2V_REFERENCE_ROOT, else the
+copy oracle/make_ref.py made in the git-ignored oracle/_ref/) on CPU under the installed PyTorch with the
+harness-level shims of SURVEY.md 8(c).  Used by oracle/make_golden.py to produce the committed fixtures in
+tests/golden/, by the GPU integration tests that run the reference's own modules, and by bench.py's
+reference arm (the reference's own modules on the host cores).
 
 Shims (none changes reference arithmetic):
   1. Tensor.cuda / Module.cuda -> identity  (reference hard-codes .cuda(gpu_id),
@@ -19,9 +19,8 @@ import sys
 import math
 import fractions
 
-# /root/reference in the build container; on the GPU box the copy oracle/make_ref.py vendored into oracle/_ref/ (git-ignored)
 _VENDORED = os.path.join(os.path.dirname(os.path.abspath(__file__)), '_ref')
-REF_ROOT = os.environ.get('V2V_REFERENCE_ROOT') or ('/root/reference' if os.path.isdir('/root/reference/models') else _VENDORED)
+REF_ROOT = os.environ.get('V2V_REFERENCE_ROOT') or _VENDORED
 
 
 def available():

@@ -3,9 +3,27 @@ and writes tests/golden/<case>.npz) and by the parity tests (which rebuild the s
 and inputs from the seeds and compare the oracle / the CUDA path with the stored outputs).
 
 Weights never travel: `det_fill_` regenerates them from (seed, parameter name, shape)."""
+import os
+
+import numpy as np
 import torch
 
 from vid2vid_b200.utils import make_opt, synth_label_sequence
+
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
+
+
+def load_golden(name):
+    """{key: array} of the fixture tests/golden/<name>.npz and its parts <name>_2.npz, <name>_3.npz, ... (files are kept
+    under 1 MB: oracle/make_golden.py splits larger fixtures by array)."""
+    out, k, path = {}, 1, os.path.join(GOLD, name + '.npz')
+    while os.path.exists(path):
+        with np.load(path) as z:
+            out.update({key: z[key] for key in z.files})
+        k += 1
+        path = os.path.join(GOLD, '%s_%d.npz' % (name, k))
+    assert out, 'no fixture %s' % name
+    return out
 
 GEN_OUT_NAMES = ['img_final', 'flow', 'weight', 'img_raw', 'img_feat', 'flow_feat', 'img_fg_feat']
 

@@ -9,11 +9,10 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box)')
-    # The CPU oracles / reference modules evaluated inside the tests get at most 32 OpenMP threads.  On the 128-thread GPU hosts
-    # PyTorch's default (every hardware thread) was measured up to two orders of magnitude slower than 32 threads for the same
-    # reference frame (bench.py's thread calibration: 0.47 s vs 82 s per band), and one evidence run of the GPU suite went from
-    # 150 s to > 600 s on a loaded host.
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100)')
+    # The CPU oracles / reference modules evaluated inside the tests get at most 32 OpenMP threads.  On many-core GPU hosts
+    # PyTorch's default (every hardware thread) can be far slower than 32 threads for the same frame, above all on a loaded
+    # host (bench.py calibrates its CPU arm the same way).
     n = str(min(32, os.cpu_count() or 1))
     os.environ.setdefault('OMP_NUM_THREADS', n)
     os.environ.setdefault('MKL_NUM_THREADS', n)

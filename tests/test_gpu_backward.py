@@ -92,7 +92,7 @@ TENSOR_UNITS = [
 
 @pytest.mark.parametrize('unit', TENSOR_UNITS, ids=[u[0] for u in TENSOR_UNITS])
 def test_tensor_core_backward_units(unit, monkeypatch):
-    """Gradients of the tcgen05 backward (data gradient as a forward conv + fold, weight gradient with pixels as the K
+    """Gradients of the tensor-core backward (data gradient as a forward conv + fold, weight gradient with pixels as the K
     dimension) against fp64 autograd, and against the fp32 SIMT backward kernels of the same plan description."""
     name, build, shape = unit[:3]
     head, scale = (unit[3], unit[4]) if len(unit) > 3 else (None, 1.0)
@@ -115,22 +115,6 @@ def test_tensor_core_backward_units(unit, monkeypatch):
         except AssertionError as e:
             bad.append(str(e)[:160])
     assert not bad, bad
-
-
-@pytest.mark.parametrize('name', ['t_c3_128', 't_d_k4s1', 't_stem6', 't_c3_24_128', 't_d_last', 't_head_tanh', 't_head_both_narrow'])
-def test_weight_gradient_tap_rows(name, monkeypatch):
-    """V2V_WG_KX=1: the kw taps of a filter row share one patch of the activation-side operand (row-shifted MN-major descriptors,
-    one accumulator per tap) -- measured no faster than one unit per tap (profiles/r02i_wgrad_layers.txt) and therefore off by
-    default, kept correct here."""
-    monkeypatch.setenv('V2V_WG_KX', '1')
-    test_tensor_core_backward_units([u for u in TENSOR_UNITS if u[0] == name][0], monkeypatch)
-
-
-@pytest.mark.parametrize('name', ['t_c3_256_128', 't_c3_320_64'])
-def test_weight_gradient_wide_n_tiles(name, monkeypatch):
-    """V2V_WG_N256=1: 256-wide N tiles (one accumulator of 256 TMEM columns); measured neutral, off by default."""
-    monkeypatch.setenv('V2V_WG_N256', '1')
-    test_tensor_core_backward_units([u for u in TENSOR_UNITS if u[0] == name][0], monkeypatch)
 
 
 HEADS = [

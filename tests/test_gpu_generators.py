@@ -12,7 +12,6 @@ from oracle.make_golden import coarse_feats
 from vid2vid_b200.utils import det_fill_, synth_label_sequence
 
 pytestmark = pytest.mark.gpu
-GOLD = os.path.join(os.path.dirname(__file__), 'golden')
 
 # Stated tolerances against the fp32 reference (DESIGN.md 4), (max |d|, mean |d|); images and masks live in [-1,1] / [0,1],
 # features are O(1) (rms ~0.7), flow is in pixels and carries the x20*2^s head scale.
@@ -40,8 +39,7 @@ def mode(request):
     NW.set_default_precision(old)
 
 
-def load(name):
-    return dict(np.load(os.path.join(GOLD, name + '.npz')))
+load = C.load_golden
 
 
 def report(name, key, out, gold):
@@ -111,7 +109,7 @@ def test_first_frame_generators(name):
 
 
 def test_generator_simt_vs_umma_same_plan():
-    """The tcgen05 kernel and the SIMT cross-check kernel evaluate the same lowered plan."""
+    """The wgmma kernel and the SIMT cross-check kernel evaluate the same lowered plan."""
     c = C.CASES['g0_small']
     inp, img_prev, mask = (t.cuda() for t in C.gen_inputs(c['label_nc'], c['h'], c['w'], c['seed']))
     outs = []

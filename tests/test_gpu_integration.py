@@ -1,13 +1,14 @@
-"""Boundary hygiene on the GPU box (SURVEY 8b): the reference-side bindings INTEGRATION.md shows are executed for real.
+"""Boundary hygiene (SURVEY 8b): the reference-side bindings INTEGRATION.md shows are executed for real.
 
   b1  the reference-shaped pybind stubs `correlation_cuda.forward(in1, in2, rbot1, rbot2, out, ...) -> 1`,
       `resample2d_cuda.forward`, `channelnorm_cuda.forward` (INTEGRATION.md section 1) bound to libv2v_b200.so, checked
-      against the C oracle, and then installed under the UNMODIFIED reference FlowNet2 (vendored oracle/_ref): the
-      reference's own Python graph (its nn.Conv2d layers run by PyTorch on the GPU, TF32 off) with our three native ops
-      must agree with our FlowNet2 (all convolutions on tcgen05).
+      against the C oracle; and our FlowNet2 (all convolutions on the tensor cores) against the UNMODIFIED reference
+      FlowNet2's output on the same weights and frames (tests/golden/reference*.npz: its own Python graph, with the
+      C oracle standing in for the three native ops the stubs above reproduce).
   b2  the one-line `networks` swap of INTEGRATION.md section 2: the reference's own Vid2VidModelG (encode_input, build_pyr,
       compute_mask and the frame loop are the reference's code) with vid2vid_b200.networks supplying netG0..2, against our
-      Vid2VidModelG on identical weights and inputs.
+      Vid2VidModelG on identical weights and inputs.  It imports the reference's sources, which build() copies into
+      oracle/_ref (oracle/make_ref.py).
 """
 import ctypes
 import fractions
@@ -15,17 +16,17 @@ import json
 import math
 import os
 import sys
-import types
 
 import numpy as np
 import pytest
 import torch
 
+import reference_inputs as RI
 from oracle import flowops
 from oracle import ref_shim
 from vid2vid_b200 import _lib as L
 
-pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not ref_shim.available(), reason='no reference tree (run oracle/make_ref.py in the build container)')]
+pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), 'golden')
 
 
@@ -91,46 +92,22 @@ def test_reference_shaped_operator_stubs_vs_c_oracle():
         corr_forward(a, b, a.new(), b.new(), a.new(), 20, 3, 20, 1, 2, 1)      # unsupported kernel_size -> exception, like AT_ERROR
 
 
-def test_reference_flownet2_with_our_native_ops_vs_our_flownet2():
-    _ref_on_path()
-    for name, fn in (('correlation_cuda', corr_forward), ('resample2d_cuda', res_forward), ('channelnorm_cuda', cn_forward)):
-        m = types.ModuleType(name)
-        m.forward = fn
-        sys.modules[name] = m
-    from models.flownet2_pytorch.networks.correlation_package import correlation as ref_corr   # noqa (reference module)
-
-    def forward(self, input1, input2):      # the legacy autograd Function wrapper does not run on current PyTorch
-        out = input1.new()
-        sys.modules['correlation_cuda'].forward(input1, input2, input1.new(), input2.new(), out, self.pad_size, self.kernel_size,
-                                                self.max_displacement, self.stride1, self.stride2, self.corr_multiply)
-        return out
-    ref_corr.Correlation.forward = forward
-    from models.flownet2_pytorch import models as ref_models   # noqa (reference module)
+def test_reference_flownet2_vs_our_flownet2():
     from oracle import flownet2_oracle as FO
     from vid2vid_b200 import flownet as FN
     keys = json.load(open(os.path.join(GOLD, 'flownet2_keys.json')))
-    sd = FO.det_state_dict(keys, seed=7)
-    ref = ref_models.FlowNet2().eval().cuda()
-    ref.load_state_dict(sd)
     ours = FN.FlowNet2()
-    ours.load_state_dict(sd)
+    ours.load_state_dict(FO.det_state_dict(keys, seed=7))
     ours = ours.cuda()
-    g = torch.Generator().manual_seed(8)
-    base = torch.rand(1, 3, 128, 192, generator=g)
-    pair = torch.stack([base, torch.roll(base, shifts=(1, 2), dims=(2, 3)) * 0.9 + 0.05], 2).cuda()
-    tf32 = torch.backends.cudnn.allow_tf32
-    torch.backends.cudnn.allow_tf32 = False
-    try:
-        with torch.no_grad():
-            r = ref(pair)
-            o = ours(pair)
-    finally:
-        torch.backends.cudnn.allow_tf32 = tf32
+    r = torch.from_numpy(RI.golden()['flownet2/pair_128x192'])
+    with torch.no_grad():
+        o = ours(RI.flownet_pair_128x192().cuda()).cpu()
     d = (r - o).abs()
-    print('reference FlowNet2 (PyTorch convs + our ops) vs ours: max|d|=%.3e mean|d|=%.3e ref max %.3f' % (d.max(), d.mean(), r.abs().max()))
+    print('reference FlowNet2 vs ours: max|d|=%.3e mean|d|=%.3e ref max %.3f' % (d.max(), d.mean(), r.abs().max()))
     assert d.max().item() <= 2e-3 * max(1.0, r.abs().max().item())
 
 
+@pytest.mark.skipif(not ref_shim.available(), reason="build() found no reference tree to copy into oracle/_ref (oracle/make_ref.py)")
 def test_reference_model_G_with_networks_swapped_in():
     _ref_on_path()
     import models.vid2vid_model_G as ref_G          # noqa (reference module)

@@ -3,7 +3,7 @@
 * cfg4: one steady-state frame at 2048x1024, all three scales chained through Vid2VidModelG.inference (ngf 128),
   against oracle.generator_oracle.ModelGOracle on identical weights / inputs / previous frames;
 * cfg2: 32 recurrent frames at 512x256 with UN-shrunken random flow heads.  The recurrence with random weights is
-  chaotic (tools/precision_study.py, profiles/r02_precision_study_recurrence.txt: the oracle evaluated with
+  chaotic (tools/precision_study.py, on the CPU: the oracle evaluated with
   fp32-rounded operands diverges from its own fp64 evaluation by x2-x60 per frame and saturates within 4-16 frames),
   so a free-running comparison of ANY two implementations is ill-posed after a few frames.  Two well-posed forms:
     - every checked frame of the 32-frame recurrent run is compared with the oracle stepped from OUR recurrent state

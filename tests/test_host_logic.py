@@ -181,7 +181,7 @@ def test_kernel_configuration_choices():
     # 1024->1024 3x3 @32x64: 2-D patch (16x8 tiles, all 9 taps from one patch), weights streamed in 32-channel K blocks
     for c in pick(c0, Cin=1024, Cout=1024):
         assert (c['TH'], c['TW'], c['R'], c['kc'], c['BN'], c['resident'], c['MG']) == (16, 8, 9, 32, 128, 0, 1)
-        assert c['units'] == 128                       # 16 M tiles x 8 N tiles: one wave on 148 SMs
+        assert c['units'] == 128                       # 16 M tiles x 8 N tiles: one wave on 132 SMs
     # 64->64 3x3 @512x1024: 2-D patch with resident weights
     for c in pick(c2, Cin=64, Cout=64, stride=1):
         assert (c['TH'], c['TW'], c['R'], c['kc'], c['resident']) == (16, 8, 9, 64, 1)
@@ -189,10 +189,10 @@ def test_kernel_configuration_choices():
     for c in pick(c2, Cin=108, Cout=48) + pick(c0, Cin=108, Cout=192):
         assert (c['TH'], c['TW'], c['R'], c['MG'], c['resident'], c['BN'], c['kc']) == (1, 128, 7, 2, 0, 64, 64)
     for c in pick(_cfg4_convs(1, 512, 1024), Cin=108, Cout=96):
-        assert (c['MG'], c['BN'], c['kc']) == (2, 96, 32)          # exact N tile for 96 output channels
-    # every configuration respects the TMEM budget: 2 stages x MG accumulators x max(32, BN) columns <= 512
+        assert (c['MG'], c['BN'], c['kc']) == (1, 96, 32)          # exact N tile for 96 output channels
+    # every configuration respects the register budget of the accumulators: MG tiles x max(32, BN) columns <= 128
     for c in c0 + c2:
-        assert 2 * c['MG'] * max(32, c['BN']) <= 512 and c['EG'] in (1, 2) and c['CG'] >= 1 and c['SG'] >= 2
+        assert c['MG'] * max(32, c['BN']) <= 128 and c['EG'] == 1 and c['CG'] >= 1 and c['SG'] >= 2
 
 
 def test_conv_macs_discriminators():
@@ -252,7 +252,7 @@ def test_pending_losses_round_trip_on_cpu():
 
 
 def test_bench_prints_exactly_one_json_line_on_stdout():
-    """The driver parses bench.py's stdout: whatever libraries print there (NCCL's version banner on the GPU boxes) is routed to
+    """The driver parses bench.py's stdout: whatever libraries print there (NCCL's version banner, for one) is routed to
     stderr, the JSON line goes to the real stdout."""
     import json
     import subprocess
@@ -265,3 +265,43 @@ def test_bench_prints_exactly_one_json_line_on_stdout():
     lines = r.stdout.splitlines()
     assert len(lines) == 1 and json.loads(lines[0]) == {'impl': 'reference', 'ok': 1}
     assert 'noise on fd 1' in r.stderr and 'noise via print' in r.stderr
+
+
+def test_bench_dump_outputs_writes_float_arrays_and_a_fixed_sample(tmp_path):
+    """bench.dump_outputs: small arrays whole, arrays above DUMP_MAX_ELEMS as the same seeded sample on every call, loss values
+    float64; the training step's (loss dict, [temporal loss dicts]) as Trainer.step returns it goes through loss_arrays."""
+    import sys
+    sys.path.insert(0, ROOT)
+    import bench
+    from vid2vid_b200.trainer import PendingLosses
+    small = torch.arange(12, dtype=torch.float32).view(3, 4)
+    big = np.arange(bench.DUMP_MAX_ELEMS + 12345, dtype=np.float32)
+    out, out_T = PendingLosses([(None, 'G_GAN'), (0, 'D_T_fake')], torch.tensor([1.5, 4.5]), 1).get()
+    arrays = dict(small=small, big=big, **bench.loss_arrays(out, out_T))
+    assert sorted(arrays) == ['big', 'loss_G_GAN', 'loss_T0_D_T_fake', 'small']
+    for d in ('a', 'b'):
+        bench.dump_outputs(str(tmp_path / d), arrays)
+    a = {f[:-4]: np.load(str(tmp_path / 'a' / f)) for f in os.listdir(str(tmp_path / 'a'))}
+    assert sorted(a) == sorted(arrays)
+    assert a['small'].dtype == np.float32 and np.array_equal(a['small'], small.numpy())
+    assert a['loss_G_GAN'].dtype == np.float64 and float(a['loss_G_GAN']) == 1.5 and float(a['loss_T0_D_T_fake']) == 4.5
+    s = a['big']
+    assert s.dtype == np.float32 and s.size == bench.DUMP_MAX_ELEMS
+    assert np.all(np.diff(s) > 0) and np.all(np.isin(s, big))                 # sorted distinct elements of the array
+    assert np.array_equal(s, np.load(str(tmp_path / 'b' / 'big.npy')))        # the same sample again
+    assert sum(os.path.getsize(str(tmp_path / 'a' / f)) for f in os.listdir(str(tmp_path / 'a'))) < 64 << 20
+
+
+def test_bench_dump_outputs_and_steps_arguments():
+    """--dump-outputs DIR and --steps K reach the workload runner; --steps 0 is rejected."""
+    import subprocess
+    import sys
+    code = ("import sys; sys.argv = ['bench.py'] + sys.argv[1:]; import bench; "
+            "bench.main.__globals__['run_ours'] = (lambda a, r, w, lr: bench.emit({'dump': a.dump_outputs, 'steps': a.steps})); "
+            "bench.main()")
+    r = subprocess.run([sys.executable, '-c', code, '--steps', '7', '--dump-outputs', 'some/dir'], cwd=ROOT, capture_output=True,
+                       text=True, timeout=300)
+    assert r.returncode == 0, r.stderr[-500:]
+    assert json.loads(r.stdout.splitlines()[-1]) == {'dump': 'some/dir', 'steps': 7}
+    r = subprocess.run([sys.executable, '-c', code, '--steps', '0'], cwd=ROOT, capture_output=True, text=True, timeout=300)
+    assert r.returncode != 0 and '--steps' in r.stderr

@@ -1,53 +1,39 @@
 """Pins oracle/losses_oracle.py (SURVEY 8 row a13: warp / flow / GAN / feature-matching losses of the training step)
-against the unmodified reference Vid2VidModelD.forward (models/vid2vid_model_D.py:92-197) on CPU, --no_vgg.
-Needs /root/reference (build container); skipped on the GPU box."""
+against the unmodified reference Vid2VidModelD.forward (models/vid2vid_model_D.py:92-197) on CPU, --no_vgg: its loss
+values on seeded inputs, with discriminators filled by det_fill_, are stored in tests/golden/reference*.npz."""
 import pytest
 import torch
 
+import reference_inputs as RI
 from oracle import losses_oracle as LO
-from oracle import ref_shim
-from vid2vid_b200.utils import make_opt
+from vid2vid_b200 import networks as NW
+from vid2vid_b200.utils import det_fill_
 
-pytestmark = pytest.mark.skipif(not ref_shim.available(), reason='reference tree not present (GPU box)')
-
-
-def _model(**kw):
-    ref_shim.install()
-    from models.vid2vid_model_D import Vid2VidModelD          # noqa (reference module)
-    opt = make_opt(label_nc=35, use_instance=True, isTrain=True, gpu_ids=[0], n_gpus_gen=1, no_vgg=True, **kw)
-    opt.add_face_disc = False
-    opt.debug = True
-    opt.load_pretrain = ''
-    torch.manual_seed(5)
-    m = Vid2VidModelD()
-    m.initialize(opt)
-    return m, opt
+GOLD = RI.golden()
 
 
-def _rand(shape, g, lo=-1.0, hi=1.0):
-    return torch.rand(shape, generator=g) * (hi - lo) + lo
+def _discriminators(opt):
+    """netD and netD_T0 as Vid2VidModelD builds them (vid2vid_model_D.py:33-46), with the weights of the stored run."""
+    input_nc = opt.label_nc + (1 if opt.use_instance else 0) + opt.output_nc
+    nc_t = opt.output_nc * opt.n_frames_D + 2 * (opt.n_frames_D - 1)
+    netD = det_fill_(NW.define_D(input_nc, opt.ndf, opt.n_layers_D, opt.norm, opt.num_D, not opt.no_ganFeat, []), seed=RI.D_SEED)
+    netD_T = det_fill_(NW.define_D(nc_t, opt.ndf, opt.n_layers_D, opt.norm, opt.num_D, not opt.no_ganFeat, []), seed=RI.D_T_SEED)
+    return netD, netD_T
 
 
 @pytest.mark.parametrize('no_first_img,with_raw', [(False, True), (True, False)])
 def test_spatial_losses_match_reference(no_first_img, with_raw):
-    m, opt = _model(n_scales_spatial=2, no_first_img=no_first_img)
-    g = torch.Generator().manual_seed(1)
-    h, w = 48, 64
-    real_B, fake_B, real_B_prev, fake_B_prev = (_rand((1, 3, h, w), g) for _ in range(4))
-    fake_B_raw = _rand((1, 3, h, w), g) if with_raw else None
-    real_A = (_rand((1, 36, h, w), g) > 0.8).float()
-    flow, flow_ref = _rand((1, 2, h, w), g, -3, 3), _rand((1, 2, h, w), g, -3, 3)
-    weight = _rand((1, 1, h, w), g, 0, 1)
-    conf = (_rand((1, 1, h, w), g) > 0).float()
+    tag = 'raw' if with_raw else 'no_first_img'
+    opt = RI.loss_opt(**RI.LOSS_MODELS[tag])
+    assert opt.no_first_img == no_first_img
+    netD, _ = _discriminators(opt)
     with torch.no_grad():
-        ref = m.forward(0, [real_B, fake_B, fake_B_raw, real_A, real_B_prev, fake_B_prev, flow, weight, flow_ref, conf])
-        ours = LO.spatial_losses(m.netD.state_dict(), real_B, fake_B, fake_B_raw, real_A, real_B_prev, fake_B_prev, flow, weight,
-                                 flow_ref, conf, lambda_F=opt.lambda_F, lambda_T=opt.lambda_T, lambda_feat=opt.lambda_feat,
-                                 n_scales_spatial=opt.n_scales_spatial, no_first_img=no_first_img, num_D=opt.num_D,
-                                 n_layers_D=opt.n_layers_D, norm=opt.norm)
-    names = ['G_VGG', 'G_GAN', 'G_GAN_Feat', 'D_real', 'D_fake', 'G_Warp', 'F_Flow', 'F_Warp', 'W']
-    assert len(ref) == len(ours) == len(names)
-    for n, a, b in zip(names, ours, ref):
+        ours = LO.spatial_losses(netD.state_dict(), *RI.spatial_loss_inputs(opt, no_first_img, with_raw), lambda_F=opt.lambda_F,
+                                 lambda_T=opt.lambda_T, lambda_feat=opt.lambda_feat, n_scales_spatial=opt.n_scales_spatial,
+                                 no_first_img=no_first_img, num_D=opt.num_D, n_layers_D=opt.n_layers_D, norm=opt.norm)
+    assert len(ours) == len(RI.LOSS_NAMES)
+    for n, a in zip(RI.LOSS_NAMES, ours):
+        b = torch.from_numpy(GOLD['losses/%s/%s' % (tag, n)])
         # (G_VGG under --no_vgg and W without --no_first_img are zeros_like(weight): H*W rows of zeros in both)
         assert a.shape == b.shape, (n, a.shape, b.shape)
         assert torch.allclose(a, b, rtol=1e-4, atol=1e-6), (n, float(a.abs().max()), float(b.abs().max()))
@@ -56,15 +42,12 @@ def test_spatial_losses_match_reference(no_first_img, with_raw):
 
 
 def test_temporal_losses_match_reference():
-    m, opt = _model()
-    g = torch.Generator().manual_seed(2)
-    h, w, tD = 48, 64, opt.n_frames_D
-    real_B, fake_B = _rand((1, tD, 3, h, w), g), _rand((1, tD, 3, h, w), g)
-    flow_ref = _rand((1, tD - 1, 2, h, w), g, -40, 40)
-    conf = (_rand((1, tD - 1, 1, h, w), g) > 0).float()
+    opt = RI.loss_opt(**RI.LOSS_MODELS['temporal'])
+    _, netD_T = _discriminators(opt)
     with torch.no_grad():
-        ref = m.forward(1, [real_B, fake_B, flow_ref, conf])
-        ours = LO.temporal_losses(m.netD_T0.state_dict(), real_B, fake_B, flow_ref, conf, n_frames_D=tD, output_nc=3,
+        ours = LO.temporal_losses(netD_T.state_dict(), *RI.temporal_loss_inputs(opt), n_frames_D=opt.n_frames_D, output_nc=3,
                                   lambda_feat=opt.lambda_feat, num_D=opt.num_D, n_layers_D=opt.n_layers_D, norm=opt.norm)
-    for n, a, b in zip(['G_T_GAN', 'G_T_GAN_Feat', 'D_T_real', 'D_T_fake', 'G_T_Warp'], ours, ref):
+    assert len(ours) == len(RI.LOSS_NAMES_T)
+    for n, a in zip(RI.LOSS_NAMES_T, ours):
+        b = torch.from_numpy(GOLD['losses/temporal/' + n])
         assert torch.allclose(a, b, rtol=1e-4, atol=1e-6), (n, float(a), float(b))

@@ -1,7 +1,5 @@
 """Pins oracle/generator_oracle.py against the committed fixtures (outputs of the unmodified
-reference, oracle/make_golden.py).  CPU-only; this is the check that travels to the GPU box."""
-import os
-
+reference, oracle/make_golden.py).  CPU-only."""
 import numpy as np
 import pytest
 import torch
@@ -12,17 +10,16 @@ from oracle.make_golden import coarse_feats
 from vid2vid_b200.utils import det_fill_, synth_label_sequence
 from vid2vid_b200 import networks as NW
 
-GOLD = os.path.join(os.path.dirname(__file__), 'golden')
+load = C.load_golden
 
 
-def load(name):
-    return dict(np.load(os.path.join(GOLD, name + '.npz')))
-
-
-def close(a, gold, tol=3e-5):
+def close(a, gold, tol=3e-5, rtol=2e-6):
+    """max |a - gold| <= tol + rtol * max |gold|.  fp32 rounding, which depends on the CPU's summation order (thread count),
+    grows with the output's magnitude: up to 5e-5 on flows of magnitude 28 (pixels x 20) with one thread, against 2e-6
+    on images in [-1, 1]."""
     a = a.detach().numpy()
     assert a.shape == gold.shape, (a.shape, gold.shape)
-    assert np.abs(a - gold).max() <= tol, np.abs(a - gold).max()
+    assert np.abs(a - gold).max() <= tol + rtol * float(np.abs(gold).max()), np.abs(a - gold).max()
 
 
 def build_state_dict(c):

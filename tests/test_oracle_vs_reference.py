@@ -1,6 +1,6 @@
-"""Pins oracle/generator_oracle.py against the unmodified reference imported from
-/root/reference (build container only; skipped on the GPU box, where the committed
-tests/golden fixtures made by oracle/make_golden.py take over)."""
+"""Pins oracle/generator_oracle.py against the unmodified reference: its outputs (and gradients) on seeded inputs are
+stored in tests/golden/reference*.npz (oracle/make_golden.py reference_checks); the weights are regenerated here with
+det_fill_ on our own modules, whose state_dict keys and shapes equal the reference's (tests/test_oracle_vs_golden.py)."""
 import os
 import sys
 
@@ -8,104 +8,82 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), '..'))
-from oracle import ref_shim, generator_oracle as GO          # noqa: E402
-from vid2vid_b200.utils import make_opt, det_fill_, synth_label_sequence   # noqa: E402
+from oracle import generator_oracle as GO                     # noqa: E402
+from vid2vid_b200 import networks as NW                        # noqa: E402
+from vid2vid_b200.utils import make_opt, det_fill_             # noqa: E402
 import cases                                                  # noqa: E402
+import reference_inputs as RI                                 # noqa: E402
 
-pytestmark = pytest.mark.skipif(not ref_shim.available(), reason='reference tree not mounted')
-
-
-def _close(a, b, tol=2e-5):
-    assert a.shape == b.shape
-    assert (a - b).abs().max().item() <= tol, (a - b).abs().max().item()
+GOLD = RI.golden()
 
 
-def _inputs(nc, h, w, seed=0):
-    g = torch.Generator().manual_seed(seed)
-    lab = synth_label_sequence(3, h, w, label_nc=nc - 1, block=4, seed=seed)
-    real_A = GO.encode_input(lab, lab, nc - 1, True)
-    inp = real_A.view(1, -1, h, w)
-    img_prev = torch.rand(1, 6, h, w, generator=g) * 2 - 1
-    mask = (lab[:, -1] == 2).float()
-    return inp, img_prev, mask
+def _close(a, key, tol=2e-5):
+    b = torch.from_numpy(GOLD[key])
+    assert a.shape == b.shape, (key, a.shape, b.shape)
+    assert (a - b).abs().max().item() <= tol, (key, (a - b).abs().max().item())
 
 
-@pytest.mark.parametrize('fg,no_flow,nd', [(True, False, 3), (False, False, 2), (True, True, 3)])
+def _close_all(prefix, names, outs):
+    for n, o in zip(names, outs):
+        key = prefix + '/' + n
+        assert (o is None) == (key not in GOLD), key
+        if o is not None:
+            _close(o, key)
+
+
+@pytest.mark.parametrize('fg,no_flow,nd', RI.COMPOSITE_VARIANTS)
 def test_composite_generator(fg, no_flow, nd):
-    N = ref_shim.networks()
     opt = make_opt(ngf=8, n_blocks=3, fg=fg, no_flow=no_flow, n_downsample_G=nd, gpu_ids=[])
-    net = det_fill_(N.define_G(18, 3, 6, 8, 'composite', nd, 'batch', 0, [], opt), seed=1)
-    inp, img_prev, mask = _inputs(6, 16, 32)
+    sd = det_fill_(NW.define_G(18, 3, 6, 8, 'composite', nd, 'batch', 0, [], opt), seed=1).state_dict()
+    inp, img_prev, mask = RI.gen_inputs(6, 16, 32)
     with torch.no_grad():
-        ref = net(inp, img_prev, mask, None, None, None, False)
-        out = GO.composite_generator(net.state_dict(), inp, img_prev, mask, False, n_downsampling=nd,
-                                     n_blocks=3, use_fg_model=fg, no_flow=no_flow)
-    for r, o in zip(ref, out):
-        if r is None:
-            assert o is None
-        else:
-            _close(r, o)
+        out = GO.composite_generator(sd, inp, img_prev, mask, False, n_downsampling=nd, n_blocks=3, use_fg_model=fg, no_flow=no_flow)
+    _close_all(RI.composite_key(fg, no_flow, nd), cases.GEN_OUT_NAMES, out)
 
 
 def test_composite_local_generator():
-    N = ref_shim.networks()
     opt = make_opt(ngf=8, n_blocks_local=2, fg=True, gpu_ids=[])
-    net = det_fill_(N.define_G(18, 3, 6, 4, 'compositeLocal', 3, 'batch', 1, [], opt), seed=2)
-    inp, img_prev, mask = _inputs(6, 16, 32)
-    g = torch.Generator().manual_seed(5)
-    c1, c2, c3 = (torch.randn(1, c, 8, 16, generator=g) for c in (8, 8, 4))
+    sd = det_fill_(NW.define_G(18, 3, 6, 4, 'compositeLocal', 3, 'batch', 1, [], opt), seed=2).state_dict()
+    inp, img_prev, mask = RI.gen_inputs(6, 16, 32)
+    c1, c2, c3 = RI.local_coarse()
     with torch.no_grad():
-        ref = net(inp, img_prev, mask, c1, c2, c3, False)
-        out = GO.composite_local_generator(net.state_dict(), inp, img_prev, mask, c1, c2, c3, False,
-                                           n_blocks_local=2, scale=1)
-    for r, o in zip(ref, out):
-        _close(r, o)
+        out = GO.composite_local_generator(sd, inp, img_prev, mask, c1, c2, c3, False, n_blocks_local=2, scale=1)
+    _close_all('composite_local', cases.GEN_OUT_NAMES, out)
 
 
 def test_single_image_generators():
-    N = ref_shim.networks()
     opt = make_opt(n_blocks=2, n_blocks_local=2, gpu_ids=[])
-    g = torch.Generator().manual_seed(3)
-    x = torch.rand(1, 5, 32, 64, generator=g)
-    netg = det_fill_(N.define_G(5, 3, 0, 8, 'global', 2, 'instance', 0, [], opt), seed=3)
-    netl = det_fill_(N.define_G(5, 3, 0, 4, 'local', 2, 'instance', 0, [], opt), seed=4)
+    x = RI.single_image_input()
+    sdg = det_fill_(NW.define_G(5, 3, 0, 8, 'global', 2, 'instance', 0, [], opt), seed=3).state_dict()
+    sdl = det_fill_(NW.define_G(5, 3, 0, 4, 'local', 2, 'instance', 0, [], opt), seed=4).state_dict()
     with torch.no_grad():
-        _close(netg(x), GO.global_generator(netg.state_dict(), x, n_downsampling=2, n_blocks=2))
-        _close(netl(x), GO.local_enhancer(netl.state_dict(), x, n_downsample_global=2, n_blocks_global=2,
-                                          n_blocks_local=2))
+        _close(GO.global_generator(sdg, x, n_downsampling=2, n_blocks=2), 'single/global')
+        _close(GO.local_enhancer(sdl, x, n_downsample_global=2, n_blocks_global=2, n_blocks_local=2), 'single/local')
 
 
 def test_discriminator():
-    N = ref_shim.networks()
-    net = det_fill_(N.define_D(9, 8, 3, 'batch', 2, True, []), seed=5)
-    g = torch.Generator().manual_seed(6)
-    x = torch.randn(2, 9, 32, 48, generator=g)
+    sd = det_fill_(NW.define_D(9, 8, 3, 'batch', 2, True, []), seed=5).state_dict()
     with torch.no_grad():
-        ref = net(x)
-        out = GO.multiscale_discriminator(net.state_dict(), x, num_D=2, n_layers=3)
-    for rt, ot in zip(ref, out):
-        for r, o in zip(rt, ot):
-            _close(r, o)
+        out = GO.multiscale_discriminator(sd, RI.discriminator_input(), num_D=2, n_layers=3)
+    n = 0
+    for i, tower in enumerate(out):
+        for j, t in enumerate(tower):
+            _close(t, 'D/t%d_l%d' % (i, j))
+            n += 1
+    assert n == sum(1 for k in GOLD if k.startswith('D/'))
 
 
 def test_model_G_inference_multiscale():
-    N = ref_shim.networks()
-    opt = make_opt(label_nc=5, use_instance=True, fg=True, fg_labels=[2], n_scales_spatial=2, ngf=8,
-                   n_blocks=2, n_blocks_local=1, use_single_G=True, n_downsample_G=2, gpu_ids=[],
-                   dataroot='City')
-    single = det_fill_(N.define_G(5, 3, 0, 8, 'global', 2, 'instance', 0, [], opt), seed=9)
-    m = ref_shim.make_model_G(opt, single)
-    det_fill_(m.netG0, seed=10)
-    det_fill_(m.netG1, seed=11)
-    orc = GO.ModelGOracle(opt, [m.netG0.state_dict(), m.netG1.state_dict()], single.state_dict(),
-                          'global', 2)
-    seq = synth_label_sequence(5, 32, 64, label_nc=5, block=4, seed=3)
+    opt = RI.inference_opt()
+    single = det_fill_(NW.define_G(5, 3, 0, 8, 'global', 2, 'instance', 0, [], opt), seed=9)
+    sds = [det_fill_(NW.build_netG(opt, s), seed=10 + s).state_dict() for s in range(2)]
+    orc = GO.ModelGOracle(opt, sds, single.state_dict(), 'global', 2)
+    seq = RI.inference_sequence()
     for t in range(3):
         A = seq[:, t:t + 3]
-        ref_B, ref_A = m.inference(A, None, A)
         o_B, o_A = orc.inference(A, A)
-        _close(ref_B, o_B)
-        _close(ref_A, o_A)
+        _close(o_B, 'inference/%d/fake_B' % t)
+        _close(o_A, 'inference/%d/real_A' % t)
 
 
 @pytest.mark.parametrize('no_first_img', [False, True])
@@ -113,36 +91,22 @@ def test_model_G_training_forward(no_first_img):
     """Vid2VidModelG.forward / generate_frame_train (vid2vid_model_G.py:114-196): two frames per call, two calls (the
     second continues from the returned fake_B_prev pyramid), two spatial scales, foreground branch.  Batch 1, as the
     reference trains: its build_pyr `.view`s a time slice of the clip, which only works for one clip per batch."""
-    opt = make_opt(label_nc=5, use_instance=True, fg=True, fg_labels=[2], n_scales_spatial=2, ngf=8, n_blocks=2,
-                   n_blocks_local=1, n_downsample_G=2, gpu_ids=[0], n_gpus_gen=1, isTrain=True, no_first_img=no_first_img,
-                   max_frames_per_gpu=2, batchSize=1, dataroot='City')
-    m = ref_shim.make_model_G(opt)
-    assert m.n_frames_load == 2
-    det_fill_(m.netG0, seed=20)
-    det_fill_(m.netG1, seed=21)
-    cases.condition_flow_heads(m.netG0, 0.05)
-    cases.condition_flow_heads(m.netG1, 0.05)
-    orc = GO.ModelGOracle(opt, [m.netG0.state_dict(), m.netG1.state_dict()])
-    tG, T = opt.n_frames_G, 2 * 2 + opt.n_frames_G - 1
-    seq = synth_label_sequence(T, 32, 64, label_nc=5, block=4, seed=4)
-    g = torch.Generator().manual_seed(6)
-    real = torch.rand(1, T, 3, 32, 64, generator=g) * 2 - 1
-    prev_ref = prev_orc = None
+    opt = RI.train_opt(no_first_img)
+    nets = [det_fill_(NW.build_netG(opt, s), seed=20 + s) for s in range(2)]
+    for net in nets:
+        cases.condition_flow_heads(net, 0.05)
+    orc = GO.ModelGOracle(opt, [net.state_dict() for net in nets])
+    seq, real = RI.train_clip(opt)
+    prev = None
     for call in range(2):
-        sl = slice(call * 2, call * 2 + 2 + tG - 1)
+        prefix = 'train_forward/%d/%d' % (int(no_first_img), call)
         with torch.no_grad():
-            A, B = seq[:, sl].contiguous(), real[:, sl].contiguous()     # the data loader hands over contiguous clips
-            r = m.forward(A, B, A, prev_ref)
-            o = orc.train_forward(A, B, A, prev_orc, n_frames_load=2)
-        for name, a, b in zip(['fake_B', 'fake_B_raw', 'flow', 'weight', 'real_A', 'real_B'], r[:6], o[:6]):
-            assert (a is None) == (b is None), name
-            if a is not None:
-                assert a.shape == b.shape, (name, a.shape, b.shape)
-                _close(a, b)
-        assert r[0].shape == (1, 2, 3, 32, 64)
-        for a, b in zip(r[6], o[6]):
-            _close(a, b)
-        prev_ref, prev_orc = r[6], o[6]
+            A, B = RI.train_call_inputs(seq, real, opt, call)
+            o = orc.train_forward(A, B, A, prev, n_frames_load=2)
+        _close_all(prefix, RI.TRAIN_OUT_NAMES, o[:6])
+        assert o[0].shape == (1, 2, 3, 32, 64)
+        _close_all(prefix, ['prev_%d' % i for i in range(len(o[6]))], o[6])
+        prev = o[6]
 
 
 def test_oracle_gradients_match_reference():
@@ -150,29 +114,21 @@ def test_oracle_gradients_match_reference():
     reference for the backward kernels (dgrad / wgrad / norm / warp) of the training rows: for one scalar objective
     built from every output of the coarse generator, d/d(parameters), d/d(previous frames) and d/d(input) must agree
     with the gradients the reference module produces."""
-    N = ref_shim.networks()
     opt = make_opt(ngf=8, n_blocks=2, fg=True, n_downsample_G=2, gpu_ids=[])
-    net = det_fill_(N.define_G(18, 3, 6, 8, 'composite', 2, 'batch', 0, [], opt), seed=31)
+    net = det_fill_(NW.define_G(18, 3, 6, 8, 'composite', 2, 'batch', 0, [], opt), seed=31)
     cases.condition_flow_heads(net, 0.05)
-    inp, img_prev, mask = _inputs(6, 16, 32, seed=2)
-    g = torch.Generator().manual_seed(9)
-
-    def objective(outs, cot):
-        return sum((o * c).sum() for o, c in zip(outs, cot) if o is not None)
-
-    x_r, p_r = inp.clone().requires_grad_(True), img_prev.clone().requires_grad_(True)
-    ref = net(x_r, p_r, mask, None, None, None, False)
-    cot = [torch.randn(o.shape, generator=g) if o is not None else None for o in ref]
-    objective(ref, cot).backward()
-    ref_grads = {k: v.grad.clone() for k, v in net.named_parameters()}
-
-    sd = {k: v.detach().clone().requires_grad_(v.dtype.is_floating_point and k in ref_grads) for k, v in net.state_dict().items()}
+    inp, img_prev, mask = RI.gen_inputs(6, 16, 32, seed=2)
+    params = {k for k, _ in net.named_parameters()}
+    assert params == {k[len('grad/'):] for k in GOLD if k.startswith('grad/')} - {'input', 'img_prev'}
+    sd = {k: v.detach().clone().requires_grad_(v.dtype.is_floating_point and k in params) for k, v in net.state_dict().items()}
     x_o, p_o = inp.clone().requires_grad_(True), img_prev.clone().requires_grad_(True)
     out = GO.composite_generator(sd, x_o, p_o, mask, False, n_downsampling=2, n_blocks=2, use_fg_model=True)
-    objective(out, cot).backward()
-    for k, gr in ref_grads.items():
+    RI.objective(out, RI.cotangents(out)).backward()
+    for k in params:
+        gr = torch.from_numpy(GOLD['grad/' + k])
         scale = max(1.0, float(gr.abs().max()))
         assert sd[k].grad is not None, k
         assert float((sd[k].grad - gr).abs().max()) <= 2e-4 * scale, (k, float((sd[k].grad - gr).abs().max()), scale)
-    for a, b in ((x_o.grad, x_r.grad), (p_o.grad, p_r.grad)):
+    for a, key in ((x_o.grad, 'grad/input'), (p_o.grad, 'grad/img_prev')):
+        b = torch.from_numpy(GOLD[key])
         assert float((a - b).abs().max()) <= 2e-4 * max(1.0, float(b.abs().max()))

@@ -3,6 +3,7 @@ v2v_plan_profile).  Usage: python tools/profile_frame.py [workload] [out_prefix]
 import json
 import os
 import sys
+import tempfile
 
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), '..'))
 sys.path.insert(0, ROOT)
@@ -16,7 +17,7 @@ KINDS = {0: 'import', 1: 'conv', 2: 'rawstats', 3: 'finalize', 4: 'apply', 5: 'e
 
 def main():
     wl_name = sys.argv[1] if len(sys.argv) > 1 else 'cfg4'
-    prefix = sys.argv[2] if len(sys.argv) > 2 else os.path.join(ROOT, 'gpurun_out', 'profile_' + wl_name)
+    prefix = sys.argv[2] if len(sys.argv) > 2 else os.path.join(tempfile.gettempdir(), 'profile_' + wl_name)
     wl = bench.WORKLOADS[wl_name]
     opt = bench.make_opt_for(wl_name)
     torch.manual_seed(0)

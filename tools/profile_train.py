@@ -1,5 +1,5 @@
 """Kernel-time breakdown of one training step (torch.profiler / CUPTI): python tools/profile_train.py [workload] [out.txt]"""
-import os, sys
+import os, sys, tempfile
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), '..'))
 sys.path.insert(0, ROOT)
 import torch
@@ -11,7 +11,7 @@ from vid2vid_b200.trainer import Trainer
 from vid2vid_b200.utils import make_opt, synth_label_sequence
 
 wl_name = sys.argv[1] if len(sys.argv) > 1 else 'cfg3'
-out_path = sys.argv[2] if len(sys.argv) > 2 else os.path.join(ROOT, 'gpurun_out', 'profile_train_%s.txt' % wl_name)
+out_path = sys.argv[2] if len(sys.argv) > 2 else os.path.join(tempfile.gettempdir(), 'profile_train_%s.txt' % wl_name)
 wl = bench.WORKLOADS[wl_name]
 H, Wd = wl['H'], wl['W']
 opt = make_opt(label_nc=35, use_instance=True, fg=True, fg_labels=[26], n_scales_spatial=wl['n_scales'], ngf=wl['ngf'], num_D=3,

@@ -1,7 +1,5 @@
 """Times every HBM-bound stand-alone kernel of the hot path at its BASELINE-config size with CUDA events and reports achieved
-GB/s against its ALGORITHMIC bytes (SURVEY 8d) and the measured copy rate (MEASURED_PEAKS.json).  The same invocations are
-what profiles/r02_hbm_*.txt capture under ncu:  python tools/time_ops.py [op ...]"""
-import json
+GB/s against its ALGORITHMIC bytes (SURVEY 8d) and the H100 SXM data-sheet HBM3 bandwidth:  python tools/time_ops.py [op ...]"""
 import os
 import sys
 
@@ -13,11 +11,8 @@ from vid2vid_b200 import networks as NW       # noqa: E402
 from vid2vid_b200 import flownet as FN        # noqa: E402
 from vid2vid_b200.plan import Plan            # noqa: E402
 
-PEAK = 6570.9
-try:
-    PEAK = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs']
-except Exception:
-    pass
+import bench                                  # noqa: E402
+PEAK = bench.peaks()[1]
 dev = torch.device('cuda', 0)
 g = torch.Generator(device='cuda').manual_seed(0)
 rnd = lambda *s: torch.rand(*s, device=dev, generator=g)

@@ -1,6 +1,6 @@
 """ctypes binding of libv2v_b200.so (C ABI declared in include/v2v_b200.h).
 
-The library is built in-tree by vid2vid_b200/build.py (nvcc, sm_100a).  There is no CPU or
+The library is built in-tree by vid2vid_b200/build.py (nvcc, sm_90a).  There is no CPU or
 PyTorch fallback: if the shared object is missing or a call fails, a RuntimeError is raised.
 """
 import ctypes as C

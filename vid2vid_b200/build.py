@@ -1,4 +1,4 @@
-"""Builds libv2v_b200.so (sm_100a) in-tree with nvcc.  No GPU is needed to build."""
+"""Builds libv2v_b200.so (sm_90a, H100) in-tree with nvcc.  No GPU is needed to build."""
 import os
 import subprocess
 import sys
@@ -9,7 +9,7 @@ SOURCES = ['conv_umma.cu', 'conv_simt.cu', 'norm.cu', 'layout.cu', 'warp.cu', 'p
            'api.cu']
 LIB = os.path.join(HERE, 'libv2v_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
+FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
          '--expt-relaxed-constexpr', '-cudart', 'static']
 
 
@@ -40,7 +40,7 @@ def build(force=False, verbose=False):
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError('nvcc failed')
-    cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-cudart', 'static', '-gencode', 'arch=compute_100a,code=sm_100a']
+    cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-cudart', 'static', '-gencode', 'arch=compute_90a,code=sm_90a']
     subprocess.check_call(cmd)
     return LIB
 

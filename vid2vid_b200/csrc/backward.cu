@@ -1,7 +1,7 @@
 // Backward kernels of the training step (SURVEY 8 row T; reference: autograd through models/networks.py:203-232,296-325,
 // 663-725 as driven by train.py:50-93).  First correct CUDA path: fp32 SIMT, shared-memory tiled implicit GEMMs that read the
 // forward plan's own buffers (halo-padded NHWC activations, fp32 / bf16 raw conv outputs, saved batch statistics) and
-// dense NHWC fp32 gradient buffers.  The forward pass stays on the tcgen05 kernel.
+// dense NHWC fp32 gradient buffers.  The forward pass stays on the wgmma kernel.
 //   conv_dgrad   dXpad[n][py][px][ci] = sum_{taps, co} dY[n][oy][ox][co] * W      (padded input extent; reflect / zero halo
 //                                                                                   folded back by fold_pad_kernel)
 //   conv_wgrad   dW[co][ci][ky][kx]  += sum_{n, oy, ox} dY[n][oy][ox][co] * Xpad[n][oy*s+ky][ox*s+kx][ci]   (split over pixels)
@@ -492,7 +492,7 @@ __global__ void convact_bwd_kernel(const float* __restrict__ dy, ActDesc out, in
 
 static inline int grid1d(size_t total) {
   size_t b = (total + 255) / 256;
-  const size_t cap = 148 * 16;
+  const size_t cap = 132 * 16;
   return (int)(b < cap ? (b ? b : 1) : cap);
 }
 
@@ -507,7 +507,7 @@ cudaError_t launch_conv_bwd(const BwdConv& p, cudaStream_t s) {
     const int gh = p.transposed ? p.H : p.oh, gw = p.transposed ? p.W : p.ow;
     const long long npix = (long long)p.N * gh * gw;
     const int tiles = ((p.Cin + 31) / 32) * ((p.Cout + 31) / 32), taps = p.kh * p.kw;
-    long long ks = (148LL * 8 + (long long)tiles * taps - 1) / ((long long)tiles * taps);
+    long long ks = (132LL * 8 + (long long)tiles * taps - 1) / ((long long)tiles * taps);
     ks = std::max(1LL, std::min(ks, (npix + 255) / 256));
     dim3 grid(tiles, taps, (unsigned)ks);
     conv_wgrad_kernel<<<grid, 256, 0, s>>>(p, (int)ks);
@@ -533,7 +533,7 @@ cudaError_t launch_norm_bwd(const NormBwd& p, cudaStream_t s) {
     const long long HW = (long long)p.H * p.W;
     if (p.C % 4 == 0 && p.C <= 1024 && p.raw.C % 4 == 0 && p.c_off % 4 == 0) {
       const int ppb = 256 / (p.C / 4);
-      const long long want_blocks = std::max(1LL, (4LL * 148) / p.N);
+      const long long want_blocks = std::max(1LL, (4LL * 132) / p.N);
       long long chunk = std::max<long long>((long long)ppb * 8, (HW + want_blocks - 1) / want_blocks);
       dim3 grid((unsigned)((HW + chunk - 1) / chunk), p.N);
       norm_bwd_reduce_vec_kernel<<<grid, 256, 2 * p.C * sizeof(float), s>>>(p, (int)chunk);

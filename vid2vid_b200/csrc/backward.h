@@ -56,11 +56,10 @@ struct WgradParams {
   int swap;                    // 0: A (M side) = OUT, B (N side) = IN;  1: A = IN, B = OUT (narrow gradient tensors)
   int a_C, b_C;                // padded channel counts of the A / B tensors: the lo half starts at channel coordinate C
   int Mblocks, Nblocks;        // A: 64-channel blocks per M tile (2, or 1 for a 64-channel tensor); B: blocks per N tile
-  int b_row, BN;               // B: bytes per pixel row of one block (128 / 64 / 32) and channels per N tile (16 .. 128)
+  int b_row, BN;               // B: bytes per pixel row of one block (128 / 64 / 32) and channels per N tile (16 / 32 / 64 / 128)
   int m_tiles, n_tiles, ntaps, ksplit;
   int chunks_total, chunks_per_unit;
   int split;                   // 1: [hi | lo] operands, three MMAs per K step
-  int kxr;                     // taps per unit that share one IN patch (kw for stride-1 filters, else 1)
   int stages;
   WgradTap taps[V2V_MAX_TAPS];
   float* stage;                // [ntaps][Mp][Np] fp32, zeroed by the launcher

@@ -1,4 +1,4 @@
-// Plain SIMT (CUDA-core, fp32-accumulate) evaluation of the same convolution plan the tcgen05 kernel
+// Plain SIMT (CUDA-core, fp32-accumulate) evaluation of the same convolution plan the wgmma kernel
 // runs: same halo-padded NHWC bf16 input, same packed bf16 weights, same tap groups, same epilogues.
 // It exists to cross-check the tensor-core kernel on the device (tests, V2V_CONV_IMPL=simt) -- it is a
 // CUDA kernel, not a CPU fallback, and is never selected by default.
@@ -71,7 +71,7 @@ __global__ void conv_simt_kernel(ActDesc in, const bf16* __restrict__ w, int Kto
 }
 
 // Per-channel (sum, sumsq) of a raw NHWC bf16 tensor, one partial row per image:
-// stats[(n*2 + {0,1}) * C + c].  Used with the SIMT conv (the tcgen05 epilogue produces these itself).
+// stats[(n*2 + {0,1}) * C + c].  Used with the SIMT conv (the wgmma kernel's epilogue produces these itself).
 __global__ void raw_stats_kernel(const void* __restrict__ raw_, int f32, int HW, int C, int Cs, stat_t* __restrict__ stats) {
   const int n = blockIdx.y, c = blockIdx.x;
   float s = 0.f, q = 0.f;
@@ -97,7 +97,7 @@ cudaError_t launch_conv_simt(const ActDesc& in, const bf16* wpacked, int Ktotal,
                              cudaStream_t stream) {
   const long long total = (long long)p.num_phases * p.N * p.grid_h * p.grid_w * p.Cout;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   conv_simt_kernel<<<blocks, 256, 0, stream>>>(in, wpacked, Ktotal, p);
   return cudaGetLastError();
 }

@@ -1,10 +1,10 @@
-// Implicit-GEMM convolution on tcgen05 tensor cores (sm_100a), persistent and warp-specialised.
+// Implicit-GEMM convolution on Hopper tensor cores (sm_90a wgmma), persistent and warp-specialised.
 //
-//   D[128 pixels x BN channels] (fp32, TMEM) = sum over (tap, K block of kc = 16/32/64 channels) A[128 x kc] * B[BN x kc]^T
+//   D[128 pixels x BN channels] (fp32, registers) = sum over (tap, K block of kc = 16/32/64 channels) A[128 x kc] * B[BN x kc]^T
 //
 // A tiles are boxes of the halo-padded NHWC bf16 activation buffer fetched by TMA (5-D tiled map,
 // 128-byte swizzle): a box of TH x TW pixels x 64 channels lands in shared memory as 128 rows of
-// 128 bytes -- exactly the K-major SWIZZLE_128B operand layout tcgen05.mma reads.  That box *is*
+// 128 bytes -- exactly the K-major SWIZZLE_128B operand layout wgmma reads.  That box *is*
 // the im2col slice for one filter tap; for stride-1 filters on row tiles (TH == 1) one box of
 // TW + R - 1 pixels serves R horizontally adjacent taps, each tap's operand being the same smem
 // patch with its start address advanced by one 128-byte row.  B tiles come from the packed weight
@@ -14,31 +14,29 @@
 // models/networks.py:132-183,247-279,571,586,685-706.
 //
 // One CTA per SM walks tiles t = blockIdx.x, += gridDim.x (M fastest, so co-running CTAs share weights in L2).
-//   warp 0        TMA producer (one elected lane)
-//   warp 1        tcgen05.mma issuer (whole warp loops, one elected lane issues) + TMEM owner
-//   warps 2..     epilogue groups of 4 warps: tcgen05.ld the accumulator.  EG = 1: one group drains both TMEM stages;
-//                 EG = 2/3: group h owns stage h, so EG tiles drain concurrently while the next one accumulates (the
-//                 epilogue, with one warp per SM sub-partition, is latency bound and the critical path of small-K layers)
-//     EPI_RAW_STATS : bf16 NHWC raw output + per-tile per-channel (sum, sumsq) partials for the following
-//                     Batch/InstanceNorm (deterministic: no atomics)
+//   warps 0-7   two consumer warpgroups: warpgroup h issues the m64nBNk16 wgmmas of rows [64 h, 64 h + 64) of every M tile
+//               (MG tiles side by side, accumulators in registers), keeping one commit group in flight and handing each
+//               operand slot back to the producer as soon as the MMAs that read it have retired.  Both then drain the
+//               accumulators through a 128 x 64 fp32 shared-memory staging tile, so that in the epilogue thread
+//               (warp q = 0..3, lane) owns pixel row 32 q + lane and warps q / q + 4 take alternate 32-channel chunks:
+//     EPI_RAW_STATS : bf16 NHWC raw output + per-channel (sum, sumsq) of the tile for the following
+//                     Batch/InstanceNorm (deterministic fixed-point atomics)
 //     EPI_HEAD_F32  : bias + tanh/sigmoid/scale -> fp32 NCHW planes (the 7x7 image/flow/weight heads)
 //     EPI_ACT_BF16  : bias + (leaky)ReLU -> interior of the next layer's padded NHWC buffer
+//   warp 8      TMA producer (one elected lane)
 #include <cstdlib>
 #include "ptx.cuh"
+#include "wgmma.cuh"
 #include "v2v_internal.h"
 #include "finalize.cuh"
 
 namespace v2v {
 
-static constexpr int kMaxGroups = 2;                      // epilogue groups of 4 warps (one TMEM lane quarter each)
-static constexpr int kMaxThreads = 64 + 128 * kMaxGroups;
-static constexpr int kEpiThreads = 128;
-// per epilogue group: [warp][sum|sumsq][128 columns] running column sums; per epilogue warp: a 32 x 17 transpose tile
-static constexpr int kRedFloatsPerGroup = 4 * 2 * 128 + 4 * 32 * 17;
-
-// V2V_DBG bit2: CTA 0 records clock64() at role events of its first 24 work units and prints them at exit
-__device__ long long g_trace[3][24][8];
-#define TRACE(role, it, ev) do { if ((p.dbg & 4) && blockIdx.x == 0 && (it) < 24) g_trace[role][it][ev] = clock64(); } while (0)
+static constexpr int kConsumerThreads = 256;              // two warpgroups
+static constexpr int kThreads = kConsumerThreads + 32;    // + the producer warp
+static constexpr int kStgStride = 65;                     // floats per staging row: row-wise and column-wise walks are conflict free
+static constexpr int kStgFloats = 128 * kStgStride;       // 128 pixel rows x 64 accumulator columns
+static constexpr int kRedFloats = 4 * 2 * 128;            // [warp quarter][sum|sumsq][128 columns] running column sums
 
 __device__ __forceinline__ float apply_act(float v, int act, float slope) {
   switch (act) {
@@ -48,22 +46,6 @@ __device__ __forceinline__ float apply_act(float v, int act, float slope) {
     case ACT_SIGMOID: return 1.f / (1.f + __expf(-v));
     default: return v;
   }
-}
-
-// Sum the 32 per-lane vectors v[0..31] over the 32 lanes; lane l ends up with the total of element l.
-// 31 shuffles instead of 160 (recursive halving).
-__device__ __forceinline__ float warp_transpose_reduce(float (&v)[32], int lane) {
-#pragma unroll
-  for (int s = 16; s >= 1; s >>= 1) {
-    const bool upper = (lane & s) != 0;
-#pragma unroll
-    for (int j = 0; j < s; ++j) {
-      float send = upper ? v[j] : v[j + s];
-      float keep = upper ? v[j + s] : v[j];
-      v[j] = keep + __shfl_xor_sync(0xffffffffu, send, s);
-    }
-  }
-  return v[0];
 }
 
 // kx-GEMM heads: acc[j] = sum_kx (value of accumulator column kx * COUT + j held by lane + kx)
@@ -84,10 +66,9 @@ __device__ __forceinline__ void head_shift_sum(const uint32_t (&r)[32], int kw, 
 }
 
 // Work units (MG consecutive M tiles of one tile row, of one (phase, N tile) "key"; M fastest) are walked by every role as u = first, first + step, ...
-// Integer division is ~150 cycles of dependent SASS on one thread, and the single MMA-issuing thread used to spend
-// ~1000 cycles per tile decoding u (measured with the V2V_DBG traces: a 1000-cycle bubble between tiles of 2100 cycles
-// of MMAs).  The iterator therefore keeps (key, N tile, phase, image, tile row, tile column) as a mixed-radix number and
-// advances it by the pre-split step with carries: divisions happen once per kernel.
+// The iterator keeps (key, N tile, phase, image, tile row, tile column) as a mixed-radix number and advances it by the
+// pre-split step with carries, so the integer divisions (~150 cycles of dependent SASS each) happen once per kernel
+// instead of once per unit on the issuing threads.
 struct UnitIter {
   int u, key, nt, phase, img, ty, txi;
   int s_img, s_ty, s_tx, step;
@@ -119,198 +100,27 @@ struct UnitIter {
   __device__ __forceinline__ int y0(const ConvKernelParams& p) const { return ty * p.TH; }
 };
 
-struct MmaCtx {
-  uint8_t* sG; uint8_t* sBres;
-  uint64_t *g_full, *g_empty, *bres_full, *bres_empty, *tmem_full, *tmem_empty, *b_full, *b_empty;
-  uint32_t tmem_base, acc_cols;
-  int group_bytes, b_tx, NS, t_first, t_step;
-};
 
-
-template <bool kWarpWide, int KMMA>
-__device__ __forceinline__ void issue_taps(const ConvKernelParams& p, uint32_t tmem_d, uint32_t al, uint32_t bl, uint32_t a_hi,
-                                           uint32_t b_hi, uint32_t idesc, uint32_t first, uint32_t a_step, uint32_t b_step,
-                                           uint32_t a_wrap) {
-  const int RW = p.RW;
-  for (int r0 = 0; r0 < p.R; r0 += RW, al += a_wrap) {
-    for (int r = 0; r < RW; ++r, al += a_step, bl += b_step) {
-      if (kWarpWide ? elect_one_sync() : true) {
-        const uint64_t ad = ((uint64_t)a_hi << 32) | al, bd = ((uint64_t)b_hi << 32) | bl;
-        umma_bf16(tmem_d, ad, bd, idesc, first);
-        if (KMMA >= 2) umma_bf16(tmem_d, ad + 2, bd + 2, idesc, 1u);
-        if (KMMA >= 4) {
-          umma_bf16(tmem_d, ad + 4, bd + 4, idesc, 1u);
-          umma_bf16(tmem_d, ad + 6, bd + 6, idesc, 1u);
-        }
+// All MMAs of one (tap, K block) for the MG accumulators: KMMA K=16 steps x the operand passes of the arithmetic mode
+// (precise plans: A_hi*B_hi + A_lo*B_hi + A_hi*B_lo, the lo halves a_half / b_half bytes further in the same slots).
+template <int BN, int MG>
+__device__ __forceinline__ void mma_tap(float (&acc)[MG][BN / 2], uint64_t ad, uint64_t bd, uint32_t a_tile16, int kmma, int ps_step,
+                                        uint32_t a_half16, uint32_t b_half16, uint32_t first) {
+#pragma unroll
+  for (int j = 0; j < MG; ++j) {
+    uint32_t f = first;
+    for (int ps = 0; ps < 3; ps += ps_step) {
+      const uint64_t a = ad + (uint64_t)j * a_tile16 + (ps == 1 ? a_half16 : 0u), b = bd + (ps == 2 ? b_half16 : 0u);
+      for (int k = 0; k < kmma; ++k) {
+        Wgmma<BN>::template mma<0, 0>(acc[j], a + 2 * k, b + 2 * k, f);      // +32 bytes along K per MMA
+        f = 1u;
       }
-      first = 1u;
     }
   }
 }
 
-// One (tap, K block) of MMAs for one accumulator: KMMA K=16 steps x the operand passes of the arithmetic mode.
-template <int KMMA>
-__device__ __forceinline__ void issue_tap(uint32_t tmem_d, uint32_t al, uint32_t bl, uint32_t a_hi, uint32_t b_hi, uint32_t idesc,
-                                          uint32_t& first, int ps_step, uint32_t a_half16, uint32_t b_half16) {
-  for (int ps = 0; ps < 3; ps += ps_step) {
-    const uint64_t ad = ((uint64_t)a_hi << 32) | (al + (ps == 1 ? a_half16 : 0u)), bd = ((uint64_t)b_hi << 32) | (bl + (ps == 2 ? b_half16 : 0u));
-    umma_bf16(tmem_d, ad, bd, idesc, first);
-    if (KMMA >= 2) umma_bf16(tmem_d, ad + 2, bd + 2, idesc, 1u);
-    if (KMMA >= 4) {
-      umma_bf16(tmem_d, ad + 4, bd + 4, idesc, 1u);
-      umma_bf16(tmem_d, ad + 6, bd + 6, idesc, 1u);
-    }
-    first = 1u;
-  }
-}
-
-// ring2 issue loop (one elected lane).  K loop of a unit: steps (tap group, K block); per step ONE patch slot (MG tiles) from
-// the A ring and ceil(R / TB) weight chunks from the B ring; tap r of the step reads the patch advanced by
-// (r / RW) * PW + (r % RW) rows.
-template <int KMMA>
-__device__ __forceinline__ void mma_role_ring2(const ConvKernelParams& p, const MmaCtx& cx) {
-  const uint32_t idesc = make_idesc_bf16(128, p.BN);
-  const int ps_step = p.split ? (p.a_exact ? 2 : 1) : 3;
-  const uint32_t a_half16 = (uint32_t)(p.a_half_bytes >> 4), b_half16 = (uint32_t)(p.b_half_bytes >> 4);
-  const uint32_t a_hi = (uint32_t)(make_kmajor_desc(0, p.sbo_a_bytes, p.layout_type) >> 32);
-  const uint32_t b_hi = (uint32_t)(make_kmajor_desc(0, p.sbo_bytes, p.layout_type) >> 32);
-  const uint32_t a_lo0 = (uint32_t)make_kmajor_desc(0, p.sbo_a_bytes, p.layout_type);
-  const uint32_t b_lo0 = (uint32_t)make_kmajor_desc(0, p.sbo_bytes, p.layout_type);
-  const uint32_t row16 = (uint32_t)(p.row_bytes >> 4), prow16 = (uint32_t)((p.PW * p.row_bytes) >> 4), btap16 = (uint32_t)(cx.b_tx >> 4);
-  const uint32_t sB_u32 = smem_u32(cx.sBres);
-  int as = 0, bs = 0, acc = 0, it = 0;
-  uint32_t apar = 0, bpar = 0, accpar = 0;
-  const int RH = p.R / p.RW;                              // patch rows of taps
-  UnitIter un;
-  un.init(p, cx.t_first, cx.t_step);
-  for (; un.valid(p); ++it) {
-    const ConvPhase ph = p.phases[un.phase];
-    un.next(p);
-    const int nsteps = (ph.group_end - ph.group_begin) * p.cblocks;
-    mbar_wait(&cx.tmem_empty[acc], accpar ^ 1);
-    tcgen05_fence_after();
-    const uint32_t tmem_d0 = cx.tmem_base + acc * p.MG * cx.acc_cols;
-    uint32_t first = 0;
-    for (int st = 0; st < nsteps; ++st) {
-      mbar_wait(&cx.g_full[as], apar);
-      tcgen05_fence_after();
-      const uint32_t a_base16 = a_lo0 + ((smem_u32(cx.sG + (size_t)as * p.MG * p.a_slot_bytes) & 0x3FFFF) >> 4);
-      uint32_t first_step = first;
-      uint32_t bchunk16 = 0;
-      int tin = 0, r = 0;                                       // tap index inside the current weight chunk / inside the step
-      for (int ky = 0; ky < RH; ++ky) {
-        for (int kx = 0; kx < p.RW; ++kx, ++r) {
-          if (tin == 0) {
-            mbar_wait(&cx.b_full[bs], bpar);
-            tcgen05_fence_after();
-            bchunk16 = b_lo0 + (((sB_u32 + (uint32_t)bs * (uint32_t)p.b_slot_bytes) & 0x3FFFF) >> 4);
-          }
-          const uint32_t al0 = a_base16 + (uint32_t)ky * prow16 + (uint32_t)kx * row16, bl = bchunk16 + (uint32_t)tin * btap16;
-          for (int j = 0; j < p.MG; ++j) {
-            uint32_t f = first_step;
-            issue_tap<KMMA>(tmem_d0 + j * cx.acc_cols, al0 + (uint32_t)j * (uint32_t)(p.a_slot_bytes >> 4), bl, a_hi, b_hi, idesc, f, ps_step,
-                            a_half16, b_half16);
-          }
-          first_step = 1u;
-          if (++tin == p.TB || r == p.R - 1) {                      // chunks hold TB taps; the last one of a step may be short
-            tin = 0;
-            umma_commit(&cx.b_empty[bs]);                          // this weight chunk is free when the MMAs above retire
-            if (++bs == p.SBr) { bs = 0; bpar ^= 1; }
-          }
-        }
-      }
-      first = 1u;
-      umma_commit(&cx.g_empty[as]);                                // ... and so is the patch slot
-      if (++as == p.SG) { as = 0; apar ^= 1; }
-    }
-    umma_commit(&cx.tmem_full[acc]);                               // accumulator(s) complete
-    if (++acc == cx.NS) { acc = 0; accpar ^= 1; }
-  }
-}
-
-// The tcgen05.mma issue loop.  kWarpWide = false: called by ONE elected lane, which runs the whole loop (no re-election
-// or warp synchronisation on the issue path; descriptors live in vector registers and are moved to uniform registers
-// per MMA).  kWarpWide = true: all 32 lanes walk the loop in lock step, so ptxas can keep the descriptor arithmetic on
-// the uniform datapath, and elect.sync guards each group of MMAs / each commit.
-template <bool kWarpWide>
-__device__ __forceinline__ void mma_role(const ConvKernelParams& p, const MmaCtx& cx) {
-  const uint32_t idesc = make_idesc_bf16(128, p.BN);
-  int gs = 0, it = 0, as = 0;
-  uint32_t gpar = 0, gen = 0, aphase = 0;
-  int prev_key = -1;
-  // tap r of a patch: next pixel (horizontal reuse) or, for kx-GEMM heads, next patch ROW (TW pixels further)
-  const uint32_t a_step = (uint32_t)(((p.headkx ? p.TW : 1) * p.row_bytes) >> 4), b_step = (uint32_t)(cx.b_tx >> 4);
-  const uint32_t a_wrap = (uint32_t)(((p.PW - p.RW) * p.row_bytes) >> 4);     // to the next patch row
-  const uint32_t sBres_u32 = smem_u32(cx.sBres);
-  const int ps_step = p.split ? (p.a_exact ? 2 : 1) : 3;
-  const uint32_t a_half16 = (uint32_t)(p.a_half_bytes >> 4), b_half16 = (uint32_t)(p.b_half_bytes >> 4);
-  // descriptors differ only in the 14-bit (address >> 4) field of the low word
-  const uint32_t a_hi = (uint32_t)(make_kmajor_desc(0, p.sbo_a_bytes, p.layout_type) >> 32);
-  const uint32_t b_hi = (uint32_t)(make_kmajor_desc(0, p.sbo_bytes, p.layout_type) >> 32);
-  const uint32_t a_lo0 = (uint32_t)make_kmajor_desc(0, p.sbo_a_bytes, p.layout_type);
-  const uint32_t b_lo0 = (uint32_t)make_kmajor_desc(0, p.sbo_bytes, p.layout_type);
-  UnitIter un;
-  un.init(p, cx.t_first, cx.t_step);
-  for (; un.valid(p); ++it) {
-    const ConvPhase ph = p.phases[un.phase];
-    const int key = un.key;
-    const bool first_of_key = key != prev_key;
-    if (p.b_resident && first_of_key && prev_key >= 0) gen ^= 1;
-    prev_key = key;
-    un.next(p);                                          // (everything below uses the values captured above)
-    const bool last_of_key = !un.valid(p) || un.key != key;
-    const int nsteps = (ph.group_end - ph.group_begin) * p.cblocks;
-    TRACE(1, it, 0);
-    mbar_wait(&cx.tmem_empty[as], aphase ^ 1);        // the epilogue has drained this accumulator stage
-    if (p.b_resident && first_of_key) mbar_wait(cx.bres_full, gen);
-    tcgen05_fence_after();
-    TRACE(1, it, 1);
-    const uint32_t tmem_d0 = cx.tmem_base + as * p.MG * cx.acc_cols;
-    for (int s0 = 0; s0 < nsteps; s0 += p.CG) {
-      const int n = min(p.CG, nsteps - s0);
-      mbar_wait(&cx.g_full[gs], gpar);
-      tcgen05_fence_after();
-      if (s0 == 0) TRACE(1, it, 2);
-      const uint32_t base = smem_u32(cx.sG + (size_t)gs * cx.group_bytes);
-      for (int i = 0; i < n; ++i) {
-        const uint32_t b_base = p.b_resident ? sBres_u32 + (s0 + i) * p.b_slot_bytes
-                                             : base + p.CG * p.MG * p.a_slot_bytes + i * p.b_slot_bytes;
-        const uint32_t bl0 = b_lo0 + ((b_base & 0x3FFFF) >> 4);
-        // MG accumulators side by side: every weight tile fetched from L2 is used for MG M tiles
-        for (int j = 0; j < p.MG; ++j) {
-          const uint32_t a_base = base + (i * p.MG + j) * p.a_slot_bytes;
-          const uint32_t tmem_d = tmem_d0 + j * cx.acc_cols;
-          uint32_t first = (s0 + i) > 0 ? 1u : 0u;
-          uint32_t al = a_lo0 + ((a_base & 0x3FFFF) >> 4), bl = bl0;
-          // tap r reads the patch shifted by (r / RW) patch rows and (r % RW) pixels; K = 16 bf16 = 32 bytes per MMA,
-          // kc/16 MMAs per smem row.  The trip-count switch sits outside the tap loops: the issuing thread has ~40
-          // cycles per MMA for small-N layers, every instruction in the loop body counts.
-          // precise plans: npass = 3 accumulates A_hi*B_hi + A_lo*B_hi + A_hi*B_lo (the lo halves sit a_half / b_half
-          // bytes further in the same slots)
-          for (int ps = 0; ps < 3; ps += ps_step) {          // ps_step: 3 = one pass (fast), 1 = three passes, 2 = {hi*hi, hi*lo}
-            const uint32_t alp = al + (ps == 1 ? a_half16 : 0u), blp = bl + (ps == 2 ? b_half16 : 0u);
-            if (p.kmma == 4) issue_taps<kWarpWide, 4>(p, tmem_d, alp, blp, a_hi, b_hi, idesc, first, a_step, b_step, a_wrap);
-            else if (p.kmma == 2) issue_taps<kWarpWide, 2>(p, tmem_d, alp, blp, a_hi, b_hi, idesc, first, a_step, b_step, a_wrap);
-            else issue_taps<kWarpWide, 1>(p, tmem_d, alp, blp, a_hi, b_hi, idesc, first, a_step, b_step, a_wrap);
-            first = 1u;
-          }
-        }
-      }
-      if (kWarpWide ? elect_one_sync() : true) {
-        umma_commit(&cx.g_empty[gs]);                   // the whole group slot is free when these MMAs retire
-        if (s0 + n >= nsteps) {
-          if (p.b_resident && last_of_key) umma_commit(cx.bres_empty);
-          umma_commit(&cx.tmem_full[as]);               // accumulator complete
-        }
-      }
-      if (++gs == p.SG) { gs = 0; gpar ^= 1; }
-    }
-    TRACE(1, it, 3);
-    if (++as == cx.NS) { as = 0; aphase ^= 1; }
-  }
-}
-
-__global__ void __launch_bounds__(kMaxThreads, 1)
+template <int BN, int MG>
+__global__ void __launch_bounds__(kThreads, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ ConvKernelParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -321,53 +131,41 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int group_bytes = p.CG * (p.MG * p.a_slot_bytes + slot_b);
   uint8_t* sG = smem;
   uint8_t* sBres = sG + (size_t)p.SG * group_bytes;
-  float* red = reinterpret_cast<float*>(sBres + (p.ring2 ? (size_t)p.SBr * p.b_slot_bytes : (p.b_resident ? (size_t)p.SB * p.b_slot_bytes : 0)));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(red + p.EG * kRedFloatsPerGroup);
+  float* stg = reinterpret_cast<float*>(sBres + (p.ring2 ? (size_t)p.SBr * p.b_slot_bytes : (p.b_resident ? (size_t)p.SB * p.b_slot_bytes : 0)));
+  float* racc = stg + kStgFloats;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(racc + kRedFloats);
   uint64_t* g_full = bars;
   uint64_t* g_empty = g_full + p.SG;
   uint64_t* bres_full = g_empty + p.SG;
   uint64_t* bres_empty = bres_full + 1;
-  uint64_t* tmem_full = bres_empty + 1;     // [kMaxGroups]
-  uint64_t* tmem_empty = tmem_full + kMaxGroups;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + kMaxGroups);
-  uint64_t* b_full = reinterpret_cast<uint64_t*>(tmem_slot + 2);       // ring2: weight ring barriers [8] + [8]
+  uint64_t* b_full = bres_empty + 1;        // ring2: weight ring barriers [8] + [8]
   uint64_t* b_empty = b_full + 8;
-  const int NS = p.EG > 1 ? p.EG : 2;       // accumulator stages in TMEM
+  uint32_t* ticket = reinterpret_cast<uint32_t*>(b_empty + 8);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t acc_cols = p.BN < 32 ? 32 : p.BN;     // columns per accumulator stage
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < NS * p.MG * acc_cols) tmem_cols <<= 1;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // (warp-uniform to the compiler)
+  const int n_consumer_warps = kConsumerThreads / 32;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int i = 0; i < p.SG; ++i) { mbar_init(&g_full[i], 1); mbar_init(&g_empty[i], 1); }
-    mbar_init(bres_full, 1); mbar_init(bres_empty, 1);
-    if (p.ring2) for (int i = 0; i < p.SBr; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < NS; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 4); }
+    for (int i = 0; i < p.SG; ++i) { mbar_init(&g_full[i], 1); mbar_init(&g_empty[i], n_consumer_warps); }
+    mbar_init(bres_full, 1); mbar_init(bres_empty, n_consumer_warps);
+    if (p.ring2) for (int i = 0; i < p.SBr; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], n_consumer_warps); }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, tmem_cols);
-    tmem_relinquish();
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_prologue();          // everything above overlaps the previous kernel's tail; nothing above touches global memory
 
   const int a_tx = p.PW * p.PH * p.row_bytes;
   const int b_tx = p.BN * p.row_bytes;
   const int t_first = blockIdx.x, t_step = gridDim.x;
 
-  if (warp == 0) {
+  if (warp == n_consumer_warps) {
     if (elect_one_sync()) {
       // ---------------------------------------------------------- TMA producer (single elected lane)
       // The K loop of a tile is a sequence of steps (tap group g, K block cb); CG consecutive steps share one
-      // full/empty barrier pair ("group slot"), so a barrier round trip and a tcgen05.commit are paid once per CG
-      // steps (measured: ~500 cycles of issue-side overhead per commit group, during which the tensor pipe idles).
+      // full/empty barrier pair ("group slot"), so a barrier round trip and a wgmma commit group are paid once per CG
+      // steps.
       int gs = 0;
       uint32_t gpar = 0, gen = 0;
       int prev_key = -1;
@@ -407,8 +205,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
         }
       } else
-      for (int pit = 0; un.valid(p); un.next(p), ++pit) {
-        TRACE(0, pit, 0);
+      for (; un.valid(p); un.next(p)) {
         const ConvPhase ph = p.phases[un.phase];
         const int x0 = un.x0(p), y0 = un.y0(p), n0 = un.n0(p);
         const int nsteps = (ph.group_end - ph.group_begin) * p.cblocks;
@@ -448,78 +245,180 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
           if (++gs == p.SG) { gs = 0; gpar ^= 1; }
         }
-        TRACE(0, pit, 2);
       }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer
-    MmaCtx cx{sG, sBres, g_full, g_empty, bres_full, bres_empty, tmem_full, tmem_empty, b_full, b_empty, tmem_base, acc_cols,
-              group_bytes, b_tx, NS, t_first, t_step};
-    if (p.ring2) {
-      if (elect_one_sync()) {
-        if (p.kmma == 4) mma_role_ring2<4>(p, cx);
-        else if (p.kmma == 2) mma_role_ring2<2>(p, cx);
-        else mma_role_ring2<1>(p, cx);
-      }
-    } else if (p.dbg & 8) {
-      mma_role<true>(p, cx);                   // whole warp walks the loop (uniform datapath), elect.sync per MMA group
-    } else if (elect_one_sync()) {
-      mma_role<false>(p, cx);                  // one elected lane runs the whole loop
     }
   } else {
-    // ------------------------------------------------------------ epilogue warps (TMEM lane quarter = warp % 4)
-    const int q = warp & 3;
-    const int eg = (warp - 2) >> 2;                       // epilogue group
-    const int etid = q * 32 + lane;
-    // running (sum, sumsq) of this warp's rows, per column of the current N tile, in shared memory; the group's four
-    // warps are combined and flushed to the (phase, image, CTA) partial row only when (phase, N tile, image) changes.
-    // Every partial row element receives at most one addend per group onto a zeroed row, and EG <= 2 when statistics
-    // are on, so the atomic adds are order independent (deterministic).
-    float* racc = red + eg * (4 * 2 * 128);
-    float* tt = red + p.EG * (4 * 2 * 128) + (eg * 4 + q) * (32 * 17);
+    // ------------------------------------------------------------ consumers: wgmma issue + epilogue
+    const int wg = warp >> 2;                             // M half of the tile this warpgroup multiplies
+    const int q = warp & 3, hc = wg;                      // epilogue: pixel rows 32 q .. 32 q + 31, chunk parity hc
+    const int row = q * 32 + lane;
+    const int ps_step = p.split ? (p.a_exact ? 2 : 1) : 3;    // 3 = one pass (fast), 1 = three passes, 2 = {hi*hi, hi*lo}
+    const uint32_t a_half16 = (uint32_t)(p.a_half_bytes >> 4), b_half16 = (uint32_t)(p.b_half_bytes >> 4);
+    const uint32_t a_tile16 = (uint32_t)(p.a_slot_bytes >> 4);
+    // rows 64.. of an M tile are eight 8-row core-matrix groups further on
+    const uint64_t a_d0 = make_kmajor_desc(0, p.sbo_a_bytes, p.layout_type) + (uint64_t)((wg * 8 * p.sbo_a_bytes) >> 4);
+    const uint64_t b_d0 = make_kmajor_desc(0, p.sbo_bytes, p.layout_type);
+    // tap r of a patch: next pixel (horizontal reuse) or, for kx-GEMM heads, next patch ROW (TW pixels further)
+    const uint32_t a_step = (uint32_t)(((p.headkx ? p.TW : 1) * p.row_bytes) >> 4), b_step = (uint32_t)(b_tx >> 4);
+    const uint32_t a_wrap = (uint32_t)(((p.PW - p.RW) * p.row_bytes) >> 4);     // to the next patch row
+    const uint32_t row16 = (uint32_t)(p.row_bytes >> 4), prow16 = (uint32_t)((p.PW * p.row_bytes) >> 4);
+    const uint32_t sB_u32 = smem_u32(sBres);
     const bool do_stats = (p.epi == EPI_RAW_STATS) && (p.stats != nullptr) && !(p.dbg & 1);
-    int acc_key = -1, acc_img = -1, acc_n0 = 0, acc_phase = 0;
     const int nchunks = p.BN / 32;
+    const int tw_shift = __ffs(p.TW) - 1;                 // TW is a power of two
+    const int ry = row >> tw_shift, rx = row & (p.TW - 1);
+
+    float acc[MG][BN / 2];
+    // Operand slots retire one commit group late: after committing group k the warpgroup waits for group k - 1 only, so
+    // the tensor core always has the next group queued.  Each warp then arrives once on the slot barriers (count 8).
+    int pend_g = -1, pend_b = -1;
+    auto retire = [&](int g, int b) {
+      __syncwarp();
+      mbar_arrive_if(&g_empty[g < 0 ? 0 : g], lane == 0 && g >= 0);
+      mbar_arrive_if(&b_empty[b < 0 ? 0 : b], lane == 0 && b >= 0);
+    };
+    auto commit_and_retire_previous = [&](int g, int b) {
+      wgmma_commit();
+      wgmma_wait<1>();
+      retire(pend_g, pend_b);
+      pend_g = g; pend_b = b;
+    };
+    auto drain = [&]() {
+      wgmma_wait<0>();
+      retire(pend_g, pend_b);
+      pend_g = pend_b = -1;
+#pragma unroll
+      for (int j = 0; j < MG; ++j) wgmma_fence_operands(acc[j]);
+    };
+    // Statistics: running (sum, sumsq) per (warp quarter, column of the current N tile) in shared memory, flushed onto the
+    // image's statistics row when (phase, N tile, image) changes.  Every (quarter, column) has one writer warp.
+    int acc_key = -1, acc_img = -1, acc_n0 = 0;
+    // flush() publishes the running sums and zeroes them again: thread c owns column c of every quarter.
     auto flush = [&]() {
-      named_bar_sync(1 + eg, kEpiThreads);                // all four warps have added their last tile
-      if (etid < p.BN && acc_n0 + etid < p.stats_C) {
+      named_bar_sync(1, kConsumerThreads);                // every warp has added its last tile
+      const int etid = threadIdx.x;
+      if (etid < p.BN) {
         float s = 0.f, qq = 0.f;
 #pragma unroll
         for (int w = 0; w < 4; ++w) {
           s += racc[(w * 2 + 0) * 128 + etid];
           qq += racc[(w * 2 + 1) * 128 + etid];
+          racc[(w * 2 + 0) * 128 + etid] = 0.f;
+          racc[(w * 2 + 1) * 128 + etid] = 0.f;
         }
         // 64-bit fixed-point integer atomics onto the image's single statistics row: order independent (deterministic)
-        atomicAdd(&p.stats[((size_t)acc_img * 2 + 0) * p.stats_C + acc_n0 + etid], (stat_t)__float2ll_rn(s * V2V_STAT_SUM_SCALE));
-        atomicAdd(&p.stats[((size_t)acc_img * 2 + 1) * p.stats_C + acc_n0 + etid], (stat_t)__float2ll_rn(qq * V2V_STAT_SQ_SCALE));
+        if (acc_n0 + etid < p.stats_C) {
+          atomicAdd(&p.stats[((size_t)acc_img * 2 + 0) * p.stats_C + acc_n0 + etid], (stat_t)__float2ll_rn(s * V2V_STAT_SUM_SCALE));
+          atomicAdd(&p.stats[((size_t)acc_img * 2 + 1) * p.stats_C + acc_n0 + etid], (stat_t)__float2ll_rn(qq * V2V_STAT_SQ_SCALE));
+        }
       }
-      named_bar_sync(1 + eg, kEpiThreads);                // racc may be cleared again
+      named_bar_sync(1, kConsumerThreads);                // every column is zero again
     };
-    // group eg handles units it = eg, eg + EG, ...; with EG > 1 its accumulator stage is always eg
-    const int tw_shift = __ffs(p.TW) - 1;                 // TW is a power of two
-    const int row = q * 32 + lane;
-    const int ry = row >> tw_shift, rx = row & (p.TW - 1);
+    for (int i = threadIdx.x; i < kRedFloats; i += kConsumerThreads) racc[i] = 0.f;    // (ordered by the first stage())
+    // accumulator columns [c0, c0 + 64) of tile jt -> staging rows (the wgmma fragment layout, see wgmma.cuh)
+    auto stage = [&](int jt, int c0) {
+#pragma unroll
+      for (int j = 0; j < MG; ++j) {
+        if (j != jt) continue;
+#pragma unroll
+        for (int b = 0; b < BN / 8; ++b) {
+          if (b * 8 < c0 || b * 8 >= c0 + 64) continue;
+          const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), col = b * 8 + 2 * (lane & 3) - c0;
+          stg[r0 * kStgStride + col] = acc[j][b * 4 + 0];
+          stg[r0 * kStgStride + col + 1] = acc[j][b * 4 + 1];
+          stg[(r0 + 8) * kStgStride + col] = acc[j][b * 4 + 2];
+          stg[(r0 + 8) * kStgStride + col + 1] = acc[j][b * 4 + 3];
+        }
+      }
+      named_bar_sync(1, kConsumerThreads);
+    };
+
+    int gs = 0, as = 0, bs = 0;
+    uint32_t gpar = 0, gen = 0, apar = 0, bpar = 0;
+    int prev_key = -1;
     UnitIter un;
-    un.init(p, t_first + eg * t_step, t_step * p.EG);
-    for (int ju = 0; un.valid(p); un.next(p), ++ju) {
-      const int it = eg + ju * p.EG;
-      const int my_as = p.EG > 1 ? eg : (ju & 1);
-      const uint32_t my_phase = p.EG > 1 ? (ju & 1) : ((ju >> 1) & 1);
-      // everything that does not depend on the accumulator is computed before waiting for it
+    un.init(p, t_first, t_step);
+    for (; un.valid(p);) {
       const ConvPhase ph = p.phases[un.phase];
-      const int gy = un.y0(p) + ry, gx0 = un.x0(p) + rx;
+      const int key = un.key;
+      const bool first_of_key = key != prev_key;
+      if (p.b_resident && first_of_key && prev_key >= 0) gen ^= 1;
+      prev_key = key;
+      // everything the epilogue needs from the iterator, captured before it advances
+      const int y0 = un.y0(p), x0 = un.x0(p), n0 = un.n0(p), n_img = un.img;
+      un.next(p);
+      const bool last_of_key = !un.valid(p) || un.key != key;
+      const int nsteps = (ph.group_end - ph.group_begin) * p.cblocks;
+
+      // ---------------- MMAs
+      if (p.b_resident && first_of_key) mbar_wait_converged(bres_full, gen);
+#pragma unroll
+      for (int j = 0; j < MG; ++j) wgmma_fence_operands(acc[j]);
+      wgmma_fence();
+      uint32_t first = 0;
+      if (p.ring2) {
+        // K loop: steps (tap group, K block); per step ONE patch slot (MG tiles) from the A ring and ceil(R / TB) weight
+        // chunks from the B ring; tap r of the step reads the patch advanced by (r / RW) * PW + (r % RW) rows.
+        const int RH = p.R / p.RW;
+        for (int st = 0; st < nsteps; ++st) {
+          mbar_wait_converged(&g_full[as], apar);
+          const uint32_t a_base16 = (smem_u32(sG + (size_t)as * p.MG * p.a_slot_bytes) & 0x3FFFF) >> 4;
+          uint32_t bchunk16 = 0;
+          int tin = 0, r = 0;
+          for (int ky = 0; ky < RH; ++ky) {
+            for (int kx = 0; kx < p.RW; ++kx, ++r) {
+              if (tin == 0) {
+                mbar_wait_converged(&b_full[bs], bpar);
+                bchunk16 = ((sB_u32 + (uint32_t)bs * (uint32_t)p.b_slot_bytes) & 0x3FFFF) >> 4;
+              }
+              mma_tap<BN, MG>(acc, a_d0 + a_base16 + (uint32_t)ky * prow16 + (uint32_t)kx * row16, b_d0 + bchunk16 + (uint32_t)tin * b_step,
+                              a_tile16, p.kmma, ps_step, a_half16, b_half16, first);
+              first = 1u;
+              if (++tin == p.TB || r == p.R - 1) {             // chunks hold TB taps; the last one of a step may be short
+                tin = 0;
+                commit_and_retire_previous(r == p.R - 1 ? as : -1, bs);      // the patch slot retires with the step's last chunk
+                if (++bs == p.SBr) { bs = 0; bpar ^= 1; }
+                wgmma_fence();
+              }
+            }
+          }
+          if (++as == p.SG) { as = 0; apar ^= 1; }
+        }
+      } else {
+        for (int s0 = 0; s0 < nsteps; s0 += p.CG) {
+          const int n = min(p.CG, nsteps - s0);
+          mbar_wait_converged(&g_full[gs], gpar);
+          const uint32_t base = smem_u32(sG + (size_t)gs * group_bytes);
+          for (int i = 0; i < n; ++i) {
+            const uint32_t b_base = p.b_resident ? sB_u32 + (s0 + i) * p.b_slot_bytes
+                                                 : base + p.CG * p.MG * p.a_slot_bytes + i * p.b_slot_bytes;
+            const uint32_t a_base = base + i * p.MG * p.a_slot_bytes;
+            uint32_t al = (a_base & 0x3FFFF) >> 4, bl = (b_base & 0x3FFFF) >> 4;
+            // tap r reads the patch shifted by (r / RW) patch rows and (r % RW) pixels
+            for (int r0 = 0; r0 < p.R; r0 += p.RW, al += a_wrap) {
+              for (int r = 0; r < p.RW; ++r, al += a_step, bl += b_step) {
+                mma_tap<BN, MG>(acc, a_d0 + al, b_d0 + bl, a_tile16, p.kmma, ps_step, a_half16, b_half16, first);
+                first = 1u;
+              }
+            }
+          }
+          commit_and_retire_previous(gs, -1);              // the whole group slot retires with these MMAs
+          if (++gs == p.SG) { gs = 0; gpar ^= 1; }
+          wgmma_fence();
+        }
+      }
+      drain();
+      __syncwarp();
+      mbar_arrive_if(bres_empty, lane == 0 && p.b_resident && last_of_key);
+
+      // ---------------- epilogue
+      const int gy = y0 + ry, gx0 = x0 + rx;
       const int oy = gy * p.oy_mul + ph.oy_add;
-      const int n0 = un.n0(p), n_img = un.img;
-      if (q == 0) TRACE(2, it, 0);
-      mbar_wait(&tmem_full[my_as], my_phase);
-      tcgen05_fence_after();
-      if (q == 0) TRACE(2, it, 1);
-      for (int jt = 0; jt < p.MG; ++jt) {                   // the unit's MG tiles sit side by side along x
-        const bool last_tile = (jt == p.MG - 1);
+#pragma unroll
+      for (int jt = 0; jt < MG; ++jt) {                   // the unit's MG tiles sit side by side along x
         const int gx = gx0 + jt * p.TW;
         const bool valid = (gy < p.grid_h) && (gx < p.grid_w);
         const int ox = gx * p.ox_mul + ph.ox_add;
-        const uint32_t taddr = tmem_base + (my_as * p.MG + jt) * acc_cols + (static_cast<uint32_t>(q * 32) << 16);
         bf16* dst = nullptr;
         float* dstf = nullptr;
         if (valid && p.epi != EPI_HEAD_F32) {
@@ -531,200 +430,157 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             dst = p.out_act.base + p.out_act.offset(n_img, oy, ox);
           }
         }
+        const float* srow = stg + row * kStgStride;
 
         if (p.epi == EPI_HEAD_F32 && p.headkx) {
-          // kx-GEMM head.  Tile = 4 rows x 32 INPUT pixels: TMEM lane quarter q = tile row, lane = pixel, accumulator
-          // column kx * Cout + c.  out(x)[c] = sum_kx D[x + kx][kx * Cout + c] is a sum over the NEXT kw - 1 lanes of the
-          // same warp: warp shuffles, no shared memory.  Lanes 32 - (kw - 1) .. 31 only feed their left neighbours
-          // (tiles advance by tile_dx = 32 - (kw - 1) pixels).
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(taddr, r);
-          tmem_ld_wait();
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[my_as]);
-          float acc[4];
-          switch (p.Cout) {
-            case 1: head_shift_sum<1>(r, p.headkx, acc); break;
-            case 2: head_shift_sum<2>(r, p.headkx, acc); break;
-            case 3: head_shift_sum<3>(r, p.headkx, acc); break;
-            default: head_shift_sum<4>(r, p.headkx, acc); break;
-          }
-          if (valid && rx < p.tile_dx) {
-            const size_t pix = (size_t)oy * p.out_W + ox;
+          // kx-GEMM head.  Tile = 4 rows x 32 INPUT pixels: warp quarter q = tile row, lane = pixel, accumulator column
+          // kx * Cout + c.  out(x)[c] = sum_kx D[x + kx][kx * Cout + c] is a sum over the NEXT kw - 1 lanes of the same
+          // warp: warp shuffles.  Lanes 32 - (kw - 1) .. 31 only feed their left neighbours (tiles advance by
+          // tile_dx = 32 - (kw - 1) pixels).
+          stage(jt, 0);
+          if (hc == 0) {
+            uint32_t r[32];
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              if (j < p.Cout) {
-                float v = acc[j];
-                if (p.bias) v += (p.bias2 && j >= p.Cout1) ? __ldg(p.bias2 + j - p.Cout1) : __ldg(p.bias + j);
-                v = apply_act(v, p.head_act[j], p.lrelu_slope) * p.head_scale[j];
-                reinterpret_cast<float*>(p.io[p.head_slot[j]])[p.head_off[j] + (size_t)n_img * p.head_bstride[j] + pix] = v;
+            for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(srow[j]);
+            float hacc[4];
+            switch (p.Cout) {
+              case 1: head_shift_sum<1>(r, p.headkx, hacc); break;
+              case 2: head_shift_sum<2>(r, p.headkx, hacc); break;
+              case 3: head_shift_sum<3>(r, p.headkx, hacc); break;
+              default: head_shift_sum<4>(r, p.headkx, hacc); break;
+            }
+            if (valid && rx < p.tile_dx) {
+              const size_t pix = (size_t)oy * p.out_W + ox;
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                if (j < p.Cout) {
+                  float v = hacc[j];
+                  if (p.bias) v += (p.bias2 && j >= p.Cout1) ? __ldg(p.bias2 + j - p.Cout1) : __ldg(p.bias + j);
+                  v = apply_act(v, p.head_act[j], p.lrelu_slope) * p.head_scale[j];
+                  reinterpret_cast<float*>(p.io[p.head_slot[j]])[p.head_off[j] + (size_t)n_img * p.head_bstride[j] + pix] = v;
+                }
               }
             }
           }
+          named_bar_sync(1, kConsumerThreads);
           continue;
         }
         if (p.epi == EPI_HEAD_F32) {
-          uint32_t r[16];
-          tmem_ld_32x32b_x16(taddr, r);
-          tmem_ld_wait();
-          if (last_tile) {
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[my_as]);
-          }
-          if (valid) {
+          stage(jt, 0);
+          if (hc == 0 && valid) {
             const size_t pix = (size_t)oy * p.out_W + ox;
 #pragma unroll
             for (int j = 0; j < V2V_MAX_HEAD; ++j) {
               if (j < p.Cout) {
-                float v = __uint_as_float(r[j]);
+                float v = srow[j];
                 if (p.bias) v += (p.bias2 && j >= p.Cout1) ? __ldg(p.bias2 + j - p.Cout1) : __ldg(p.bias + j);
                 v = apply_act(v, p.head_act[j], p.lrelu_slope) * p.head_scale[j];
                 reinterpret_cast<float*>(p.io[p.head_slot[j]])[p.head_off[j] + (size_t)n_img * p.head_bstride[j] + pix] = v;
               }
             }
           }
+          named_bar_sync(1, kConsumerThreads);
           continue;
         }
 
-        if (do_stats && (un.key != acc_key || n_img != acc_img)) {
+        if (do_stats && (key != acc_key || n_img != acc_img)) {
           if (acc_key >= 0) flush();
-          for (int c = lane; c < 2 * 128; c += 32) racc[q * 256 + c] = 0.f;
-          __syncwarp();
-          acc_key = un.key; acc_img = n_img; acc_n0 = n0; acc_phase = un.phase;
+          acc_key = key; acc_img = n_img; acc_n0 = n0;
         }
-        for (int c = 0; c < nchunks; ++c) {
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(taddr + c * 32, r);
-          tmem_ld_wait();
-          if (q == 0 && c == 0) TRACE(2, it, 3);
-          if (last_tile && c == nchunks - 1) {    // accumulators fully read: hand the TMEM stage back to the MMA warp
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[my_as]);
-          }
-          float v[32];
-          const int col0 = n0 + c * 32;
+        for (int c0 = 0; c0 < nchunks; c0 += 2) {
+          stage(jt, c0 * 32);
+          const int c = c0 + hc;
+          if (c < nchunks) {
+            float v[32];
+            const int col0 = n0 + c * 32;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = valid ? __uint_as_float(r[j]) : 0.f;
-          if (p.epi == EPI_ACT_BF16) {
+            for (int j = 0; j < 32; ++j) v[j] = valid ? srow[hc * 32 + j] : 0.f;
+            if (p.epi == EPI_ACT_BF16) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              float b = (p.bias && col0 + j < p.Cout) ? __ldg(p.bias + col0 + j) : 0.f;
-              v[j] = (col0 + j < p.Cout) ? apply_act(v[j] + b, p.act, p.lrelu_slope) : 0.f;
-            }
-          }
-          if (valid && !(p.dbg & 2)) {
-            if (dstf) {                                // precise plan: fp32 raw output
-#pragma unroll
-              for (int qv = 0; qv < 8; ++qv)
-                if (col0 + qv * 4 < p.out_C)
-                  *reinterpret_cast<float4*>(dstf + col0 + qv * 4) = make_float4(v[qv * 4], v[qv * 4 + 1], v[qv * 4 + 2], v[qv * 4 + 3]);
-            } else if (p.epi == EPI_ACT_BF16 && p.out_act.split) {
-#pragma unroll
-              for (int qv = 0; qv < 4; ++qv) {
-                if (col0 + qv * 8 < p.out_C) {
-                  float lo[8];
-#pragma unroll
-                  for (int j = 0; j < 8; ++j) lo[j] = v[qv * 8 + j] - __bfloat162float(__float2bfloat16_rn(v[qv * 8 + j]));
-                  uint4 pk, pl;
-                  pk.x = pack_bf16x2(v[qv * 8 + 0], v[qv * 8 + 1]); pl.x = pack_bf16x2(lo[0], lo[1]);
-                  pk.y = pack_bf16x2(v[qv * 8 + 2], v[qv * 8 + 3]); pl.y = pack_bf16x2(lo[2], lo[3]);
-                  pk.z = pack_bf16x2(v[qv * 8 + 4], v[qv * 8 + 5]); pl.z = pack_bf16x2(lo[4], lo[5]);
-                  pk.w = pack_bf16x2(v[qv * 8 + 6], v[qv * 8 + 7]); pl.w = pack_bf16x2(lo[6], lo[7]);
-                  *reinterpret_cast<uint4*>(dst + col0 + qv * 8) = pk;
-                  *reinterpret_cast<uint4*>(dst + p.out_act.C + col0 + qv * 8) = pl;
-                }
+              for (int j = 0; j < 32; ++j) {
+                float b = (p.bias && col0 + j < p.Cout) ? __ldg(p.bias + col0 + j) : 0.f;
+                v[j] = (col0 + j < p.Cout) ? apply_act(v[j] + b, p.act, p.lrelu_slope) : 0.f;
               }
-            } else {
+            }
+            if (valid && !(p.dbg & 2)) {
+              if (dstf) {                                // precise plan: fp32 raw output
 #pragma unroll
-              for (int qv = 0; qv < 4; ++qv) {
-                if (col0 + qv * 8 < p.out_C) {
-                  uint4 pk;
-                  pk.x = pack_bf16x2(v[qv * 8 + 0], v[qv * 8 + 1]);
-                  pk.y = pack_bf16x2(v[qv * 8 + 2], v[qv * 8 + 3]);
-                  pk.z = pack_bf16x2(v[qv * 8 + 4], v[qv * 8 + 5]);
-                  pk.w = pack_bf16x2(v[qv * 8 + 6], v[qv * 8 + 7]);
-                  *reinterpret_cast<uint4*>(dst + col0 + qv * 8) = pk;
+                for (int qv = 0; qv < 8; ++qv)
+                  if (col0 + qv * 4 < p.out_C)
+                    *reinterpret_cast<float4*>(dstf + col0 + qv * 4) = make_float4(v[qv * 4], v[qv * 4 + 1], v[qv * 4 + 2], v[qv * 4 + 3]);
+              } else if (p.epi == EPI_ACT_BF16 && p.out_act.split) {
+#pragma unroll
+                for (int qv = 0; qv < 4; ++qv) {
+                  if (col0 + qv * 8 < p.out_C) {
+                    float lo[8];
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) lo[j] = v[qv * 8 + j] - __bfloat162float(__float2bfloat16_rn(v[qv * 8 + j]));
+                    uint4 pk, pl;
+                    pk.x = pack_bf16x2(v[qv * 8 + 0], v[qv * 8 + 1]); pl.x = pack_bf16x2(lo[0], lo[1]);
+                    pk.y = pack_bf16x2(v[qv * 8 + 2], v[qv * 8 + 3]); pl.y = pack_bf16x2(lo[2], lo[3]);
+                    pk.z = pack_bf16x2(v[qv * 8 + 4], v[qv * 8 + 5]); pl.z = pack_bf16x2(lo[4], lo[5]);
+                    pk.w = pack_bf16x2(v[qv * 8 + 6], v[qv * 8 + 7]); pl.w = pack_bf16x2(lo[6], lo[7]);
+                    *reinterpret_cast<uint4*>(dst + col0 + qv * 8) = pk;
+                    *reinterpret_cast<uint4*>(dst + p.out_act.C + col0 + qv * 8) = pl;
+                  }
+                }
+              } else {
+#pragma unroll
+                for (int qv = 0; qv < 4; ++qv) {
+                  if (col0 + qv * 8 < p.out_C) {
+                    uint4 pk;
+                    pk.x = pack_bf16x2(v[qv * 8 + 0], v[qv * 8 + 1]);
+                    pk.y = pack_bf16x2(v[qv * 8 + 2], v[qv * 8 + 3]);
+                    pk.z = pack_bf16x2(v[qv * 8 + 4], v[qv * 8 + 5]);
+                    pk.w = pack_bf16x2(v[qv * 8 + 6], v[qv * 8 + 7]);
+                    *reinterpret_cast<uint4*>(dst + col0 + qv * 8) = pk;
+                  }
                 }
               }
             }
-          }
-          if (q == 0 && c == nchunks - 1) TRACE(2, it, 4);
-          if (do_stats) {
-            // column sums over this warp's 32 rows through a padded shared-memory transpose, 16 columns per pass:
-            // lane = row stores 16 values (stride 17: conflict free); lane l then walks column l % 16 over rows
-            // 16 * (l / 16) .. +15 (banks 17 r + 16 (l / 16) + l % 16: conflict free) and one xor-16 shuffle joins
-            // the two half sums.  Lanes 0-15 keep the first pass, lanes 16-31 the second: lane l owns column l.
-            float s_keep = 0.f, q_keep = 0.f;
-            if (p.dbg & 16) {
-              // register-only variant (recursive-halving shuffles, 2 x 31 per chunk): no shared-memory traffic, which
-              // the tensor core's operand reads compete for in the small-N layers
-              float v2[32];
+            if (do_stats) {
+              // column sums over this warp's 32 rows: each lane writes its (masked) row back into the staging tile, then
+              // lane l walks column l down the 32 rows (banks (r + l) mod 32: conflict free)
+              float* sw = stg + hc * 32;
 #pragma unroll
-              for (int j = 0; j < 32; ++j) v2[j] = v[j] * v[j];
-              s_keep = warp_transpose_reduce(v, lane);
-              q_keep = warp_transpose_reduce(v2, lane);
-            } else
-#pragma unroll
-            for (int h2 = 0; h2 < 2; ++h2) {
-              __syncwarp();
-#pragma unroll
-              for (int j = 0; j < 16; ++j) tt[lane * 17 + j] = v[h2 * 16 + j];
+              for (int j = 0; j < 32; ++j) sw[row * kStgStride + j] = v[j];
               __syncwarp();
               float s = 0.f, qq = 0.f;
-              const float* colp = tt + (lane >> 4) * (16 * 17) + (lane & 15);
 #pragma unroll
-              for (int r2 = 0; r2 < 16; ++r2) {
-                const float x = colp[r2 * 17];
+              for (int r2 = 0; r2 < 32; ++r2) {
+                const float x = sw[(q * 32 + r2) * kStgStride + lane];
                 s += x;
                 qq = fmaf(x, x, qq);
               }
-              s += __shfl_xor_sync(0xffffffffu, s, 16);
-              qq += __shfl_xor_sync(0xffffffffu, qq, 16);
-              if ((lane >> 4) == h2) { s_keep = s; q_keep = qq; }
+              racc[(q * 2 + 0) * 128 + c * 32 + lane] += s;
+              racc[(q * 2 + 1) * 128 + c * 32 + lane] += qq;
             }
-            racc[(q * 2 + 0) * 128 + c * 32 + lane] += s_keep;
-            racc[(q * 2 + 1) * 128 + c * 32 + lane] += q_keep;
           }
+          named_bar_sync(1, kConsumerThreads);             // the staging tile may be overwritten
         }
-        if (q == 0) TRACE(2, it, 5);
       }
-      if (q == 0) TRACE(2, it, 2);
     }
     if (do_stats && acc_key >= 0) flush();
   }
 
-  tcgen05_fence_before();
   __threadfence();                                  // this thread's statistics atomics are visible device-wide
   __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, tmem_cols);
   if (p.n_fin > 0) {
     // Statistics finalisation by the LAST CTA to get here (ticket counter, zeroed with the statistics rows before every run):
     // all rows are complete then; every other CTA has exited, nobody waits.
-    if (threadIdx.x == 0) *tmem_slot = atomicAdd(p.fin_counter, 1u);
+    if (threadIdx.x == 0) *ticket = atomicAdd(p.fin_counter, 1u);
     __syncthreads();
-    if (*tmem_slot == gridDim.x - 1) {
+    if (*ticket == gridDim.x - 1) {
       __threadfence();
       for (int f = 0; f < p.n_fin; ++f)
         for (int c = threadIdx.x; c < p.fin[f].C; c += blockDim.x) channel_side_effects(p.fin[f], c);
     }
   }
-  if ((p.dbg & 4) && blockIdx.x == 0 && threadIdx.x == 0) {
-    const long long t0 = g_trace[0][0][0];
-    for (int it = 0; it < 24; ++it)
-      printf("trace it=%2d prod: start %6lld issued %6lld | mma: start %6lld tmem_empty %6lld first_a %6lld done %6lld | "
-             "epi: start %6lld full %6lld ld(last tile) %6lld stored %6lld stats %6lld done %6lld\n", it,
-             g_trace[0][it][0] - t0, g_trace[0][it][2] - t0, g_trace[1][it][0] - t0, g_trace[1][it][1] - t0,
-             g_trace[1][it][2] - t0, g_trace[1][it][3] - t0, g_trace[2][it][0] - t0, g_trace[2][it][1] - t0,
-             g_trace[2][it][3] - t0, g_trace[2][it][4] - t0, g_trace[2][it][5] - t0, g_trace[2][it][2] - t0);
-  }
 }
 
 bool pdl_enabled() {
-  // opt-in (V2V_PDL=1): measured on cfg4 it is correct but slower (16.4 vs 15.6 ms/frame; cfg2 5.0 vs 4.6): the early-launched
-  // blocks of the elementwise kernels sit in griddepcontrol.wait holding thread slots the persistent conv CTAs then wait for
+  // opt-in (V2V_PDL=1): the early-launched blocks of the elementwise kernels sit in griddepcontrol.wait holding thread slots
+  // the persistent conv CTAs then wait for
   static const bool on = [] { const char* e = getenv("V2V_PDL"); return e && e[0] == '1'; }();
   return on;
 }
@@ -735,25 +591,43 @@ int device_sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
 
-cudaError_t launch_conv_umma(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvKernelParams& p,
-                             cudaStream_t stream) {
-  const size_t operands = p.ring2 ? (size_t)p.SG * p.MG * p.a_slot_bytes + (size_t)p.SBr * p.b_slot_bytes
-                                  : (size_t)p.SG * p.CG * ((size_t)p.MG * p.a_slot_bytes + (p.b_resident ? 0 : p.b_slot_bytes)) +
-                                        (p.b_resident ? (size_t)p.SB * p.b_slot_bytes : 0);
-  const size_t smem = operands + 1024 /*align*/ + (size_t)p.EG * kRedFloatsPerGroup * sizeof(float) +
-                      (2 * p.SG + 2 + 2 * kMaxGroups + 2 + 16) * sizeof(uint64_t);
+template <int BN, int MG>
+static cudaError_t launch_bn_mg(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvKernelParams& p, size_t smem, cudaStream_t stream) {
   static size_t configured = 0;
   if (smem > configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<BN, MG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     configured = smem;
   }
-  return launch_pdl(conv_umma_kernel, dim3(p.grid), dim3(64 + 128 * p.EG), smem, stream, tmA, tmB, p);
+  return launch_pdl(conv_umma_kernel<BN, MG>, dim3(p.grid), dim3(kThreads), smem, stream, tmA, tmB, p);
+}
+
+size_t conv_umma_smem_bytes(const ConvKernelParams& p) {
+  const size_t operands = p.ring2 ? (size_t)p.SG * p.MG * p.a_slot_bytes + (size_t)p.SBr * p.b_slot_bytes
+                                  : (size_t)p.SG * p.CG * ((size_t)p.MG * p.a_slot_bytes + (p.b_resident ? 0 : p.b_slot_bytes)) +
+                                        (p.b_resident ? (size_t)p.SB * p.b_slot_bytes : 0);
+  return operands + 1024 /*align*/ + (size_t)(kStgFloats + kRedFloats) * sizeof(float) + (2 * p.SG + 2 + 16 + 1) * sizeof(uint64_t);
+}
+
+cudaError_t launch_conv_umma(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvKernelParams& p,
+                             cudaStream_t stream) {
+  const size_t smem = conv_umma_smem_bytes(p);
+  // the N tile and the M blocking fix the accumulator registers: one instantiation per plan choice (V2V_MAX_ACC_COLS)
+  switch (p.BN * 4 + p.MG) {
+    case 16 * 4 + 1: return launch_bn_mg<16, 1>(tmA, tmB, p, smem, stream);
+    case 32 * 4 + 1: return launch_bn_mg<32, 1>(tmA, tmB, p, smem, stream);
+    case 32 * 4 + 2: return launch_bn_mg<32, 2>(tmA, tmB, p, smem, stream);
+    case 64 * 4 + 1: return launch_bn_mg<64, 1>(tmA, tmB, p, smem, stream);
+    case 64 * 4 + 2: return launch_bn_mg<64, 2>(tmA, tmB, p, smem, stream);
+    case 96 * 4 + 1: return launch_bn_mg<96, 1>(tmA, tmB, p, smem, stream);
+    case 128 * 4 + 1: return launch_bn_mg<128, 1>(tmA, tmB, p, smem, stream);
+    default: return cudaErrorInvalidConfiguration;
+  }
 }
 
 }  // namespace v2v

@@ -1,4 +1,4 @@
-// sm_100a replacements for the three native FlowNet2 operators of the reference
+// sm_90a replacements for the three native FlowNet2 operators of the reference
 // (models/flownet2_pytorch/networks/{correlation,resample2d,channelnorm}_package/*.cu).
 // All three are fp32, NCHW, HBM/L2-bound; outputs are caller-owned (C-ABI in include/v2v_b200.h).
 #include "ptx.cuh"
@@ -148,7 +148,7 @@ __global__ void channelnorm_kernel(const float* __restrict__ in, float* __restri
 
 static inline int grid1d(size_t total) {
   size_t b = (total + 255) / 256;
-  const size_t cap = 148 * 16;
+  const size_t cap = 132 * 16;
   return (int)(b < cap ? (b ? b : 1) : cap);
 }
 

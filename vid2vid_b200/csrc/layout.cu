@@ -208,7 +208,7 @@ __global__ void bias_affine_kernel(float* scale, float* shift, const float* bias
 cudaError_t launch_act_copy(const CopyParams& p, cudaStream_t stream) {
   const size_t total = (size_t)p.out.N * (p.out.H + p.out.pad_t + p.out.pad_b) * (p.out.W + p.out.pad_l + p.out.pad_r) * p.in.Cvalid;
   size_t b = (total + 255) / 256;
-  if (b > 148 * 16) b = 148 * 16;
+  if (b > 132 * 16) b = 132 * 16;
   return launch_pdl(act_copy_kernel, dim3((unsigned)(b ? b : 1)), dim3(256), 0, stream, p);
 }
 
@@ -308,7 +308,7 @@ cudaError_t launch_pack_weights(const PackParams& p, cudaStream_t stream) {
   }
   const long long total = (long long)(p.headkx ? p.headkx * p.Cout : p.Cout) * p.ntaps * p.Cp;
   long long b = (total + 255) / 256;
-  if (b > 148 * 16) b = 148 * 16;
+  if (b > 132 * 16) b = 132 * 16;
   pack_weights_kernel<<<(int)b, 256, 0, stream>>>(p);
   return cudaGetLastError();
 }

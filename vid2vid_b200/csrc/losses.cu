@@ -132,7 +132,7 @@ __global__ void resample_bwd_kernel(const float* __restrict__ img, const float* 
 
 static inline int grid1d(size_t total) {
   size_t b = (total + 255) / 256;
-  const size_t cap = 148 * 8;
+  const size_t cap = 132 * 8;
   return (int)(b < cap ? (b ? b : 1) : cap);
 }
 

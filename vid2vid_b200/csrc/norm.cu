@@ -119,8 +119,8 @@ __global__ void __launch_bounds__(256) norm_apply_kernel(ApplyParams p) {
 
 // Row-segment variant (default).  A block owns one padded output row (n, yp) and a segment of it; a thread keeps ONE
 // 8-channel vector v = t % vecs for its whole life, so scale / shift live in registers and there is no division or
-// 64-bit index arithmetic per item: the grid-stride kernel above issues ~260 instructions per 16-byte item (ncu:
-// issue slots 77 % busy, IPC 3.1, 2.7 TB/s) and is instruction bound, this one ~45.
+// 64-bit index arithmetic per item: the grid-stride kernel above issues ~260 instructions per 16-byte item and is
+// instruction bound, this one ~45.
 // Consecutive threads cover the C * 2 contiguous bytes of a pixel, then the next pixel: loads and stores are coalesced.
 struct RowAddr { size_t base; int xs; size_t plane; int parity, C, pad_l; };   // C = bf16 elements per pixel
 __device__ __forceinline__ RowAddr row_addr(const ActDesc& a, int n, int y) {     // y relative to the interior
@@ -183,8 +183,7 @@ __global__ void __launch_bounds__(256) norm_apply_rows_kernel(ApplyParams p, int
   }
   const int x_end = min(Wpad, (int)(blockIdx.x + 1) * xt);
   // Batches of NB items: all loads of a batch are issued before the first use, so a thread keeps several 16-byte loads
-  // in flight -- one load per thread leaves the kernel latency bound (~21 KB in flight per SM against the ~35 KB HBM3e
-  // needs at 6.5 TB/s).
+  // in flight -- one load per thread leaves the kernel latency bound.
   for (int xb = blockIdx.x * xt + pl; xb < x_end; xb += NB * ppb) {
     uint4 r[NB][NW], q0[NADD > 0 ? NB : 1][NW], q1[NADD > 1 ? NB : 1][NW];
     bool live[NB];
@@ -263,7 +262,7 @@ __global__ void __launch_bounds__(256) norm_apply_rows_kernel(ApplyParams p, int
 
 static inline int grid_for(long long total, int block) {
   long long b = (total + block - 1) / block;
-  const long long cap = 148LL * 16;
+  const long long cap = 132LL * 16;
   return (int)(b < cap ? (b > 0 ? b : 1) : cap);
 }
 

@@ -1,7 +1,7 @@
 // Plan runtime: lowers a graph of logical values / convolution units (described through the C ABI in
 // include/v2v_b200.h) to halo-padded NHWC bf16 buffers, TMA tensor maps, packed weight matrices and a
 // flat kernel sequence, captures the sequence in a CUDA graph and replays it per frame.
-// This is the B200-native counterpart of the nn.Module surface the reference's Vid2VidModelG calls
+// This is the H100-native counterpart of the nn.Module surface the reference's Vid2VidModelG calls
 // (netG.forward, models/vid2vid_model_G.py:225-226; module bodies models/networks.py:117-419,634-725).
 #include <algorithm>
 #include <cmath>
@@ -86,7 +86,7 @@ struct ConvGeom {
 
 
 static inline int round_up_i(int a, int b) { return round_up(a, b); }
-static const int kSmemBudget = 200 * 1024;      // operand slots + resident weights (227 KB - 2 x 12.5 KB epilogue scratch - alignment - barriers)
+static const int kSmemBudget = 188 * 1024;      // operand slots + resident weights (227 KB - 36.5 KB epilogue staging - alignment - barriers)
 static const int kResidentMax = 150 * 1024;
 
 // 2-D patch mode (stride-1 filters): a tile of 16 rows x 8 pixels makes every 8-row core-matrix group of the A operand
@@ -110,7 +110,7 @@ static bool choose_patch2d(const v2v_conv_desc& c, bool head, int N, int grid_h,
   // weights again for every tile costs more L2 traffic than the second pass over the activations)
   for (int pass = 0; pass < 2; ++pass) {
     const int bn = pass == 0 ? bn0 : bn0 / 2;
-    // (measured on 128->128 @256x512: 58 us with the halved N tile vs 50 us streamed, so pass 2 is opt-in)
+    // (pass 2 is opt-in: it has not been measured to pay off)
     static const bool half_ok = [] { const char* e = getenv("V2V_P2D_HALF"); return e && e[0] == '1'; }();
     if (pass == 1 && (!half_ok || bn0 < 128 || m_total < 4LL * sms)) break;
     if (m_total <= sms) break;
@@ -126,10 +126,9 @@ static bool choose_patch2d(const v2v_conv_desc& c, bool head, int N, int grid_h,
     }
   }
   // Streamed weights: only when a CTA sees few M tiles (the weights pass through once per unit either way, and the
-  // patch saves the activation re-reads: 1024->1024 @32x64 50 us vs 58.6 us with one box per tap).  With many M tiles
-  // per CTA the row-tile path with M blocking shares each weight tile between tiles instead (measured: 128->128 @256x512
-  // 54 us here vs 51 us row tiles even before M blocking), and K blocks below 32 channels turn the 49 taps of a 7x7
-  // filter into 1 KB TMA boxes (108->32 @1024x2048: 2.16 ms vs 1.49 ms).
+  // patch saves the activation re-reads of one box per tap).  With many M tiles per CTA the row-tile path with M
+  // blocking shares each weight tile between tiles instead, and K blocks below 32 channels would turn the 49 taps of a
+  // 7x7 filter into 1 KB TMA boxes.
   if (m_total >= 4LL * sms) return false;
   // (precise plans: halve the N tile before going below 32-channel K blocks; 32-byte rows ingest badly)
   for (int bn = bn0; bn >= (sp == 2 && !head ? std::min(bn0, 64) : bn0); bn >>= 1)
@@ -141,7 +140,7 @@ static bool choose_patch2d(const v2v_conv_desc& c, bool head, int N, int grid_h,
   return false;
 }
 
-// head: 0 = no, 1 = small-Cout head, 2 = head that may use the kx-GEMM form (tcgen05 implementation only)
+// head: 0 = no, 1 = small-Cout head, 2 = head that may use the kx-GEMM form (tensor-core implementation only)
 static int conv_geometry(const v2v_conv_desc& c, int head, int N, int H, int W, bool allow_reuse, int sp, ConvGeom* g) {
   memset(g, 0, sizeof(*g));
   V2V_REQUIRE(c.kh >= 1 && c.kw >= 1 && c.kh * c.kw <= V2V_MAX_TAPS, V2V_ERR_UNSUPPORTED, "kernel %dx%d unsupported",
@@ -312,7 +311,7 @@ struct XOp {
 
 using namespace v2v;
 
-// Tensor-core backward of one conv op of a training plan (precise plans, tcgen05 implementation):
+// Tensor-core backward of one conv op of a training plan (precise plans, tensor-core implementation):
 //   data gradient   = a FORWARD conv of the output gradient, run by a sub-plan on conv_umma_kernel:
 //                       mode 1  stride-1 conv          -> stride-1 conv, zero pad k-1, weights transposed + flipped; the result covers
 //                                                         the padded input extent and fold_add folds the (reflect) halo back
@@ -526,21 +525,17 @@ static void fill_conv_params(v2v_plan* P, GOp& op) {
   const int m_tiles = kp.N * kp.tiles_x * kp.tiles_y;
   // M blocking for row-tile filters whose weights must be streamed (the 7x7 stems over the 108-channel label input):
   // per M tile such a layer pulls taps*Cp*BN*2 bytes of weights through L2 -> SM (802 KB for 108->48, 13 GB per launch at
-  // 2048x1024), i.e. 64 B per SM clock at the full MMA rate against the ~42 B/clk an SM ingests.  MG = 2 consecutive x
-  // tiles accumulate side by side in TMEM and share every weight tile.  The (K block, N tile, MG) choice is measured,
-  // not modelled (gpurun sweep with V2V_FORCE, ms per launch):
-  //     108->48 @1024x2048 : (64,64,1) 1.73  (64,64,2) 1.51  (32,64,2) 2.19  (32,64,4) 1.98  (64,32,2) 2.65
-  //     108->96 @512x1024  : (64,64,1) 0.875 (64,64,2) 0.769 (32,96,2) 0.622 (64,96,1) 0.826 (32,128,2) 0.828
-  //     108->192 @256x512  : (64,64,2) 0.316 (32,96,2) 0.323 (64,96,1) 0.337 (32,128,2) 0.351
-  //     128->128 3x3 @256x512 : (64,128,1) 52.2 us (64,128,2) 52.3 (32,128,2) 66.8 (64,64,2) 64.5   -> 3x3 stays as it was
-  // 64-byte rows (32-channel K blocks) cost ingest rate (requests, not bytes, are the limit) unless they buy an exact
-  // N tile (Cout = 96), and 4 tiles per unit (all 512 TMEM columns) were always slower than 2.
+  // 2048x1024), more than an SM ingests at the full MMA rate.  MG = 2 consecutive x tiles accumulate side by side in
+  // registers and share every weight tile, within the accumulator budget V2V_MAX_ACC_COLS.  64-byte rows (32-channel K
+  // blocks) cost TMA request rate, so they are used only where they buy an exact N tile (Cout = 96).  V2V_FORCE=kc,bn,mg
+  // overrides the choice for timing experiments.
   bool mblock = false;
   if (!p2d && !op.conv.transposed && op.conv.stride == 1 && g.R >= 5 && g.n_phases == 1 && op.kind != G_HEAD &&
       m_tiles >= 4 * device_sm_count() &&
       (long long)sp * op.conv.kh * op.conv.kw * kp.Cp * std::min(64, kp.BN) * 2 > kResidentMax) {   // cannot stay resident
     int c_kc = std::min(kp.Cp, 64), c_bn = std::min(64, round_up(op.conv.Cout, 32)), c_mg = 2;
     if (round_up(op.conv.Cout, 32) == 96 && kp.Cp % 32 == 0) { c_kc = 32; c_bn = 96; }
+    c_mg = std::max(1, std::min(c_mg, V2V_MAX_ACC_COLS / c_bn));      // (the exact 96-wide N tile leaves room for one tile)
     if (const char* ef = getenv("V2V_FORCE")) sscanf(ef, "%d,%d,%d", &c_kc, &c_bn, &c_mg);      // timing experiments
     const char* em = getenv("V2V_MG");
     if (em && atoi(em) == 0) c_mg = 0;                                                           // V2V_MG=0: off
@@ -548,7 +543,7 @@ static void fill_conv_params(v2v_plan* P, GOp& op) {
     const int cand[4][3] = {{c_kc, c_bn, c_mg}, {32, c_bn, c_mg}, {32, 64, c_mg}, {32, 64, 1}};
     for (int ci = 0; ci < (sp == 2 ? 4 : 1) && !mblock; ++ci) {
       const int t_kc = cand[ci][0], t_bn = cand[ci][1], t_mg = cand[ci][2];
-      if (t_mg < 1 || kp.Cp % t_kc || t_bn % 32 || t_bn > 128 || kp.tiles_x % t_mg || 2 * t_mg * std::max(32, t_bn) > 512) continue;
+      if (t_mg < 1 || kp.Cp % t_kc || t_bn % 32 || t_bn > 128 || kp.tiles_x % t_mg || t_mg * std::max(32, t_bn) > V2V_MAX_ACC_COLS) continue;
       const int a_slot = sp * round_up((g.TW + g.R - 1) * g.TH * t_kc * 2, 1024), b_slot = sp * round_up(g.R * t_bn * t_kc * 2, 1024);   // (never a head)
       if (2 * (t_mg * a_slot + b_slot) <= kSmemBudget) { kp.kc = t_kc; kp.BN = t_bn; kp.MG = t_mg; mblock = true; }
     }
@@ -565,13 +560,8 @@ static void fill_conv_params(v2v_plan* P, GOp& op) {
   kp.sbo_a_bytes = p2d ? kp.PW * kp.row_bytes : 8 * kp.row_bytes;
   kp.a_half_bytes = round_up(kp.PW * kp.PH * kp.row_bytes, 1024);
   kp.a_slot_bytes = sp * kp.a_half_bytes;
-  // Epilogue groups: layers whose K loop is shorter than the epilogue of a tile (small Cin * taps) are epilogue bound
-  // with one group; statistics allow at most 2 groups (order-independent atomic adds need <= 2 addends per element).
-  {
-    const char* eg = getenv("V2V_EG");
-    kp.EG = eg ? std::max(1, std::min(2, atoi(eg))) : 2;
-  }
-  // shared-memory budget: 227 KB - epilogue scratch (12.5 KB per group) - alignment slack - barriers
+  kp.EG = 1;                   // the two consumer warpgroups of conv_umma_kernel drain every tile together
+  // shared-memory budget: 227 KB - epilogue staging - alignment slack - barriers
   const int budget = kSmemBudget;
   // a weight slot holds the R taps served by one activation patch; keep >= 2 slots + 3 patches in the budget
   if (sp == 2 && !p2d && !mblock && g.R > 1 && !g.headkx) {
@@ -615,33 +605,31 @@ static void fill_conv_params(v2v_plan* P, GOp& op) {
   }
   kp.SB = kp.b_resident ? nB : 0;
   // Decoupled operand rings for streamed-weight layers whose coupled stages forced a narrow K block or N tile (see
-  // ConvKernelParams::ring2): 64-byte rows halve the TMA request efficiency (measured ~0.3 smem rows per clock whatever the row
-  // size) and N < 128 MMAs waste issue slots, which is what bounded 1024->1024 (kc 32) and every streamed precise layer.
+  // ConvKernelParams::ring2): 64-byte rows cost TMA request rate and narrow N tiles cost MMA issue slots.
   kp.ring2 = 0;
   {
     static const bool ring2_ok = [] { const char* e = getenv("V2V_RING2"); return !(e && e[0] == '0'); }();
     const int kc_nat = std::min(kp.Cp, 64), bn_nat = std::min(128, round_up(op.conv.Cout, 32));
-    // Measured (profiles/r02c_*): a gain for precise plans (108->96 2.20 -> 1.58 ms, 128->128 1.68 -> 1.26, 1024->1024 4.92 ->
-    // 4.18); bf16 plans and the exact-input finest stem were faster with the coupled stages (fewer barrier round trips per
-    // MMA), so they keep them.
+    // Precise plans only: bf16 plans and the exact-input finest stem keep the coupled stages (fewer barrier round trips
+    // per MMA).
     if (ring2_ok && sp == 2 && !kp.a_exact && P->impl == V2V_IMPL_UMMA && !kp.b_resident && g.R >= 3 && !g.headkx && g.n_phases == 1 &&
         op.kind != G_HEAD && (kp.kc < kc_nat || kp.BN < bn_nat)) {
       const int nhA = 2;
       const int a_half = round_up(kp.PW * kp.PH * kc_nat * 2, 1024);
       bool found = false;
       int f_bn = 0, f_mg = 0, f_tb = 0, f_sbr = 0;
-      // N tile: the natural one unless that leaves SMs idle (512->512 @32x64: 64 tiles of 128 columns on 148 SMs)
+      // N tile: the natural one unless that leaves SMs idle (512->512 @32x64: 64 tiles of 128 columns)
       const long long units_nat = (long long)kp.N * kp.tiles_x * kp.tiles_y * ((op.conv.Cout + bn_nat - 1) / bn_nat);
       const int bns[2] = {bn_nat, bn_nat / 2}, mgs[2] = {kp.MG, 1};
-      const bool too_few = units_nat * 5 < (long long)sms * 3;      // 512->512 @32x64: 64 tiles on 148 SMs -- the coupled BN 64 path wins (0.89 vs 1.00 ms)
+      const bool too_few = units_nat * 5 < (long long)sms * 3;      // then the coupled path with a halved N tile fills the SMs
       for (int bi = 0; bi < 2 && !found && !too_few; ++bi) {
         const int bn = bns[bi];
         if (bn < 32 || bn % 32 || (bi == 1 && bn < 64)) continue;
         for (int mi = 0; mi < 2 && !found; ++mi) {
           const int mg = mgs[mi];
-          if (mg < 1 || kp.tiles_x % mg || 2 * mg * std::max(32, bn) > 512 || (mi == 1 && mgs[0] == 1)) continue;
-          // taps per weight chunk: as many as leave >= 3 chunks in flight (a commit + barrier round trip per chunk costs the
-          // issuing thread ~500 cycles: fewer, longer chunks)
+          if (mg < 1 || kp.tiles_x % mg || mg * std::max(32, bn) > V2V_MAX_ACC_COLS || (mi == 1 && mgs[0] == 1)) continue;
+          // taps per weight chunk: as many as leave >= 3 chunks in flight (every chunk costs a commit group and a barrier
+          // round trip: fewer, longer chunks)
           for (int tb = std::min(g.R, 4); tb >= 1 && !found; --tb) {
             const int chunk = sp * round_up(tb * bn * kc_nat * 2, 1024);
             const int sbr = (budget - 2 * mg * nhA * a_half) / chunk;
@@ -663,9 +651,8 @@ static void fill_conv_params(v2v_plan* P, GOp& op) {
       }
     }
   }
-  // Commit groups.  Measured on B200: every tcgen05.commit / barrier round trip costs the issuing warp ~500 cycles
-  // during which the tensor pipe idles (its queue is shallow), so CG consecutive K-loop steps share one barrier pair;
-  // a step issues R * kmma MMAs of max(40, BN/2) cycles each (smem operand fetch floors small-N MMAs at ~40 cycles).
+  // Commit groups: CG consecutive K-loop steps share one barrier pair and one wgmma commit group, so that the barrier
+  // round trips are paid once per group; `est` is a step's MMA work in cycle-like units (small-N MMAs are floored).
   if (!kp.ring2) {
     const int slot = kp.MG * kp.a_slot_bytes + (kp.b_resident ? 0 : kp.b_slot_bytes);
     const int avail = budget - (kp.b_resident ? nB * kp.b_slot_bytes : 0);
@@ -870,30 +857,17 @@ static int build_backward_units(v2v_plan* P, cudaStream_t stream) {
           w.taps[ky * c.kw + kx] = s2 ? WgradTap{(int8_t)(((ky & 1) << 1) | (kx & 1)), (int8_t)(ky >> 1), (int8_t)(kx >> 1), 0}
                                       : WgradTap{0, (int8_t)ky, (int8_t)kx, 0};
       V2V_REQUIRE(!s2 || a_in.parity, V2V_ERR_STATE, "internal: stride-2 weight gradient needs a parity-plane operand");
-      // Measured (profiles/r02i_wgrad_layers.txt): an MN-major MMA (M = 128, K = 16) costs ~100 cycles for any N <= 128 and ~200
-      // at N = 256 -- half the K-major rate -- so this kernel is MMA-issue bound, not operand-traffic bound.  Two variants that
-      // only save operand traffic are therefore opt-in experiments:
-      //   * V2V_WG_KX=1: the kw taps of a filter row share one IN patch (kxr = kw): 1024->1024 98 -> 103 us, narrow 7x7 unchanged;
-      //   * V2V_WG_N256=1: 256-wide N tiles: 1024->1024 98 -> 99 us.
-      w.kxr = 1;
-      {
-        const char* ek = getenv("V2V_WG_KX");
-        const bool kx_on = ek && ek[0] == '1';
-        if (kx_on && u.mode == 1 && c.kw > 1 && kp + c.kw - 1 <= a_in.Wp && c.kw * std::max(32, w.BN) <= 512) w.kxr = c.kw;
-        const char* e2 = getenv("V2V_WG_N256");
-        if (w.kxr == 1 && aB.C >= 256 && e2 && e2[0] == '1') { w.BN = 256; w.Nblocks = 4; w.n_tiles = (aB.C + 255) / 256; }
-      }
       const int stage_bytes = (int)wgrad_stage_smem_bytes(w);
       w.stages = std::max(2, std::min(6, kSmemBudget / stage_bytes));
       w.chunks_total = w.N * w.gh * w.xsegs;
-      const int base_units = (w.ntaps / w.kxr) * w.m_tiles * w.n_tiles;
+      const int base_units = w.ntaps * w.m_tiles * w.n_tiles;
       const int want = std::max(1, (2 * device_sm_count() + base_units - 1) / base_units);
       w.chunks_per_unit = std::max(std::min(8, w.chunks_total), (w.chunks_total + want - 1) / want);
       w.ksplit = (w.chunks_total + w.chunks_per_unit - 1) / w.chunks_per_unit;
       // parameter gradient [R][Cc][taps]: rows = channels of OUT, columns = channels of IN
       u.M = u.mode == 2 ? c.Cin : c.Cout; u.M1 = u.mode == 2 ? c.Cin : c.Cout - c.Cout2; u.Nv = u.mode == 2 ? c.Cout : c.Cin;
       rc = make_tmap_act(&u.tmOut, a_out, kp, 1, std::min(a_out.C, 64)); if (rc) { P->bwd.push_back(u); return rc; }
-      rc = make_tmap_act(&u.tmIn, a_in, kp + w.kxr - 1, 1, std::min(a_in.C, 64)); if (rc) { P->bwd.push_back(u); return rc; }
+      rc = make_tmap_act(&u.tmIn, a_in, kp, 1, std::min(a_in.C, 64)); if (rc) { P->bwd.push_back(u); return rc; }
       u.wgrad = true;
       stage_max = std::max(stage_max, wgrad_stage_bytes(w));
     }
@@ -1458,7 +1432,7 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
             side.num_batches_tracked = reinterpret_cast<long long*>(op.norm.num_batches_tracked);
             side.scale = r.scale; side.shift = r.shift; side.mean_out = r.mean; side.rstd_out = r.rstd;
             if (first) {
-              // scale / shift come from the tail of the producing tcgen05 launch (last-CTA finalisation, conv_umma.cu); the
+              // scale / shift come from the tail of the producing tensor-core launch (last-CTA finalisation, conv_umma.cu); the
               // SIMT cross-check implementation and a third slice of one raw use a stats_finalize launch instead
               static const bool tail_ok = [] { const char* e = getenv("V2V_FUSED_FIN"); return !(e && e[0] == '0'); }();
               GOp& prod = P->gops[r.conv_op];

@@ -62,8 +62,8 @@ __global__ void __launch_bounds__(256) avgpool3s2_kernel(const float* __restrict
 }
 
 // W % 4 == 0: a thread produces two adjacent outputs from one 16-byte load (+ one scalar) per input row: 3x fewer load
-// instructions and twice the bytes in flight per thread (the scalar kernel above ran at 47 % of the copy rate, latency bound:
-// profiles/r02_hbm_ops_ncu.txt).  Same summation order -> same results.
+// instructions and twice the bytes in flight per thread (the scalar kernel above is latency bound).  Same summation order ->
+// same results.
 __global__ void __launch_bounds__(128) avgpool3s2_vec_kernel(const float* __restrict__ in, float* __restrict__ out, int P, int H, int W,
                                                              int Ho, int Wo) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;      // output pair index: outputs 2k, 2k + 1 read input columns 4k-1 .. 4k+3
@@ -130,7 +130,7 @@ __global__ void tensor2im_u8_kernel(const float* __restrict__ img, uint8_t* __re
 
 static inline int grid1d(size_t total) {
   size_t b = (total + 255) / 256;
-  const size_t cap = 148 * 16;
+  const size_t cap = 132 * 16;
   return (int)(b < cap ? (b ? b : 1) : cap);
 }
 

@@ -20,7 +20,7 @@ typedef __nv_bfloat16 bf16;
 //
 // Precise plans (split == 1, "bf16x3"): every value x is stored as the bf16 pair hi = bf16(x), lo = bf16(x - hi)
 // (16 mantissa bits together), a pixel holding [hi channels 0..C) | lo channels 0..C)]: 2*C bf16 per pixel.  The conv
-// kernel then accumulates A_hi*B_hi + A_lo*B_hi + A_hi*B_lo in fp32 (three tcgen05.mma per K block; the dropped lo*lo
+// kernel then accumulates A_hi*B_hi + A_lo*B_hi + A_hi*B_lo in fp32 (three wgmma per K block; the dropped lo*lo
 // term is 2^-18 relative), which makes the conv stack fp32-class while staying on the bf16 tensor pipe.
 struct ActDesc {
   bf16* base;
@@ -59,6 +59,9 @@ enum EpiMode { EPI_RAW_STATS = 0, EPI_HEAD_F32 = 1, EPI_ACT_BF16 = 2 };
 #define V2V_MAX_TAPS 64
 #define V2V_MAX_PHASES 4
 #define V2V_MAX_HEAD 16
+// widest accumulator of one conv work unit (MG * BN fp32 columns; conv_umma.cu keeps it in registers, two warpgroups
+// x 64 rows): wider units spill
+#define V2V_MAX_ACC_COLS 128
 
 // One "patch group": an A box (plane, dy, dx) that serves `R` consecutive taps (shifted by one
 // pixel = one 128-byte smem row each).  tap0 = index of the first tap in the packed weight matrix.
@@ -106,7 +109,7 @@ struct ConvKernelParams {
   int Cout, BN;                      // valid output channels, N tile (16/32/64/128)
   int Cp, cblocks;                   // padded input channels, K blocks per tap (Cp / kc)
   int kc, row_bytes, kmma;           // channels per K block (16/32/64), smem row bytes (2*kc), MMAs per row (kc/16)
-  int layout_type, sbo_bytes;        // UMMA smem-descriptor swizzle code (6/4/2) and 8-row group stride (8*row_bytes)
+  int layout_type, sbo_bytes;        // smem-descriptor swizzle code (6/4/2: 32B/64B/128B) and 8-row group stride (8*row_bytes)
   int R, RW;                         // taps served per A patch (1 = none); taps per patch row (tap r: row r / RW, column r % RW)
   int PW, PH;                        // patch extent in pixels (TMA box)
   int sbo_a_bytes;                   // A operand 8-row group stride: 8*row_bytes (row tiles) or PW*row_bytes (2-D patch)
@@ -150,7 +153,7 @@ struct ConvKernelParams {
   const float* bias;                 // may be null
   const float* bias2; int Cout1;     // fused heads: channels >= Cout1 take bias2[j - Cout1]
   int dbg;                           // timing experiments only (V2V_DBG): bit0 skip stats, bit1 skip output stores
-  int EG;                            // epilogue groups (4 warps each); EG > 1: group h owns TMEM accumulator stage h
+  int EG;                            // epilogue groups (always 1: both consumer warpgroups drain every tile)
   int grid;                          // CTAs launched (persistent); also the stats partial rows per (phase, image)
   // EPI_HEAD_F32: per output channel destination = io[head_slot] + head_off (+ n * head_bstride),
   // activation and scale.  Caller pointers are read from the device IO table at run time.
@@ -183,7 +186,7 @@ struct ApplyParams {
   ActDesc add[2];          // interior is read (any padding / parity)
   ActDesc out;
   int pad_mode;            // PadMode of out's halo
-  int fused;               // (unused: the block-prologue variant measured 2x slower than reading the arrays, profiles/README.md)
+  int fused;               // (unused: a block-prologue variant was slower than reading the arrays)
   int update_running;
   FinalizeParams fin;
 };

@@ -171,7 +171,7 @@ __global__ void resample_kernel(const float* __restrict__ img, const float* __re
 
 static inline int grid1d(size_t total) {
   size_t b = (total + 255) / 256;
-  const size_t cap = 148 * 16;
+  const size_t cap = 132 * 16;
   return (int)(b < cap ? (b ? b : 1) : cap);
 }
 

@@ -1,4 +1,4 @@
-// Weight gradient of a convolution on tcgen05 tensor cores (sm_100a): a GEMM whose K dimension is the PIXEL index,
+// Weight gradient of a convolution on Hopper tensor cores (sm_90a wgmma): a GEMM whose K dimension is the PIXEL index,
 //
 //   G[tap][m][n] = sum over grid pixels (img, y, x) of OUT[img][y][x][m] * IN[img][(y, x) @ tap][n]
 //
@@ -8,39 +8,40 @@
 // pixel being [hi C | lo C] bf16.  A TMA box of KP pixels x 64 channels lands in shared memory as KP rows of 128 bytes with
 // the 128-byte swizzle -- the canonical *MN-major* SWIZZLE_128B operand layout (64 contiguous M / N elements per K index,
 // 8-K groups 1024 bytes apart, 64-element blocks one box apart), so no transposed copy of any tensor is made: the same
-// bytes serve the forward conv K-major and this kernel MN-major.
+// bytes serve the forward conv K-major and this kernel MN-major (wgmma's transpose flags).
 //
-// One CTA per work unit (tap -- or, opt-in, the kw taps of a filter row --, M tile of 128 channels of one tensor, N tile of
-// 16 .. 128 (256) channels of the other, K split); the K loop walks row segments of KP pixels through a ring of
-// shared-memory stages.  Measured on B200: an MN-major MMA (M = 128, K = 16) costs ~100 cycles for any N <= 128, about half the
-// K-major rate, so the kernel is MMA-issue bound at 260-400 TFLOP/s algorithmic (x3 issued in precise plans) on the trunk layers.
-//   warp 0     TMA producer (one elected lane)
-//   warp 1     tcgen05.mma issuer (one elected lane) + TMEM owner; precise plans accumulate OUT_hi*IN_hi + OUT_lo*IN_hi +
-//              OUT_hi*IN_lo like the forward kernel
-//   warps 2-5  epilogue: tcgen05.ld the 128 x BN fp32 accumulator and add it to the staging buffer G (vector atomics: the K
-//              splits of one (tap, tile) meet there); unstage_wgrad_kernel then adds G into the caller's gradient tensor in
-//              the parameter's own layout [M][N][kh][kw].
+// One CTA per work unit (tap, M tile of 128 channels of one tensor, N tile of 16 .. 128 channels of the other, K split);
+// the K loop walks row segments of KP pixels through a ring of shared-memory stages.
+//   warps 0-7  two consumer warpgroups: warpgroup h accumulates rows [64 h, 64 h + 64) of the M tile (its 64-channel A
+//              block) in registers; precise plans accumulate OUT_hi*IN_hi + OUT_lo*IN_hi + OUT_hi*IN_lo like the forward
+//              kernel.  At the end each thread adds its accumulator fragment to the staging buffer G (vector atomics: the
+//              K splits of one (tap, tile) meet there); unstage_wgrad_kernel then adds G into the caller's gradient tensor
+//              in the parameter's own layout [M][N][kh][kw].
+//   warp 8     TMA producer (one elected lane)
 #include <cstdlib>
 #include "ptx.cuh"
+#include "wgmma.cuh"
 #include "v2v_internal.h"
 #include "backward.h"
 
 namespace v2v {
 
-static constexpr int kWgThreads = 192;
+static constexpr int kWgConsumers = 256;
+static constexpr int kWgThreads = kWgConsumers + 32;
 
 __device__ __forceinline__ uint64_t make_mnmajor_desc(uint32_t smem_addr, int lbo_bytes, int sbo_bytes, int layout_type) {
   // MN-major, swizzled: one K index = one shared-memory row of 128 / 64 / 32 bytes (64 / 32 / 16 contiguous M or N elements,
-  // layout type 2 / 4 / 6); SBO = distance between groups of 8 K indices (8 rows), LBO = distance between row-wide blocks
+  // layout type 2 / 4 / 6 as in make_kmajor_desc); SBO = distance between groups of 8 K indices (8 rows), LBO = distance
+  // between row-wide blocks
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
   d |= static_cast<uint64_t>(layout_type) << 61;
   return d;
 }
 
+template <int BN>
 __global__ void __launch_bounds__(kWgThreads, 1)
 wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmIn,
                   const __grid_constant__ WgradParams p) {
@@ -48,12 +49,7 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmOut, const __grid_consta
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   // A operand (M side, 128 rows of the accumulator): two 64-channel blocks of 128-byte rows.  B operand (N side): Nblocks
   // blocks of b_row bytes per pixel (128: 64 channels; 64 / 32: a 32- / 16-channel tensor in one block).
-  // kxr > 1 (stride-1 filters): a unit covers the kxr taps of one filter row.  The IN tensor is fetched once per chunk as a
-  // patch of KP + kxr - 1 pixels; tap kx reads it with the descriptor start advanced by kx pixel rows (rows are the K index of
-  // an MN-major operand; the swizzle applies to absolute address bits, so a row-shifted start stays consistent -- the same
-  // property the forward kernel's tap reuse rests on), each tap into its own accumulator columns.
-  const int pxA = p.KP + (p.swap ? p.kxr - 1 : 0), pxB = p.KP + (p.swap ? 0 : p.kxr - 1);
-  const int boxA = pxA * 128, boxB = pxB * p.b_row;               // bytes one TMA box delivers
+  const int boxA = p.KP * 128, boxB = p.KP * p.b_row;              // bytes one TMA box delivers
   const int blkA = (boxA + 1023) & ~1023, blkB = (boxB + 1023) & ~1023;      // block strides in shared memory (TMA destinations 1024-byte aligned)
   const int nh = p.split ? 2 : 1;
   const int a_half = 2 * blkA, b_half = p.Nblocks * blkB;
@@ -62,23 +58,17 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmOut, const __grid_consta
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * stage_bytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + p.stages;
-  uint64_t* acc_full = empty + p.stages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int BN = p.BN;
-  const int acc_cols = BN < 32 ? 32 : BN;                          // accumulator stride of one tap
-  uint32_t tmem_cols = 32;
-  while ((int)tmem_cols < p.kxr * acc_cols) tmem_cols <<= 1;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // (warp-uniform to the compiler)
+  const int n_consumer_warps = kWgConsumers / 32;
 
-  // unit -> (K split, tap group, M tile, N tile), tiles fastest: the CTAs running together walk the same pixel range, so every
+  // unit -> (K split, tap, M tile, N tile), tiles fastest: the CTAs running together walk the same pixel range, so every
   // operand row is fetched from HBM once and then served by L2 to the other (tap, tile) units
   int u = blockIdx.x;
   const int nt = u % p.n_tiles; u /= p.n_tiles;
   const int mt = u % p.m_tiles; u /= p.m_tiles;
-  const int ngroups = p.ntaps / p.kxr;
-  const int tap = (u % ngroups) * p.kxr;                           // first tap of the group
-  const int ks = u / ngroups;
+  const int tap = u % p.ntaps;
+  const int ks = u / p.ntaps;
   const int c_begin = ks * p.chunks_per_unit;
   const int c_end = min(p.chunks_total, c_begin + p.chunks_per_unit);
   const int nchunks = c_end - c_begin;                           // >= 1 by construction (launcher)
@@ -86,20 +76,12 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmOut, const __grid_consta
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmOut);
     tma_prefetch_desc(&tmIn);
-    for (int i = 0; i < p.stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(acc_full, 1);
+    for (int i = 0; i < p.stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], n_consumer_warps); }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, tmem_cols);
-    tmem_relinquish();
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == n_consumer_warps) {
     if (elect_one_sync()) {
       const WgradTap t = p.taps[tap];
       // swap == 0: A = OUT (gradient side, grid pixel itself), B = IN (activation side, shifted by the tap); swap == 1: the
@@ -130,62 +112,61 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmOut, const __grid_consta
         if (++xs == p.xsegs) { xs = 0; if (++y == p.gh) { y = 0; ++img; } }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one_sync()) {
-      const uint32_t idesc = make_idesc_bf16(128, BN) | (1u << 15) | (1u << 16);      // A and B MN-major
-      const int ps_step = p.split ? 1 : 3;
-      const int b_layout = p.b_row == 128 ? 2 : (p.b_row == 64 ? 4 : 6);
-      const int b_kstep = 16 * p.b_row, b_sbo = 8 * p.b_row;        // 16 pixels per MMA = two 8-row groups
-      const int a_shift = p.swap ? 128 : 0, b_shift = p.swap ? 0 : p.b_row;      // one pixel row of the IN patch per tap
-      int s = 0; uint32_t par = 0;
-      uint32_t first = 0;
-      for (int c = 0; c < nchunks; ++c) {
-        mbar_wait(&full[s], par);
-        tcgen05_fence_after();
-        const uint32_t a0 = smem_u32(smem + (size_t)s * stage_bytes), b0 = a0 + a_bytes;
-        for (int kx = 0; kx < p.kxr; ++kx) {
-          const uint32_t tmem_d = tmem_base + kx * acc_cols;
-          for (int ps = 0; ps < 3; ps += ps_step) {
-            const uint32_t a = a0 + (ps == 1 ? a_half : 0) + kx * a_shift, b = b0 + (ps == 2 ? b_half : 0) + kx * b_shift;
-            for (int k = 0; k < p.kmma; ++k)
-              umma_bf16(tmem_d, make_mnmajor_desc(a + k * 2048, blkA, 1024, 2), make_mnmajor_desc(b + k * b_kstep, blkB, b_sbo, b_layout), idesc,
-                        (first | (uint32_t)(ps > 0) | (uint32_t)(k > 0)) ? 1u : 0u);
+  } else {
+    const int wg = warp >> 2;                                     // A block (M half) of this warpgroup
+    const bool active = p.Mblocks == 2 || wg == 0;               // a 64-channel A tensor has no second half
+    const int ps_step = p.split ? 1 : 3;
+    const int b_layout = p.b_row == 128 ? 2 : (p.b_row == 64 ? 4 : 6);
+    const int b_kstep = 16 * p.b_row, b_sbo = 8 * p.b_row;        // 16 pixels per MMA = two 8-row groups
+    float acc[BN / 2];
+    int s = 0; uint32_t par = 0;
+    uint32_t first = 0;
+    int pend = -1;                                                // stage whose MMAs are still in flight
+    for (int c = 0; c < nchunks; ++c) {
+      mbar_wait_converged(&full[s], par);
+      if (active) {
+        wgmma_fence_operands(acc);
+        wgmma_fence();
+        const uint32_t a0 = smem_u32(smem + (size_t)s * stage_bytes) + wg * blkA, b0 = smem_u32(smem + (size_t)s * stage_bytes) + a_bytes;
+        for (int ps = 0; ps < 3; ps += ps_step) {
+          const uint32_t a = a0 + (ps == 1 ? a_half : 0), b = b0 + (ps == 2 ? b_half : 0);
+          for (int k = 0; k < p.kmma; ++k) {
+            Wgmma<BN>::template mma<1, 1>(acc, make_mnmajor_desc(a + k * 2048, blkA, 1024, 2), make_mnmajor_desc(b + k * b_kstep, blkB, b_sbo, b_layout),
+                                          first);
+            first = 1u;
           }
         }
-        first = 1u;
-        umma_commit(&empty[s]);
-        if (++s == p.stages) { s = 0; par ^= 1; }
+        wgmma_commit();
+        wgmma_wait<1>();                                          // the previous stage's MMAs have retired
       }
-      umma_commit(acc_full);
+      __syncwarp();
+      mbar_arrive_if(&empty[pend < 0 ? 0 : pend], lane == 0 && pend >= 0);
+      pend = s;
+      if (++s == p.stages) { s = 0; par ^= 1; }
     }
-  } else {
-    const int q = warp & 3;                                       // TMEM lane quarter of this warp
-    const int row = q * 32 + lane;
-    const int m = mt * (p.Mblocks * 64) + row;
-    const bool valid = row < (p.Mblocks == 2 ? 128 : 64) && m < p.Mp;
-    mbar_wait(acc_full, 0);
-    tcgen05_fence_after();
-    const int n0 = nt * BN;
-    for (int kx = 0; kx < p.kxr; ++kx) {
-      float* dst = p.stage + ((size_t)(tap + kx) * p.Mp + (valid ? m : 0)) * p.Np + n0;
-      for (int c = 0; c < BN / 16; ++c) {
-        uint32_t r[16];
-        tmem_ld_32x32b_x16(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + kx * acc_cols + c * 16, r);
-        tmem_ld_wait();
-        if (valid) {
+    if (active) {
+      wgmma_wait<0>();
+      wgmma_fence_operands(acc);
+    }
+    __syncwarp();
+    mbar_arrive_if(&empty[pend < 0 ? 0 : pend], lane == 0 && pend >= 0);
+    if (active) {
+      // fragment (see wgmma.cuh): rows w * 16 + lane / 4 (+ 8) of this half, column pairs b * 8 + 2 (lane % 4)
+      const int n0 = nt * BN;
+      const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (n0 + c * 16 + j * 4 < p.Np)
-              atomicAdd(reinterpret_cast<float4*>(dst + c * 16 + j * 4),
-                        make_float4(__uint_as_float(r[j * 4]), __uint_as_float(r[j * 4 + 1]), __uint_as_float(r[j * 4 + 2]),
-                                    __uint_as_float(r[j * 4 + 3])));
+      for (int i = 0; i < 2; ++i) {
+        const int m = mt * (p.Mblocks * 64) + r0 + 8 * i;
+        if (m >= p.Mp) continue;
+        float* dst = p.stage + ((size_t)tap * p.Mp + m) * p.Np + n0;
+#pragma unroll
+        for (int b = 0; b < BN / 8; ++b) {
+          const int col = b * 8 + 2 * (lane & 3);
+          if (n0 + col < p.Np) atomicAdd(reinterpret_cast<float2*>(dst + col), make_float2(acc[b * 4 + i * 2], acc[b * 4 + i * 2 + 1]));
         }
       }
     }
   }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, tmem_cols);
 }
 
 // G[tap][m][n] -> parameter gradient [R][Cc][taps] (+=) with (row, column) = (m, n), or (n, m) when the operands were swapped;
@@ -204,12 +185,23 @@ __global__ void __launch_bounds__(256) unstage_wgrad_kernel(const float* __restr
   }
 }
 
+template <int BN>
+static cudaError_t launch_wgrad_bn(const CUtensorMap& tmOut, const CUtensorMap& tmIn, const WgradParams& p, int units, size_t smem, cudaStream_t s) {
+  static size_t configured = 0;
+  if (smem > configured) {
+    cudaError_t e = cudaFuncSetAttribute(wgrad_umma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    configured = smem;
+  }
+  wgrad_umma_kernel<BN><<<units, kWgThreads, smem, s>>>(tmOut, tmIn, p);
+  return cudaGetLastError();
+}
+
 size_t wgrad_stage_bytes(const WgradParams& p) { return (size_t)p.ntaps * p.Mp * p.Np * sizeof(float); }
 
 // shared memory of one pipeline stage (must match the kernel's layout)
 size_t wgrad_stage_smem_bytes(const WgradParams& p) {
-  const int pxA = p.KP + (p.swap ? p.kxr - 1 : 0), pxB = p.KP + (p.swap ? 0 : p.kxr - 1);
-  const size_t blkA = ((size_t)pxA * 128 + 1023) & ~(size_t)1023, blkB = ((size_t)pxB * p.b_row + 1023) & ~(size_t)1023;
+  const size_t blkA = ((size_t)p.KP * 128 + 1023) & ~(size_t)1023, blkB = ((size_t)p.KP * p.b_row + 1023) & ~(size_t)1023;
   return (size_t)(p.split ? 2 : 1) * (2 * blkA + p.Nblocks * blkB);
 }
 
@@ -218,22 +210,23 @@ cudaError_t launch_wgrad_umma(const CUtensorMap& tmOut, const CUtensorMap& tmIn,
   cudaError_t e = cudaMemsetAsync(p.stage, 0, wgrad_stage_bytes(p), s);
   if (e != cudaSuccess) return e;
   const size_t stage_bytes = wgrad_stage_smem_bytes(p);
-  const size_t smem = (size_t)p.stages * stage_bytes + 1024 + (2 * p.stages + 2) * sizeof(uint64_t);
-  static size_t configured = 0;
-  if (smem > configured) {
-    e = cudaFuncSetAttribute(wgrad_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    configured = smem;
-  }
-  const int units = (p.ntaps / p.kxr) * p.m_tiles * p.n_tiles * p.ksplit;
+  const size_t smem = (size_t)p.stages * stage_bytes + 1024 + 2 * p.stages * sizeof(uint64_t);
+  const int units = p.ntaps * p.m_tiles * p.n_tiles * p.ksplit;
   static const bool log = getenv("V2V_WG_LOG") != nullptr;        // one line per launch, to pair with a profiler's kernel list
-  if (log) fprintf(stderr, "wgrad kxr %d grid %dx%dx%d taps %d aC %d bC %d BN %d swap %d KP %d units %d (ksplit %d x %d chunks) R %d Cc %d\n", p.kxr, p.N, p.gh, p.gw,
+  if (log) fprintf(stderr, "wgrad grid %dx%dx%d taps %d aC %d bC %d BN %d swap %d KP %d units %d (ksplit %d x %d chunks) R %d Cc %d\n", p.N, p.gh, p.gw,
                    p.ntaps, p.a_C, p.b_C, p.BN, p.swap, p.KP, units, p.ksplit, p.chunks_per_unit, R, Cc);
-  wgrad_umma_kernel<<<units, kWgThreads, smem, s>>>(tmOut, tmIn, p);
+  switch (p.BN) {
+    case 16: e = launch_wgrad_bn<16>(tmOut, tmIn, p, units, smem, s); break;
+    case 32: e = launch_wgrad_bn<32>(tmOut, tmIn, p, units, smem, s); break;
+    case 64: e = launch_wgrad_bn<64>(tmOut, tmIn, p, units, smem, s); break;
+    case 128: e = launch_wgrad_bn<128>(tmOut, tmIn, p, units, smem, s); break;
+    default: return cudaErrorInvalidConfiguration;
+  }
+  if (e != cudaSuccess) return e;
   e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   const long long total = (long long)R * Cc * p.ntaps;
-  const int blocks = (int)std::min<long long>((total + 255) / 256, 148 * 16);
+  const int blocks = (int)std::min<long long>((total + 255) / 256, 132 * 16);
   unstage_wgrad_kernel<<<blocks, 256, 0, s>>>(p.stage, p.Mp, p.Np, p.swap, R, R1, Cc, p.ntaps, dw, dw2);
   return cudaGetLastError();
 }
@@ -268,7 +261,7 @@ __global__ void __launch_bounds__(256) fold_add_kernel(const float* __restrict__
 cudaError_t launch_fold_add(const float* src, int Cs, int PH, int PW, float* dx, int N, int H, int W, int C, int pad, int reflect,
                             cudaStream_t s) {
   const size_t total = (size_t)N * H * W * C;
-  const int blocks = (int)std::min<size_t>((total + 255) / 256, 148 * 16);
+  const int blocks = (int)std::min<size_t>((total + 255) / 256, 132 * 16);
   fold_add_kernel<<<blocks, 256, 0, s>>>(src, Cs, PH, PW, dx, N, H, W, C, pad, reflect);
   return cudaGetLastError();
 }

@@ -1,11 +1,11 @@
-"""B200 drop-ins for the reference optical-flow stack: FlowNet2 (models/flownet2_pytorch/models.py:30-160 with
+"""H100 drop-ins for the reference optical-flow stack: FlowNet2 (models/flownet2_pytorch/models.py:30-160 with
 FlowNetC / FlowNetS / FlowNetSD / FlowNetFusion, networks/*.py) and the vid2vid wrapper FlowNet
 (models/flownet.py:12-62) that turns it into the (flow, confidence) training targets.
 
 The torch.nn layers are parameter containers with the reference's state_dict keys (pinned by
 tests/golden/flownet2_keys.json, the reference's own 220 keys / 162,518,834 parameters), so
 FlowNet2_checkpoint.pth.tar loads unchanged.  forward() describes each sub-network once per input shape to the plan
-runtime (tcgen05 convolutions in the precise split-bf16 mode -- FlowNet2 has no norm layers to absorb operand rounding --
+runtime (wgmma convolutions in the precise split-bf16 mode -- FlowNet2 has no norm layers to absorb operand rounding --
 bias + LeakyReLU(0.1) units, channel concatenation, the correlation op) and chains the plans with the stand-alone CUDA
 operators (resample2d, channelnorm, x4 upsampling).  There is no PyTorch / cuDNN fallback.
 """

@@ -1,6 +1,6 @@
-"""Vid2VidModelD on the B200 engine: the discriminator-side model of the training step (models/vid2vid_model_D.py:13-213)
+"""Vid2VidModelD on the H100 engine: the discriminator-side model of the training step (models/vid2vid_model_D.py:13-213)
 with the same initialize(opt) / forward(scale_T, tensors_list) / get_losses / loss_names, the towers running through the
-plan runtime (forward on tcgen05, hand-written backward kernels) and every loss term through libv2v_b200.so
+plan runtime (forward on wgmma, hand-written backward kernels) and every loss term through libv2v_b200.so
 (masked L1, LSGAN, feature matching, the two resample warps).  The VGG perceptual term needs downloaded weights and is
 outside the hot path (DESIGN.md section 5): `--no_vgg` is required, as in the oracle and the reference pin."""
 import torch

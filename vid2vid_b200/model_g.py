@@ -1,4 +1,4 @@
-"""Vid2VidModelG on the B200 engine: same public methods and per-clip state as
+"""Vid2VidModelG on the H100 engine: same public methods and per-clip state as
 models/vid2vid_model_G.py (initialize / encode_input / inference / generate_frame_infer /
 generate_first_frame / compute_mask / build_pyr), with every tensor op routed to libv2v_b200.so.
 

@@ -1,10 +1,10 @@
-"""B200 drop-ins for the generator / discriminator modules of models/networks.py.
+"""H100 drop-ins for the generator / discriminator modules of models/networks.py.
 
 Each class keeps the reference's constructor signature, attribute names and state_dict keys
 (index-based Sequential keys included, e.g. `model_down_img.4.weight`), so reference checkpoints load
 unchanged (models/base_model.py:63-107) -- the torch.nn layers below are *parameter containers*
 only.  forward() never calls them: it describes the network once per input shape to the plan
-runtime (vid2vid_b200/plan.py -> libv2v_b200.so), which runs hand-written sm_100a kernels.
+runtime (vid2vid_b200/plan.py -> libv2v_b200.so), which runs hand-written sm_90a kernels.
 There is no PyTorch/cuDNN fallback.
 
 Norm semantics (SURVEY App. B #1): Batch/InstanceNorm always use the statistics of the current
@@ -215,7 +215,7 @@ def emit_head_pair(plan, mods_a, dst_a, mods_b, dst_b, v):
 def emit_unit_pair(plan, mods_a, mods_b, v):
     """First units of two branches that read the same value with the same geometry (the 7x7 stems model_down_seg.1 and
     indv_down.1, networks.py:132,153) as ONE convolution with stacked weights; each half keeps its own norm layer.
-    The small-N 7x7 stems are MMA-issue bound (a 128 x N x 16 MMA costs ~40 cycles for any N <= 32), so sharing the
+    The small-N 7x7 stems are MMA-issue bound (a narrow MMA costs nearly what a wider one does), so sharing the
     instructions halves their cost.  Returns (value_a, value_b)."""
     (ua,), (ub,) = _units(mods_a), _units(mods_b)
     _, ca, pmode, pad, na, act_a, slope_a = ua

@@ -1,4 +1,4 @@
-"""The training step of train.py:50-93 on the B200 engine, one process per GPU.
+"""The training step of train.py:50-93 on the H100 engine, one process per GPU.
 
   * `FlatGrads`: every parameter's .grad is a view into ONE flat fp32 buffer laid out [G | D | D_T0 | ...]; a step issues a
     single NCCL all-reduce(SUM) / world over it (SURVEY 8e) -- the replacement of DataParallel's per-forward parameter
