@@ -23,7 +23,12 @@
 //                     Batch/InstanceNorm (deterministic fixed-point atomics)
 //     EPI_HEAD_F32  : bias + tanh/sigmoid/scale -> fp32 NCHW planes (the 7x7 image/flow/weight heads)
 //     EPI_ACT_BF16  : bias + (leaky)ReLU -> interior of the next layer's padded NHWC buffer
-//   warp 8      TMA producer (one elected lane)
+//   warps 8-11  producer warpgroup: one elected lane of warp 8 issues every TMA, warps 9-11 leave at once
+// Registers: the 384-thread block launches at 168 registers per thread (65536 / 384); setmaxnreg then lowers the
+// producer warpgroup to kProducerRegs and raises the two consumer warpgroups to kConsumerRegs (128 * 40 + 256 * 232 <=
+// 65536), so that the accumulators and the epilogue of every instantiation fit without spilling.
+// The kernel contains no call (no printf, no division slow path, see mbar_wait in ptx.cuh): ptxas would otherwise
+// serialise every wgmma, and the commit groups below would never overlap.
 #include <cstdlib>
 #include "ptx.cuh"
 #include "wgmma.cuh"
@@ -33,7 +38,8 @@
 namespace v2v {
 
 static constexpr int kConsumerThreads = 256;              // two warpgroups
-static constexpr int kThreads = kConsumerThreads + 32;    // + the producer warp
+static constexpr int kThreads = kConsumerThreads + 128;   // + the producer warpgroup
+static constexpr int kProducerRegs = 40, kConsumerRegs = 232;
 static constexpr int kStgStride = 65;                     // floats per staging row: row-wise and column-wise walks are conflict free
 static constexpr int kStgFloats = 128 * kStgStride;       // 128 pixel rows x 64 accumulator columns
 static constexpr int kRedFloats = 4 * 2 * 128;            // [warp quarter][sum|sumsq][128 columns] running column sums
@@ -43,7 +49,7 @@ __device__ __forceinline__ float apply_act(float v, int act, float slope) {
     case ACT_RELU: return fmaxf(v, 0.f);
     case ACT_LRELU: return v > 0.f ? v : v * slope;
     case ACT_TANH: return tanhf(v);
-    case ACT_SIGMOID: return 1.f / (1.f + __expf(-v));
+    case ACT_SIGMOID: return rcp_rn_ge1(1.f + __expf(-v));           // = 1 / (1 + e^-v) without a call
     default: return v;
   }
 }
@@ -124,7 +130,9 @@ __global__ void __launch_bounds__(kThreads, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ ConvKernelParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // 1024-byte aligned (SWIZZLE_128B); an offset from smem_raw rather than an integer round trip keeps every pointer below
+  // in the shared address space (32-bit addresses, LDS / STS) instead of generic 64-bit ones
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   // group slots: [SG][ CG activation patches | CG streamed weight slots ], then the resident weight set (if any)
   // ring2: [SG patch slots of MG tiles][SBr weight slots]
   const int slot_b = (p.b_resident || p.ring2) ? 0 : p.b_slot_bytes;
@@ -160,8 +168,9 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int b_tx = p.BN * p.row_bytes;
   const int t_first = blockIdx.x, t_step = gridDim.x;
 
-  if (warp == n_consumer_warps) {
-    if (elect_one_sync()) {
+  if (warp >= n_consumer_warps) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == n_consumer_warps && elect_one_sync()) {
       // ---------------------------------------------------------- TMA producer (single elected lane)
       // The K loop of a tile is a sequence of steps (tap group g, K block cb); CG consecutive steps share one
       // full/empty barrier pair ("group slot"), so a barrier round trip and a wgmma commit group are paid once per CG
@@ -249,6 +258,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
   } else {
     // ------------------------------------------------------------ consumers: wgmma issue + epilogue
+    setmaxnreg_inc<kConsumerRegs>();
     const int wg = warp >> 2;                             // M half of the tile this warpgroup multiplies
     const int q = warp & 3, hc = wg;                      // epilogue: pixel rows 32 q .. 32 q + 31, chunk parity hc
     const int row = q * 32 + lane;
@@ -351,7 +361,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int nsteps = (ph.group_end - ph.group_begin) * p.cblocks;
 
       // ---------------- MMAs
-      if (p.b_resident && first_of_key) mbar_wait_converged(bres_full, gen);
+      if (p.b_resident && first_of_key) mbar_wait(bres_full, gen);
 #pragma unroll
       for (int j = 0; j < MG; ++j) wgmma_fence_operands(acc[j]);
       wgmma_fence();
@@ -361,14 +371,14 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         // chunks from the B ring; tap r of the step reads the patch advanced by (r / RW) * PW + (r % RW) rows.
         const int RH = p.R / p.RW;
         for (int st = 0; st < nsteps; ++st) {
-          mbar_wait_converged(&g_full[as], apar);
+          mbar_wait(&g_full[as], apar);
           const uint32_t a_base16 = (smem_u32(sG + (size_t)as * p.MG * p.a_slot_bytes) & 0x3FFFF) >> 4;
           uint32_t bchunk16 = 0;
           int tin = 0, r = 0;
           for (int ky = 0; ky < RH; ++ky) {
             for (int kx = 0; kx < p.RW; ++kx, ++r) {
               if (tin == 0) {
-                mbar_wait_converged(&b_full[bs], bpar);
+                mbar_wait(&b_full[bs], bpar);
                 bchunk16 = ((sB_u32 + (uint32_t)bs * (uint32_t)p.b_slot_bytes) & 0x3FFFF) >> 4;
               }
               mma_tap<BN, MG>(acc, a_d0 + a_base16 + (uint32_t)ky * prow16 + (uint32_t)kx * row16, b_d0 + bchunk16 + (uint32_t)tin * b_step,
@@ -387,7 +397,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       } else {
         for (int s0 = 0; s0 < nsteps; s0 += p.CG) {
           const int n = min(p.CG, nsteps - s0);
-          mbar_wait_converged(&g_full[gs], gpar);
+          mbar_wait(&g_full[gs], gpar);
           const uint32_t base = smem_u32(sG + (size_t)gs * group_bytes);
           for (int i = 0; i < n; ++i) {
             const uint32_t b_base = p.b_resident ? sB_u32 + (s0 + i) * p.b_slot_bytes
@@ -561,19 +571,19 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     }
     if (do_stats && acc_key >= 0) flush();
-  }
 
-  __threadfence();                                  // this thread's statistics atomics are visible device-wide
-  __syncthreads();
-  if (p.n_fin > 0) {
-    // Statistics finalisation by the LAST CTA to get here (ticket counter, zeroed with the statistics rows before every run):
-    // all rows are complete then; every other CTA has exited, nobody waits.
-    if (threadIdx.x == 0) *ticket = atomicAdd(p.fin_counter, 1u);
-    __syncthreads();
-    if (*ticket == gridDim.x - 1) {
-      __threadfence();
-      for (int f = 0; f < p.n_fin; ++f)
-        for (int c = threadIdx.x; c < p.fin[f].C; c += blockDim.x) channel_side_effects(p.fin[f], c);
+    __threadfence();                                // this thread's statistics atomics are visible device-wide
+    if (p.n_fin > 0) {
+      // Statistics finalisation by the LAST CTA to get here (ticket counter, zeroed with the statistics rows before every
+      // run): all rows are complete then; every other CTA has exited, nobody waits.  Only the consumers wrote statistics.
+      named_bar_sync(1, kConsumerThreads);
+      if (threadIdx.x == 0) *ticket = atomicAdd(p.fin_counter, 1u);
+      named_bar_sync(1, kConsumerThreads);
+      if (*ticket == gridDim.x - 1) {
+        __threadfence();
+        for (int f = 0; f < p.n_fin; ++f)
+          for (int c = threadIdx.x; c < p.fin[f].C; c += kConsumerThreads) channel_side_effects(p.fin[f], c);
+      }
     }
   }
 }

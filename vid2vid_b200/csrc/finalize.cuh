@@ -1,7 +1,9 @@
 // Batch / instance-norm affine of ONE channel from the fixed-point statistics rows (see FinalizeParams): the few
 // double-precision operations sit in the mean / variance subtraction only.  Shared by the normalise pass prologue
-// (csrc/norm.cu) and the stand-alone stats_finalize_kernel.
+// (csrc/norm.cu), the stand-alone stats_finalize_kernel and the tail of conv_umma_kernel, which must stay call-free: the
+// divisions are div_rn_normal (ptx.cuh), whose operands here are counts and fixed-point sums, never near underflow.
 #pragma once
+#include "ptx.cuh"
 #include "v2v_internal.h"
 
 namespace v2v {
@@ -17,8 +19,8 @@ __device__ __forceinline__ ChannelAffine channel_affine(const FinalizeParams& p,
     q += (long long)__ldcg(p.stats + ((size_t)i * 2 + 1) * p.Cs + p.c_off + c);
   }
   const double cnt = p.count * (n1 - n0);
-  const double mean = (double)s * (1.0 / (double)V2V_STAT_SUM_SCALE) / cnt;
-  double var = (double)q * (1.0 / (double)V2V_STAT_SQ_SCALE) / cnt - mean * mean;
+  const double mean = div_rn_normal((double)s * (1.0 / (double)V2V_STAT_SUM_SCALE), cnt);
+  double var = div_rn_normal((double)q * (1.0 / (double)V2V_STAT_SQ_SCALE), cnt) - mean * mean;
   if (var < 0) var = 0;
   ChannelAffine a;
   a.rstd = rsqrtf((float)var + p.eps);
@@ -27,7 +29,7 @@ __device__ __forceinline__ ChannelAffine channel_affine(const FinalizeParams& p,
   a.scale = g * a.rstd;
   a.mean = (float)mean;
   a.shift = b - a.mean * a.scale;
-  a.var_unbiased = var * (cnt / (cnt > 1 ? cnt - 1 : 1));
+  a.var_unbiased = var * div_rn_normal(cnt, cnt > 1 ? cnt - 1 : 1);
   return a;
 }
 
@@ -49,8 +51,8 @@ __device__ __forceinline__ void channel_side_effects(const FinalizeParams& p, in
   }
   if (p.running_mean) {
     const float bias = p.conv_bias ? p.conv_bias[c] : 0.f;
-    p.running_mean[c] = (1.f - p.momentum) * p.running_mean[c] + p.momentum * ((float)(rm / p.N) + bias);
-    p.running_var[c] = (1.f - p.momentum) * p.running_var[c] + p.momentum * (float)(rv / p.N);
+    p.running_mean[c] = (1.f - p.momentum) * p.running_mean[c] + p.momentum * ((float)div_rn_normal(rm, p.N) + bias);
+    p.running_var[c] = (1.f - p.momentum) * p.running_var[c] + p.momentum * (float)div_rn_normal(rv, p.N);
     if (c == 0 && p.num_batches_tracked) *p.num_batches_tracked += 1;
   }
 }

@@ -123,7 +123,7 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmOut, const __grid_consta
     uint32_t first = 0;
     int pend = -1;                                                // stage whose MMAs are still in flight
     for (int c = 0; c < nchunks; ++c) {
-      mbar_wait_converged(&full[s], par);
+      mbar_wait(&full[s], par);
       if (active) {
         wgmma_fence_operands(acc);
         wgmma_fence();
