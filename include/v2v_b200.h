@@ -115,6 +115,11 @@ int v2v_mse_const_backward(const float* x, int64_t numel, float target, const fl
 int v2v_avgpool3s2_backward(const float* grad_out, float* grad_in, int P, int H, int W, v2v_stream_t stream);
 int v2v_resample_backward(const float* image, const float* flow, const float* grad_out, float* grad_image, float* grad_flow, int N,
                           int C, int H, int W, int align_corners, v2v_stream_t stream);
+/* AvgPool2d(2, stride=2, count_include_pad=False) on P planes: in (P,H,W) -> out (P,H/2,W/2) (floor; the `while
+ * x.size(3) > 1024` downsample of VGGLoss, models/networks.py:782-786), and its backward (grad_in written, zero on the rows /
+ * columns the floor drops). */
+int v2v_avgpool2(const float* in, float* out, int P, int H, int W, v2v_stream_t stream);
+int v2v_avgpool2_backward(const float* grad_out, float* grad_in, int P, int H, int W, v2v_stream_t stream);
 
 /* FlowNet2 glue (models/flownet2_pytorch/models.py:97-160, models/flownet.py:43-58), fp32 NCHW.
  * flownet_prep: the image pair -> x (B,6,H,W) = (pair - mean over both frames and all pixels, per sample and colour) / rgb_max,
@@ -217,6 +222,14 @@ int v2v_g_concat(v2v_plan* plan, const int* values, int n, int* value_out);
  * correlation kernel on plan-internal scratch.  kernel_size 1, stride1 1, pad_size == max_displacement only. */
 int v2v_g_correlation(v2v_plan* plan, int value_a, int value_b, int pad_size, int kernel_size, int max_displacement, int stride1,
                       int stride2, int act, float slope, int* value_out);
+/* value = MaxPool2d(2, stride 2)(value_in) (floor; VGG19's pools, models/networks.py:840-869).  Precise plans compare hi + lo
+ * and copy the winning pair; the backward routes the gradient to the first maximum of each window in row-major order. */
+int v2v_g_maxpool2(v2v_plan* plan, int value_in, int* value_out);
+/* io[slot][index] (fp32) = mean |x - y| over the (N, C, H, W) elements of two values of the same shape (nn.L1Loss of the VGG
+ * features, models/networks.py:788-790).  Deterministic (ordered partial sums).  The y operand is detached: the backward adds
+ * grad[index] / numel * sign(x - y) into x's gradient only, and values that only feed detached operands get no gradient
+ * buffer and no backward work. */
+int v2v_g_feature_l1(v2v_plan* plan, int value_x, int value_y, int slot, int index);
 /* Export a value as fp32 NCHW into the caller tensor bound to `slot`. */
 int v2v_g_export(v2v_plan* plan, int value, int slot);
 /* Fused warp / blend / fg composite on caller tensors (slots; -1 = absent).  s_raw is read (head output)
@@ -253,7 +266,8 @@ int v2v_plan_repack(v2v_plan* plan, v2v_stream_t stream);
 int v2v_plan_run(v2v_plan* plan, void* const* io_ptrs, int n_io, int use_graph, v2v_stream_t stream);
 
 /* Runs the plan once eagerly with a CUDA event after every kernel: kinds[i] (0 import, 1 conv, 2 raw-stats,
- * 3 stats-finalize, 4 norm-apply, 5 export, 6 composite), ms[i] device time, macs[i] algorithmic conv MACs. */
+ * 3 stats-finalize, 4 norm-apply, 5 export, 6 composite, 7 memset, 8 copy, 9 correlation, 10 max-pool, 11 feature L1),
+ * ms[i] device time, macs[i] algorithmic conv MACs. */
 int v2v_plan_profile(v2v_plan* plan, void* const* io_ptrs, int n_io, v2v_stream_t stream, int max_ops, int* kinds,
                      float* ms, double* macs, int* n_ops);
 

@@ -26,6 +26,8 @@ cudaError_t launch_mse_const_fwd(const float*, long long, float, double*, float*
 cudaError_t launch_mse_const_bwd(const float*, long long, float, const float*, float*, cudaStream_t);
 cudaError_t launch_avgpool3s2_bwd(const float*, float*, int, int, int, cudaStream_t);
 cudaError_t launch_resample_bwd(const float*, const float*, const float*, float*, float*, int, int, int, int, int, cudaStream_t);
+cudaError_t launch_avgpool2(const float*, float*, int, int, int, cudaStream_t);
+cudaError_t launch_avgpool2_bwd(const float*, float*, int, int, int, cudaStream_t);
 struct FgLabels { int v[16]; };
 cudaError_t launch_fg_mask(const float*, float*, int, int, int, int, int, int, FgLabels, int, cudaStream_t);
 }  // namespace v2v
@@ -193,6 +195,16 @@ int v2v_mse_const_backward(const float* x, int64_t numel, float target, const fl
 int v2v_avgpool3s2_backward(const float* grad_out, float* grad_in, int P, int H, int W, v2v_stream_t stream) {
   API_REQUIRE(grad_out && grad_in && P > 0 && H > 0 && W > 0, "avgpool3s2 backward: bad arguments");
   API_CUDA(launch_avgpool3s2_bwd(grad_out, grad_in, P, H, W, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+int v2v_avgpool2(const float* in, float* out, int P, int H, int W, v2v_stream_t stream) {
+  API_REQUIRE(in && out && P > 0 && H >= 2 && W >= 2, "avgpool2: bad arguments");
+  API_CUDA(launch_avgpool2(in, out, P, H, W, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+int v2v_avgpool2_backward(const float* grad_out, float* grad_in, int P, int H, int W, v2v_stream_t stream) {
+  API_REQUIRE(grad_out && grad_in && P > 0 && H >= 2 && W >= 2, "avgpool2 backward: bad arguments");
+  API_CUDA(launch_avgpool2_bwd(grad_out, grad_in, P, H, W, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
 int v2v_resample_backward(const float* image, const float* flow, const float* grad_out, float* grad_image, float* grad_flow, int N,

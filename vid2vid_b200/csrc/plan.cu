@@ -248,6 +248,7 @@ struct Value {
   float* gval = nullptr;     // training plans: gradient of the value, dense NHWC fp32 [N][H][W][C]
   int input_slot = -1;       // >= 0: the value is an import of that IO slot (data gradient only on request)
   bool exact_bf16 = false;   // caller promise: every element is exactly representable in bf16 (one-hot labels, edge maps)
+  bool detached = false;     // every consumer is a detached operand (or skipped in the backward): no gradient buffer
 };
 struct Raw {
   int N, H, W, C;
@@ -262,7 +263,7 @@ struct Raw {
   bool no_stats = false;           // backward sub-plans: the conv output feeds no norm layer
 };
 
-enum GKind { G_INPUT, G_CONV, G_NORM_ACT, G_CONV_ACT, G_HEAD, G_EXPORT, G_COMPOSITE, G_CONCAT, G_CORR, G_RAWIN };
+enum GKind { G_INPUT, G_CONV, G_NORM_ACT, G_CONV_ACT, G_HEAD, G_EXPORT, G_COMPOSITE, G_CONCAT, G_CORR, G_RAWIN, G_MAXPOOL, G_FEATL1 };
 struct GOp {
   GKind kind;
   // input
@@ -278,7 +279,8 @@ struct GOp {
   v2v_head_channel head[V2V_MAX_HEAD];
   CompositeParams comp{};
   std::vector<int> cat_in;   // G_CONCAT: source values in channel order
-  int value_in2 = -1;        // G_CORR: second operand
+  int value_in2 = -1;        // G_CORR: second operand; G_FEATL1: the (detached) target operand
+  int l1_index = 0;          // G_FEATL1: element of the output slot
   int corr[5] = {0, 0, 0, 0, 0};   // pad, kernel, max_disp, stride1, stride2
   const float* ext_raw = nullptr; int ext_C = 0;   // G_RAWIN: dense NHWC fp32 tensor owned by the parent plan (a gradient buffer)
   // backward sub-plans: pack the forward weights [Cout_f][Cin_f][kh][kw] (+ second set from output channel dg_Cout1 on) transposed
@@ -292,7 +294,7 @@ struct GOp {
   ConvKernelParams kp{};
 };
 
-enum XKind { X_IMPORT, X_CONV, X_RAWSTATS, X_FINALIZE, X_APPLY, X_EXPORT, X_COMPOSITE, X_MEMSET, X_COPY, X_CORR };
+enum XKind { X_IMPORT, X_CONV, X_RAWSTATS, X_FINALIZE, X_APPLY, X_EXPORT, X_COMPOSITE, X_MEMSET, X_COPY, X_CORR, X_MAXPOOL, X_FEATL1 };
 struct XOp {
   XKind kind;
   int gop = -1;
@@ -303,6 +305,8 @@ struct XOp {
   CompositeParams comp{};
   CopyParams copy{};
   CorrParams corr{};
+  PoolParams pool{};
+  FeatL1Params fl1{};
   RawDesc rawd{}; stat_t* stats = nullptr; int stats_C = 0;
   void* ms_ptr = nullptr; size_t ms_bytes = 0;
 };
@@ -349,6 +353,7 @@ struct v2v_plan {
   std::vector<GOp> gops;
   std::vector<ActDesc> acts;
   std::vector<int> act_pad_mode;
+  std::vector<char> op_live;    // per graph op: visited by the backward (0: all its outputs only feed detached operands)
   std::vector<XOp> xops;
   int n_slots = 0;
   double conv_macs = 0.0;
@@ -357,7 +362,7 @@ struct v2v_plan {
   // arena layout (size_arena) and device memory
   struct RawOff { size_t raw = 0, stats = 0, scale = 0, shift = 0; };
   bool sized = false, arena_owned = true;
-  std::vector<size_t> act_off, w_off, corr_off;
+  std::vector<size_t> act_off, w_off, corr_off, l1_off;
   std::vector<RawOff> raw_off;
   size_t stats_begin = 0, stats_end = 0;
   void* arena = nullptr; size_t arena_bytes = 0;
@@ -452,6 +457,40 @@ static Req conv_req(const v2v_conv_desc& c, const ConvGeom& g) {
   return r;
 }
 
+// Backward liveness.  A value all of whose consumers are detached operands (the target side of a feature L1), or ops that
+// are themselves skipped, gets no gradient buffer, and an op all of whose outputs are such values is skipped by the
+// backward (no data-gradient conv, no dY buffer).  Ops are in execution order, so walking them backwards sees every
+// consumer of a value before its producer.  Heads, exports, composites and feature L1 nodes feed outputs and always run.
+// A value that has no consumer at all keeps its gradient buffer: in a plan without feature L1 nodes every op stays live.
+static void mark_backward_liveness(v2v_plan* P) {
+  const size_t nv = P->values.size(), nr = P->raws.size();
+  std::vector<int> uses(nv, 0), raw_uses(nr, 0);
+  std::vector<char> live(nv, 0), raw_live(nr, 0);
+  auto dead = [&](int v) { return uses[v] > 0 && !live[v]; };
+  auto use = [&](int v, bool l) { if (v < 0) return; ++uses[v]; if (l) live[v] = 1; };
+  P->op_live.assign(P->gops.size(), 1);
+  for (int i = (int)P->gops.size() - 1; i >= 0; --i) {
+    const GOp& op = P->gops[i];
+    bool ol = true;
+    switch (op.kind) {
+      case G_INPUT: case G_RAWIN: case G_NORM_ACT: case G_CONV_ACT: case G_CONCAT: case G_CORR: case G_MAXPOOL:
+        ol = !dead(op.value_out); break;
+      case G_CONV: ol = !(raw_uses[op.raw] > 0 && !raw_live[op.raw]); break;
+      default: break;
+    }
+    P->op_live[i] = ol;
+    switch (op.kind) {
+      case G_CONV: case G_CONV_ACT: case G_HEAD: case G_EXPORT: case G_MAXPOOL: use(op.value_in, ol); break;
+      case G_NORM_ACT: ++raw_uses[op.raw]; if (ol) raw_live[op.raw] = 1; use(op.add[0], ol); use(op.add[1], ol); break;
+      case G_CONCAT: for (int v : op.cat_in) use(v, ol); break;
+      case G_CORR: use(op.value_in, ol); use(op.value_in2, ol); break;
+      case G_FEATL1: use(op.value_in, true); use(op.value_in2, false); break;
+      default: break;
+    }
+  }
+  for (size_t v = 0; v < nv; ++v) P->values[v].detached = dead((int)v);
+}
+
 // Host-only lowering: requirements, buffer descriptors (no addresses), kernel parameter skeletons.
 static int lower(v2v_plan* P) {
   if (P->lowered) return 0;
@@ -473,11 +512,14 @@ static int lower(v2v_plan* P) {
       P->values[op.value_in].interior_use = true;
     } else if (op.kind == G_CONCAT) {
       for (int v : op.cat_in) P->values[v].interior_use = true;
-    } else if (op.kind == G_CORR) {
+    } else if (op.kind == G_CORR || op.kind == G_FEATL1) {
       P->values[op.value_in].interior_use = true;
       P->values[op.value_in2].interior_use = true;
+    } else if (op.kind == G_MAXPOOL) {
+      P->values[op.value_in].interior_use = true;
     }
   }
+  mark_backward_liveness(P);
   for (auto& v : P->values) {
     if (v.reqs.empty()) { Req r{}; r.mode = PAD_NONE; v.reqs.push_back(r); }
     v.bufs.clear();
@@ -719,6 +761,8 @@ static int run_xop(v2v_plan* P, const XOp& x, cudaStream_t s) {
       V2V_CUDA(launch_correlation(x.corr.in1, x.corr.in2, x.corr.out, x.corr.N, x.corr.C, x.corr.H, x.corr.W, x.corr.pad, x.corr.k,
                                   x.corr.max_disp, x.corr.s1, x.corr.s2, s));
       break;
+    case X_MAXPOOL: V2V_CUDA(launch_maxpool2(x.pool, s)); break;
+    case X_FEATL1: V2V_CUDA(launch_feature_l1(x.fl1, s)); break;
     case X_CONV: {
       const GOp& op = P->gops[x.gop];
       if (P->impl == V2V_IMPL_UMMA) V2V_CUDA(launch_conv_umma(op.tmA, op.tmB, op.kp, s));
@@ -735,11 +779,24 @@ static int alloc_training(v2v_plan* P, cudaStream_t stream) {
   auto take = [&](size_t bytes) { size_t o = off; off = round_up_sz(off + bytes, 256); return o; };
   std::vector<size_t> vo(P->values.size()), ro(P->raws.size()), go(P->gops.size(), 0), so(P->n_slots, (size_t)-1);
   int cmax = 1, nmax = 1;
-  for (size_t i = 0; i < P->values.size(); ++i) { const Value& v = P->values[i]; vo[i] = take((size_t)v.N * v.H * v.W * v.C * 4); nmax = std::max(nmax, v.N); }
-  for (size_t i = 0; i < P->raws.size(); ++i) { const Raw& r = P->raws[i]; ro[i] = take(r.desc.elems() * 4); cmax = std::max(cmax, r.C); }
+  // (values and ops the backward skips, mark_backward_liveness, get no buffer)
+  const size_t none = (size_t)-1;
+  for (size_t i = 0; i < P->values.size(); ++i) {
+    const Value& v = P->values[i];
+    vo[i] = v.detached ? none : take((size_t)v.N * v.H * v.W * v.C * 4);
+    nmax = std::max(nmax, v.N);
+  }
+  for (size_t i = 0; i < P->raws.size(); ++i) {
+    const Raw& r = P->raws[i];
+    ro[i] = (r.conv_op >= 0 && !P->op_live[r.conv_op]) ? none : take(r.desc.elems() * 4);
+    cmax = std::max(cmax, r.C);
+  }
+  std::vector<char> has_gdz(P->gops.size(), 0);
   for (size_t i = 0; i < P->gops.size(); ++i) {
     const GOp& op = P->gops[i];
+    if (!P->op_live[i]) continue;
     if (op.kind == G_HEAD || op.kind == G_CONV_ACT) {
+      has_gdz[i] = 1;
       const Value& vin = P->values[op.value_in];
       go[i] = take((size_t)vin.N * op.geom.out_h * op.geom.out_w * round_up(op.conv.Cout, 8) * 4);   // channel stride: multiple of 8
       cmax = std::max(cmax, op.conv.Cout);
@@ -757,9 +814,9 @@ static int alloc_training(v2v_plan* P, cudaStream_t stream) {
   V2V_CUDA(cudaMalloc(&P->garena, P->garena_bytes));
   V2V_CUDA(cudaMemsetAsync(P->garena, 0, P->garena_bytes, stream));
   uint8_t* b = reinterpret_cast<uint8_t*>(P->garena);
-  for (size_t i = 0; i < P->values.size(); ++i) P->values[i].gval = reinterpret_cast<float*>(b + vo[i]);
-  for (size_t i = 0; i < P->raws.size(); ++i) P->raws[i].graw = reinterpret_cast<float*>(b + ro[i]);
-  for (size_t i = 0; i < P->gops.size(); ++i) if (go[i] || P->gops[i].kind == G_HEAD || P->gops[i].kind == G_CONV_ACT) P->gops[i].gdz = reinterpret_cast<float*>(b + go[i]);
+  for (size_t i = 0; i < P->values.size(); ++i) P->values[i].gval = vo[i] == none ? nullptr : reinterpret_cast<float*>(b + vo[i]);
+  for (size_t i = 0; i < P->raws.size(); ++i) P->raws[i].graw = ro[i] == none ? nullptr : reinterpret_cast<float*>(b + ro[i]);
+  for (size_t i = 0; i < P->gops.size(); ++i) if (has_gdz[i]) P->gops[i].gdz = reinterpret_cast<float*>(b + go[i]);
   P->gslot.assign(P->n_slots, nullptr);
   for (int sidx = 0; sidx < P->n_slots; ++sidx) if (so[sidx] != (size_t)-1) P->gslot[sidx] = reinterpret_cast<float*>(b + so[sidx]);
   P->gsums = reinterpret_cast<float*>(b + sums_off);
@@ -780,6 +837,7 @@ static int build_backward_units(v2v_plan* P, cudaStream_t stream) {
   for (size_t i = 0; i < P->gops.size(); ++i) {
     const GOp& op = P->gops[i];
     if (op.kind != G_CONV && op.kind != G_CONV_ACT && op.kind != G_HEAD) continue;
+    if (!P->op_live[i]) continue;                 // forward-only branch: no data-gradient sub-plan
     const v2v_conv_desc& c = op.conv;
     const Value& vin = P->values[op.value_in];
     const int oh = op.geom.out_h, ow = op.geom.out_w;
@@ -881,6 +939,15 @@ static int build_backward_units(v2v_plan* P, cudaStream_t stream) {
   return 0;
 }
 
+static FeatL1Params featl1_params(const v2v_plan* P, const GOp& op) {
+  FeatL1Params f{};
+  f.x = P->acts[P->values[op.value_in].bufs[0]]; f.y = P->acts[P->values[op.value_in2].bufs[0]];
+  f.Cvalid = P->values[op.value_in].C;
+  f.io = P->io_dev; f.slot = op.slot; f.index = op.l1_index;
+  f.blocks = feature_l1_blocks(f.x);
+  return f;
+}
+
 // Backward of one recorded forward (the plan's buffers still hold it).  Walks the graph ops in reverse.
 static int run_backward(v2v_plan* P, void* const* io, void* const* gio, const std::unordered_map<const void*, void*>& pg,
                         cudaStream_t s) {
@@ -934,7 +1001,20 @@ static int run_backward(v2v_plan* P, void* const* io, void* const* gio, const st
   };
   for (int i = (int)P->gops.size() - 1; i >= 0; --i) {
     const GOp& op = P->gops[i];
+    if (!P->op_live[i]) continue;
     switch (op.kind) {
+      case G_FEATL1: {
+        if (gio[op.slot]) {
+          const FeatL1Params fp = featl1_params(P, op);
+          V2V_CUDA(launch_feature_l1_bwd(fp, reinterpret_cast<const float*>(gio[op.slot]), P->values[op.value_in].gval, s));
+        }
+        break;
+      }
+      case G_MAXPOOL: {
+        PoolParams pp{P->acts[P->values[op.value_in].bufs[0]], P->acts[P->values[op.value_out].bufs[0]]};
+        V2V_CUDA(launch_maxpool2_bwd(pp, P->values[op.value_out].gval, P->values[op.value_in].gval, s));
+        break;
+      }
       case G_EXPORT: {
         const Value& v = P->values[op.value_in];
         if (gio[op.slot]) V2V_CUDA(launch_grad_import(reinterpret_cast<const float*>(gio[op.slot]), v.gval, v.N, v.C, 0, v.C, v.H, v.W, s));
@@ -1212,6 +1292,31 @@ int v2v_g_correlation(v2v_plan* p, int value_a, int value_b, int pad_size, int k
   return 0;
 }
 
+int v2v_g_maxpool2(v2v_plan* p, int value_in, int* value_out) {
+  V2V_REQUIRE(p && !p->lowered && value_out, V2V_ERR_STATE, "plan already lowered or null");
+  V2V_REQUIRE(value_in >= 0 && value_in < (int)p->values.size(), V2V_ERR_INVALID, "bad value id %d", value_in);
+  const Value a = p->values[value_in];
+  V2V_REQUIRE(a.H >= 2 && a.W >= 2, V2V_ERR_INVALID, "max-pool input %dx%d is smaller than its window", a.H, a.W);
+  GOp op; op.kind = G_MAXPOOL; op.value_in = value_in;
+  op.value_out = new_value(p, a.N, a.H / 2, a.W / 2, a.C);
+  p->gops.push_back(op);
+  *value_out = op.value_out;
+  return 0;
+}
+
+int v2v_g_feature_l1(v2v_plan* p, int value_x, int value_y, int slot, int index) {
+  V2V_REQUIRE(p && !p->lowered, V2V_ERR_STATE, "plan already lowered or null");
+  V2V_REQUIRE(value_x >= 0 && value_x < (int)p->values.size() && value_y >= 0 && value_y < (int)p->values.size() && value_x != value_y,
+              V2V_ERR_INVALID, "bad value ids %d, %d", value_x, value_y);
+  V2V_REQUIRE(slot >= 0 && index >= 0, V2V_ERR_INVALID, "bad output slot %d / index %d", slot, index);
+  const Value a = p->values[value_x], b = p->values[value_y];
+  V2V_REQUIRE(a.N == b.N && a.C == b.C && a.H == b.H && a.W == b.W, V2V_ERR_INVALID, "feature L1 operands differ in shape");
+  GOp op; op.kind = G_FEATL1; op.value_in = value_x; op.value_in2 = value_y; op.slot = slot; op.l1_index = index;
+  p->n_slots = std::max(p->n_slots, slot + 1);
+  p->gops.push_back(op);
+  return 0;
+}
+
 int v2v_g_export(v2v_plan* p, int value, int slot) {
   V2V_REQUIRE(p && !p->lowered, V2V_ERR_STATE, "plan already lowered or null");
   V2V_REQUIRE(value >= 0 && value < (int)p->values.size() && slot >= 0, V2V_ERR_INVALID, "bad export");
@@ -1277,6 +1382,12 @@ static int size_arena(v2v_plan* P) {
     if (P->gops[i].kind == G_CORR) {
       const Value& a = P->values[P->gops[i].value_in], &o = P->values[P->gops[i].value_out];
       P->corr_off[i] = take((2 * (size_t)a.N * a.C * a.H * a.W + (size_t)o.N * o.C * o.H * o.W) * sizeof(float));
+    }
+  P->l1_off.assign(P->gops.size(), 0);
+  for (size_t i = 0; i < P->gops.size(); ++i)
+    if (P->gops[i].kind == G_FEATL1) {
+      const Value& x = P->values[P->gops[i].value_in];
+      P->l1_off[i] = take((size_t)feature_l1_blocks(make_act(x, x.reqs[0], P->precise)) * sizeof(double));
     }
   // all norm-statistics rows live in one contiguous region that is zeroed at the start of every run
   P->stats_begin = off;
@@ -1487,6 +1598,23 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
         }
         break;
       }
+      case G_MAXPOOL: {
+        const Value& vo = P->values[op.value_out];
+        for (size_t m = 0; m < vo.bufs.size(); ++m) {
+          V2V_REQUIRE(P->act_pad_mode[vo.bufs[m]] != PAD_REFLECT, V2V_ERR_UNSUPPORTED, "max-pool output needs a zero / no halo");
+          XOp x; x.kind = X_MAXPOOL; x.gop = (int)i;
+          x.pool.in = P->acts[P->values[op.value_in].bufs[0]]; x.pool.out = P->acts[vo.bufs[m]];
+          P->xops.push_back(x);
+        }
+        break;
+      }
+      case G_FEATL1: {
+        XOp x; x.kind = X_FEATL1; x.gop = (int)i;
+        x.fl1 = featl1_params(P, op);
+        x.fl1.partials = reinterpret_cast<double*>(base + P->l1_off[i]);
+        P->xops.push_back(x);
+        break;
+      }
       case G_CORR: {
         const Value& va = P->values[op.value_in], &vb = P->values[op.value_in2], &vo = P->values[op.value_out];
         float* sa = reinterpret_cast<float*>(base + corr_off[i]);
@@ -1650,14 +1778,21 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
     snprintf(t, sizeof(t),
              "%s{\"kind\":%d,\"Cin\":%d,\"Cout\":%d,\"k\":[%d,%d],\"stride\":%d,\"transposed\":%d,\"in\":%d,\"TH\":%d,\"TW\":%d,"
              "\"R\":%d,\"groups\":%d,\"phases\":%d,\"grid\":[%d,%d],\"out\":[%d,%d],"
-             "\"BN\":%d,\"kc\":%d,\"MG\":%d,\"CG\":%d,\"SG\":%d,\"resident\":%d,\"EG\":%d,\"units\":%d,\"split\":%d,\"ring2\":%d,\"TB\":%d,\"SBr\":%d}",
+             "\"BN\":%d,\"kc\":%d,\"MG\":%d,\"CG\":%d,\"SG\":%d,\"resident\":%d,\"EG\":%d,\"units\":%d,\"split\":%d,\"ring2\":%d,\"TB\":%d,\"SBr\":%d,"
+             "\"grad\":%d}",
              first ? "" : ",", (int)op.kind, op.conv.Cin, op.conv.Cout, op.conv.kh, op.conv.kw, op.conv.stride, op.conv.transposed,
              op.value_in, g.TH, g.TW, g.R, g.n_groups, g.n_phases, g.grid_h, g.grid_w, g.out_h, g.out_w,
-             kp.BN, kp.kc, kp.MG, kp.CG, kp.SG, kp.b_resident, kp.EG, kp.total_units, kp.split, kp.ring2, kp.TB, kp.SBr);
+             kp.BN, kp.kc, kp.MG, kp.CG, kp.SG, kp.b_resident, kp.EG, kp.total_units, kp.split, kp.ring2, kp.TB, kp.SBr,
+             (int)P->op_live[&op - P->gops.data()]);
     s += t;
     first = false;
   }
-  snprintf(t, sizeof(t), "],\"conv_macs\":%.0f,\"n_slots\":%d}", P->conv_macs, P->n_slots);
+  // ops the backward visits (0 for the forward-only branch of a feature L1 target) and values without a gradient buffer
+  int bwd_ops = 0, detached = 0;
+  for (char l : P->op_live) bwd_ops += l;
+  for (const Value& v : P->values) detached += v.detached;
+  snprintf(t, sizeof(t), "],\"conv_macs\":%.0f,\"n_slots\":%d,\"ops\":%zu,\"backward_ops\":%d,\"detached_values\":%d}", P->conv_macs,
+           P->n_slots, P->gops.size(), bwd_ops, detached);
   s += t;
   if (buf && cap > 0) {
     size_t n = std::min((size_t)cap - 1, s.size());

@@ -249,6 +249,21 @@ struct CompositeParams {
   int use_warp;            // 0: img_final = img_raw (use_raw_only / no_flow)
 };
 
+// 2x2 / stride-2 max-pool (floor) between two activation buffers: out interior = max over each window of in's interior
+// (precise plans compare hi + lo and copy the winning pair)
+struct PoolParams {
+  ActDesc in, out;
+};
+// feature L1 (vgg.cu): io[slot][index] = mean |x - y| over the valid channels of two values of the same shape
+struct FeatL1Params {
+  ActDesc x, y;
+  int Cvalid;
+  void* const* io;
+  int slot, index;
+  double* partials;        // [blocks]: one ordered partial sum per block (no float atomics: replays are bit-identical)
+  int blocks;
+};
+
 cudaError_t launch_raw_stats(const RawDesc& raw, stat_t* stats, int stats_C, cudaStream_t stream);
 
 // x = hi + lo with hi = bf16(x), lo = bf16(x - hi)
@@ -266,6 +281,13 @@ cudaError_t launch_act_copy(const CopyParams& p, cudaStream_t stream);
 cudaError_t launch_bias_affine(float* scale, float* shift, const float* bias, int N, int C, int stride, cudaStream_t stream);
 cudaError_t launch_correlation(const float*, const float*, float*, int, int, int, int, int, int, int, int, int, cudaStream_t);
 cudaError_t launch_composite(const CompositeParams& p, cudaStream_t stream);
+cudaError_t launch_maxpool2(const PoolParams& p, cudaStream_t stream);
+// gin (dense NHWC fp32, in's logical extent and Cvalid channels) += gout routed to the first maximum of each window
+cudaError_t launch_maxpool2_bwd(const PoolParams& p, const float* gout, float* gin, cudaStream_t stream);
+cudaError_t launch_feature_l1(const FeatL1Params& p, cudaStream_t stream);
+// gx (dense NHWC fp32) += g[index] / numel * sign(x - y)
+cudaError_t launch_feature_l1_bwd(const FeatL1Params& p, const float* g, float* gx, cudaStream_t stream);
+int feature_l1_blocks(const ActDesc& x);
 int device_sm_count();
 
 

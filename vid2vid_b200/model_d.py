@@ -1,8 +1,8 @@
 """Vid2VidModelD on the H100 engine: the discriminator-side model of the training step (models/vid2vid_model_D.py:13-213)
 with the same initialize(opt) / forward(scale_T, tensors_list) / get_losses / loss_names, the towers running through the
 plan runtime (forward on wgmma, hand-written backward kernels) and every loss term through libv2v_b200.so
-(masked L1, LSGAN, feature matching, the two resample warps).  The VGG perceptual term needs downloaded weights and is
-outside the hot path (DESIGN.md section 5): `--no_vgg` is required, as in the oracle and the reference pin."""
+(masked L1, LSGAN, feature matching, the two resample warps) and the VGG19 perceptual loss (networks.VGGLoss: frozen VGG
+plans on the wgmma conv path, max-pool and feature-L1 nodes, backward into the generated image only)."""
 import torch
 import torch.nn as nn
 
@@ -33,8 +33,6 @@ class Vid2VidModelD(HostScheduleMixin, nn.Module):
         self.gpu_ids = opt.gpu_ids
         self.tD = opt.n_frames_D
         self.output_nc = opt.output_nc
-        if not opt.no_vgg:
-            raise NotImplementedError('VGG loss needs downloaded weights; run with --no_vgg (DESIGN.md section 5)')
         if getattr(opt, 'add_face_disc', False):
             raise NotImplementedError('face discriminator (edge2face demo) is out of scope')
         dev = torch.device('cuda', self.gpu_ids[0] if len(self.gpu_ids) else torch.cuda.current_device())
@@ -47,6 +45,8 @@ class Vid2VidModelD(HostScheduleMixin, nn.Module):
             setattr(self, 'netD_T' + str(s), networks.define_D(nc_t, opt.ndf, opt.n_layers_D, opt.norm, opt.num_D,
                                                                 not opt.no_ganFeat, []).to(dev))
         self.old_lr = opt.lr
+        if not opt.no_vgg:                  # :66-67 (frozen: in no optimizer and not in the trainer's flat gradient buffer)
+            self.criterionVGG = networks.VGGLoss(dev, synthetic=getattr(opt, 'synthetic_weights', False))
         self.loss_names = ['G_VGG', 'G_GAN', 'G_GAN_Feat', 'D_real', 'D_fake', 'G_Warp', 'F_Flow', 'F_Warp', 'W']
         self.loss_names_T = ['G_T_GAN', 'G_T_GAN_Feat', 'D_T_real', 'D_T_fake', 'G_T_Warp']
         beta1, beta2, lr = (0, 0.9, opt.lr * 2) if opt.TTUR else (opt.beta1, 0.999, opt.lr)        # :78-84
@@ -125,11 +125,13 @@ class Vid2VidModelD(HostScheduleMixin, nn.Module):
                 loss_W = ops.l1_loss(weight, None, conf_ref)                                                             # :128-130
         else:
             loss_F_Flow = loss_F_Warp = loss_W = torch.zeros_like(conf_ref)
-        loss_G_VGG = torch.zeros_like(loss_W)
+        loss_G_VGG = (self.criterionVGG(fake_B, real_B) * opt.lambda_feat) if not opt.no_vgg else torch.zeros_like(loss_W)  # :136
         loss_D_real, loss_D_fake, loss_G_GAN, loss_G_GAN_Feat = self.compute_loss_D(self.netD, real_A, real_B, fake_B)
         fake_B_warp_ref = self.resample(fake_B_prev, flow_ref)
         loss_G_Warp = ops.l1_loss(fake_B, fake_B_warp_ref.detach(), conf_ref) * opt.lambda_T                            # :139-140
         if fake_B_raw is not None:
+            if not opt.no_vgg:
+                loss_G_VGG = loss_G_VGG + self.criterionVGG(fake_B_raw, real_B) * opt.lambda_feat                         # :143-144
             r = self.compute_loss_D(self.netD, real_A, real_B, fake_B_raw)
             loss_D_real, loss_D_fake = loss_D_real + r[0], loss_D_fake + r[1]
             loss_G_GAN, loss_G_GAN_Feat = loss_G_GAN + r[2], loss_G_GAN_Feat + r[3]

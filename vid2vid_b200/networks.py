@@ -848,3 +848,174 @@ class SequentialRunner(_Planned):
         tplan = self._get_plan(key, x.device, lambda p: self._describe(p, N, C, H, W), train=True)
         (res,) = _PlanFunction.apply(self, tplan, [x, out], (0,), (1,), (0,), *([x] + list(self.parameters())))
         return res
+
+
+# ------------------------------------------------------------------------------------ VGG19 perceptual loss
+VGG19_FILE = 'vgg19-dcbb9e9d.pth'      # torchvision's ImageNet VGG19 checkpoint, as its hub cache names it
+_VGG_CFG = [64, 64, 'M', 128, 128, 'M', 256, 256, 256, 256, 'M', 512, 512, 512, 512, 'M', 512]   # -> features[0:30]
+_VGG_SLICES = ((0, 2), (2, 7), (7, 12), (12, 21), (21, 30))    # slice k ends at relu{k}_1 (models/networks.py:849-858)
+
+
+def vgg19_weights_path():
+    return os.path.join(torch.hub.get_dir(), 'checkpoints', VGG19_FILE)
+
+
+def vgg19_features():
+    """torchvision's vgg19().features[0:30] as a list: the same layers at the same indices (3x3 convs with zero padding 1 and
+    bias, ReLU, 2x2 max-pools).  Built with the global RNG state saved and restored: the weights are always replaced
+    (load_vgg19_weights), and turning the loss on must not change the initialisation of anything created after it."""
+    layers, c = [], 3
+    with torch.random.fork_rng(devices=[]):
+        for v in _VGG_CFG:
+            if v == 'M':
+                layers.append(nn.MaxPool2d(kernel_size=2, stride=2, padding=0, dilation=1, ceil_mode=False))
+            else:
+                layers += [nn.Conv2d(c, v, kernel_size=3, padding=1), nn.ReLU(inplace=True)]
+                c = v
+    return layers
+
+
+def load_vgg19_weights(vgg, synthetic=False, seed=0):
+    """Fill `vgg` (a Vgg19) from torchvision's cached ImageNet checkpoint, mapping its `features.{i}` keys to the slice keys.
+    Nothing is ever downloaded.  Without the file: a seeded torchvision-style init (kaiming-normal fan_out weights, zero
+    bias) when `synthetic`, FileNotFoundError otherwise."""
+    path = vgg19_weights_path()
+    if os.path.exists(path):
+        sd = torch.load(path, map_location='cpu', weights_only=True)
+        mapped = {}
+        for k, (a, b) in enumerate(_VGG_SLICES):
+            for i in range(a, b):
+                for leaf in ('weight', 'bias'):
+                    if 'features.%d.%s' % (i, leaf) in sd:
+                        mapped['slice%d.%d.%s' % (k + 1, i, leaf)] = sd['features.%d.%s' % (i, leaf)]
+        vgg.load_state_dict(mapped)
+        return vgg
+    if not synthetic:
+        raise FileNotFoundError('VGG19 weights not found at %s (torchvision\'s ImageNet VGG19 checkpoint); copy the file '
+                                'there, or set synthetic_weights for a seeded random init' % path)
+    return vgg19_synthetic_(vgg, seed)
+
+
+def vgg19_synthetic_(vgg, seed=0):
+    """Seeded torchvision-style init of a Vgg19 in place: kaiming-normal (fan_out, ReLU gain) weights, zero bias.  Depends only
+    on the seed (a private generator, the global RNG is untouched)."""
+    g = torch.Generator().manual_seed(seed)
+    with torch.no_grad():
+        for name, t in vgg.state_dict().items():
+            if name.endswith('.weight'):
+                fan_out = t.shape[0] * t.shape[2] * t.shape[3]
+                t.copy_(torch.randn(t.shape, generator=g) * (2.0 / fan_out) ** 0.5)
+            else:
+                t.zero_()
+    return vgg
+
+
+class Vgg19(_Planned):
+    """models/networks.py:840-869: slice1 .. slice5 of VGG19's features, frozen, with the reference's module tree and
+    state_dict keys (slice1.0.weight .. slice5.28.bias).  forward(X) returns the five relu{k}_1 maps; VGGLoss instead runs
+    feature_l1(x, y), which never leaves the plan's buffers.  Each conv is a bias + ReLU unit on the wgmma conv kernel, each
+    pool a max-pool node."""
+
+    def __init__(self, requires_grad=False):
+        super().__init__()
+        feats = vgg19_features()
+        for k, (a, b) in enumerate(_VGG_SLICES):
+            s = nn.Sequential()
+            for i in range(a, b):
+                s.add_module(str(i), feats[i])
+            setattr(self, 'slice%d' % (k + 1), s)
+        if not requires_grad:
+            for p in self.parameters():
+                p.requires_grad = False
+
+    def _branch(self, plan, v):
+        outs = []
+        for k in range(5):
+            for m in getattr(self, 'slice%d' % (k + 1)):
+                if isinstance(m, nn.Conv2d):
+                    v = plan.conv_act(v, conv_desc(m), L.ACT_RELU, 0.0)      # (the ReLU that follows is fused)
+                elif isinstance(m, nn.MaxPool2d):
+                    v = plan.maxpool2(v)
+            outs.append(v)
+        return outs
+
+    def _describe(self, plan, N, H, W):
+        """The loss plan: slot 0 = x, slot 1 = y (the target), slot 2 = (5,) fp32 per-level mean |x_k - y_k|.  Both branches
+        run the same frozen weights (packed once per branch); the y branch only feeds detached operands, so the backward
+        skips it entirely."""
+        fx = self._branch(plan, plan.input(0, N, 3, 0, 3, H, W))
+        fy = self._branch(plan, plan.input(1, N, 3, 0, 3, H, W))
+        for k in range(5):
+            plan.feature_l1(fx[k], fy[k], 2, k)
+
+    def _describe_features(self, plan, N, H, W):
+        for k, v in enumerate(self._branch(plan, plan.input(0, N, 3, 0, 3, H, W))):
+            plan.export(v, 1 + k)
+
+    @staticmethod
+    def feature_shapes(H, W):
+        shapes = []
+        for k, c in enumerate((64, 128, 256, 512, 512)):
+            shapes.append((c, H, W))
+            H, W = H // 2, W // 2
+        return shapes
+
+    def forward(self, X):
+        """The five feature maps (inference only: VGGLoss differentiates through feature_l1)."""
+        self._require_cuda(X)
+        if self._wants_grad(X):
+            raise NotImplementedError('Vgg19.forward has no backward; VGGLoss differentiates through Vgg19.feature_l1')
+        X = X.contiguous()
+        N, _, H, W = X.shape
+        plan = self._get_plan(('VGGF', N, H, W), X.device, lambda p: self._describe_features(p, N, H, W))
+        outs = [torch.empty((N, c, h, w), device=X.device, dtype=torch.float32) for c, h, w in self.feature_shapes(H, W)]
+        plan.run([X] + outs, self.use_cuda_graph)
+        return outs
+
+    def feature_l1(self, x, y):
+        """(5,) fp32 tensor of mean |vgg(x)_k - vgg(y)_k.detach()|, k = relu1_1 .. relu5_1.  Differentiable in x only."""
+        self._require_cuda(x, y)
+        x, y = x.contiguous(), y.detach().contiguous()
+        if x.shape != y.shape or x.dim() != 4 or x.shape[1] != 3:
+            raise ValueError('VGG inputs must be two (N, 3, H, W) tensors of the same shape, got %s and %s' % (tuple(x.shape), tuple(y.shape)))
+        N, _, H, W = x.shape
+        train = self._wants_grad(x)
+        plan = self._get_plan(('VGGL', N, H, W), x.device, lambda p: self._describe(p, N, H, W), train=train)
+        out = torch.empty(5, device=x.device, dtype=torch.float32)
+        io = [x, y, out]
+        if not train:
+            plan.run(io, self.use_cuda_graph)
+            return out
+        (res,) = _PlanFunction.apply(self, plan, io, (0,), (2,), (0, 1), *([x] + list(self.parameters())))
+        return res
+
+
+class AvgPool2(nn.Module):
+    """nn.AvgPool2d(2, stride=2, count_include_pad=False) on the engine (ops.avgpool2, autograd-aware)."""
+
+    kernel_size = stride = 2
+
+    def forward(self, x):
+        from . import ops
+        return ops.avgpool2(x)
+
+
+class VGGLoss(nn.Module):
+    """models/networks.py:776-791: sum_k w_k * mean |vgg(x)_k - vgg(y)_k.detach()| with w = 1/32 .. 1, the images halved by
+    a 2x2 mean while wider than 1024 pixels.  No ImageNet normalisation: the images go in as they are, in [-1, 1], as in
+    the reference.  `vgg`, `weights` and `downsample` have the reference's meaning."""
+
+    def __init__(self, gpu_id=0, synthetic=False, seed=0):
+        super().__init__()
+        self.vgg = load_vgg19_weights(Vgg19(), synthetic=synthetic, seed=seed).cuda(gpu_id)
+        self.weights = [1.0 / 32, 1.0 / 16, 1.0 / 8, 1.0 / 4, 1.0]
+        self.downsample = AvgPool2()
+
+    def forward(self, x, y):
+        while x.size()[3] > 1024:
+            x, y = self.downsample(x), self.downsample(y)
+        levels = self.vgg.feature_l1(x, y)
+        loss = 0
+        for i in range(len(self.weights)):
+            loss += self.weights[i] * levels[i]
+        return loss

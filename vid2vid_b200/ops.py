@@ -200,6 +200,40 @@ def _avgpool3s2_fwd(x):
     return out
 
 
+def _avgpool2_fwd(x):
+    x = x.contiguous()
+    _chk(x)
+    h, w = x.shape[-2:]
+    out = torch.empty(tuple(x.shape[:-2]) + (h // 2, w // 2), device=x.device, dtype=torch.float32)
+    with _on(x):
+        _ck(L.lib().v2v_avgpool2(_p(x), _p(out), x.numel() // (h * w), h, w, _st(x)))
+    return out
+
+
+class AvgPool2Function(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        ctx.shape = x.shape
+        return _avgpool2_fwd(x.detach())
+
+    @staticmethod
+    def backward(ctx, g):
+        h, w = ctx.shape[-2:]
+        g = g.contiguous()
+        gin = torch.empty(ctx.shape, device=g.device, dtype=torch.float32)
+        with _on(g):
+            _ck(L.lib().v2v_avgpool2_backward(_p(g), _p(gin), gin.numel() // (h * w), h, w, _st(g)))
+        return gin
+
+
+def avgpool2(x):
+    """AvgPool2d(2, stride=2, count_include_pad=False) over the last two dims (VGGLoss's downsample, networks.py:782-786);
+    autograd-aware."""
+    if torch.is_grad_enabled() and x.requires_grad:
+        return AvgPool2Function.apply(x)
+    return _avgpool2_fwd(x)
+
+
 def fg_mask(real_As, ts, fg_labels):
     """compute_mask (vid2vid_model_G.py:322-330): (b, T, C, h, w) -> (b, 1, h, w)."""
     real_As = real_As.contiguous()

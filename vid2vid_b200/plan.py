@@ -136,6 +136,16 @@ class Plan:
                                           C.byref(v)))
         return v.value
 
+    def maxpool2(self, vin):
+        v = C.c_int()
+        L.check(L.lib().v2v_g_maxpool2(self._h, vin, C.byref(v)))
+        return v.value
+
+    def feature_l1(self, vx, vy, slot, index):
+        """io[slot][index] = mean |x - y|; y is detached (no gradient, no backward work for what only feeds it)."""
+        L.check(L.lib().v2v_g_feature_l1(self._h, vx, vy, slot, index))
+        self.n_slots = max(self.n_slots, slot + 1)
+
     def export(self, v, slot):
         L.check(L.lib().v2v_g_export(self._h, v, slot))
         self.n_slots = max(self.n_slots, slot + 1)
