@@ -121,6 +121,27 @@ int v2v_resample_backward(const float* image, const float* flow, const float* gr
 int v2v_avgpool2(const float* in, float* out, int P, int H, int W, v2v_stream_t stream);
 int v2v_avgpool2_backward(const float* grad_out, float* grad_in, int P, int H, int W, v2v_stream_t stream);
 
+/* The edge2face first-frame generator's non-conv steps (models/vid2vid_model_G.py:231-320), deterministic (no float atomics).
+ * Both read the id map as floats and require every value to be an integer in range: anything else is V2V_ERR_INVALID
+ * (inside CUDA-graph capture the host cannot wait for the check: the affected outputs are NaN / chosen is -1 instead).
+ *   instance_mean: Encoder.forward's instance-wise average pooling (models/networks.py:617-632).  x, out (N,C,H,W) (out may
+ *     be x); inst (N,1,H,W) ids in [0, n_ids), n_ids <= V2V_MAX_INSTANCE_IDS.  out[n,c,p] = mean of x[n,c,q] over the pixels q
+ *     of image n with inst[n,q] == inst[n,p], summed in double and divided once.
+ *   face_features: get_face_features + dists_min (models/vid2vid_model_G.py:290-320, models/base_model.py:136-144).
+ *     pooled (N,feat_num,H,W) Encoder output; inst (N,1,H,W) labels in [0, n_labels); table (n_labels, max_rows, table_stride)
+ *     = features.npy packed per label (only the first feat_num columns are read); rows[n_labels] (host) = rows per label.
+ *     For each label present, feat_ori = pooled at its first pixel in flat (n, y, x) order; dists[m] = sum over present
+ *     labels and k of (feat_ori - table[label][m][k])^2 for m < num_images (absent labels contribute nothing); *chosen
+ *     (device int32) = the first minimum; out[n,k,p] = table[inst][min(chosen, rows[inst] - 1)][k].  A present label with
+ *     fewer than num_images rows is V2V_ERR_INVALID.  n_labels <= V2V_FACE_MAX_LABELS, feat_num <= V2V_FACE_MAX_FEAT. */
+#define V2V_MAX_INSTANCE_IDS 256
+#define V2V_FACE_MAX_LABELS 32
+#define V2V_FACE_MAX_FEAT 64
+int v2v_instance_mean(const float* x, const float* inst, float* out, int N, int C, int H, int W, int n_ids, v2v_stream_t stream);
+int v2v_face_features(const float* pooled, const float* inst, const float* table, const int* rows, int n_labels, int max_rows,
+                      int num_images, int feat_num, int table_stride, float* out, int* chosen, int N, int H, int W,
+                      v2v_stream_t stream);
+
 /* FlowNet2 glue (models/flownet2_pytorch/models.py:97-160, models/flownet.py:43-58), fp32 NCHW.
  * flownet_prep: the image pair -> x (B,6,H,W) = (pair - mean over both frames and all pixels, per sample and colour) / rgb_max,
  *   frame 0 in channels 0-2, frame 1 in 3-5 (models.py:97-103); x1 (may be NULL) = the frame-1 half as its own contiguous

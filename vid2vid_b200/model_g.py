@@ -83,25 +83,57 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
 
     # ------------------------------------------------------------------ first-frame generator
     def load_single_G(self):
-        """vid2vid_model_G.py:261-288.  The architecture per loadSize is the reference's; weights are
-        loaded from checkpoints/label2city_single/ (a missing file raises, as torch.load does in the reference) unless
-        opt.synthetic_weights is set (synthetic benchmarking has no checkpoints)."""
+        """vid2vid_model_G.py:261-288.  The architecture per dataset / loadSize is the reference's; weights are loaded from
+        checkpoints/label2city_single/ or checkpoints/edge2face_single/ (a missing file raises FileNotFoundError naming it, as
+        torch.load does in the reference) unless opt.synthetic_weights is set and the file is absent (synthetic benchmarking
+        has no checkpoints: seeded initialisation, and for the face model a seeded synthetic features table).  Nothing is
+        downloaded."""
         opt = self.opt
-        if 'City' not in opt.dataroot:
-            raise ValueError('Single image generator does not exist')
-        single_path = 'checkpoints/label2city_single/'
-        if opt.loadSize == 512:
-            load_path, netG = single_path + 'latest_net_G_512.pth', networks.define_G(35, 3, 0, 64, 'global', 3, 'instance', 0, [], opt)
-        elif opt.loadSize == 1024:
-            load_path, netG = single_path + 'latest_net_G_1024.pth', networks.define_G(35, 3, 0, 64, 'global', 4, 'instance', 0, [], opt)
-        elif opt.loadSize == 2048:
-            load_path, netG = single_path + 'latest_net_G_2048.pth', networks.define_G(35, 3, 0, 32, 'local', 4, 'instance', 0, [], opt)
+        if 'City' in opt.dataroot:
+            single_path = 'checkpoints/label2city_single/'
+            if opt.loadSize == 512:
+                load_path, netG = single_path + 'latest_net_G_512.pth', networks.define_G(35, 3, 0, 64, 'global', 3, 'instance', 0, [], opt)
+            elif opt.loadSize == 1024:
+                load_path, netG = single_path + 'latest_net_G_1024.pth', networks.define_G(35, 3, 0, 64, 'global', 4, 'instance', 0, [], opt)
+            elif opt.loadSize == 2048:
+                load_path, netG = single_path + 'latest_net_G_2048.pth', networks.define_G(35, 3, 0, 32, 'local', 4, 'instance', 0, [], opt)
+            else:
+                raise ValueError('Single image generator does not exist')
+        elif 'face' in opt.dataroot:
+            single_path = 'checkpoints/edge2face_single/'
+            load_path = single_path + 'latest_net_G.pth'
+            opt.feat_num = 16
+            netG = networks.define_G(15, 3, 0, 64, 'global_with_features', 3, 'instance', 0, [], opt)
+            self.netE = self._load(networks.define_G(3, 16, 0, 16, 'encoder', 4, 'instance', 0, []), single_path + 'latest_net_E.pth')
+            self.load_face_features(single_path + 'features.npy')
         else:
             raise ValueError('Single image generator does not exist')
-        if getattr(opt, 'synthetic_weights', False) and not os.path.exists(load_path):
-            return netG.to(self.device_)            # benchmarks / tests: random initialisation, stated in `data`
-        netG.load_state_dict(torch.load(load_path, map_location=self.device_))      # missing file raises, as the reference does
-        return netG.to(self.device_)
+        return self._load(netG, load_path)
+
+    def _load(self, net, path):
+        if not (getattr(self.opt, 'synthetic_weights', False) and not os.path.exists(path)):
+            if not os.path.exists(path):
+                raise FileNotFoundError('first-frame generator weights not found: %s' % path)
+            net.load_state_dict(torch.load(path, map_location=self.device_))
+        return net.to(self.device_)
+
+    def load_face_features(self, path='checkpoints/edge2face_single/features.npy', features=None):
+        """The nearest-neighbour table of get_face_features: `features` ({label: (rows, feat_num + 1)}) if given, else the
+        pickled dict at `path` -- read only from that local file, with np.load(encoding='latin1', allow_pickle=True), as the
+        reference reads it (vid2vid_model_G.py:295-296) -- else, with opt.synthetic_weights,
+        networks.synthetic_face_features(16 rows); otherwise FileNotFoundError naming the path.  Packed once onto the
+        device."""
+        if features is None:
+            if os.path.exists(path):
+                import numpy as np
+                features = np.load(path, encoding='latin1', allow_pickle=True).item()
+            elif getattr(self.opt, 'synthetic_weights', False):
+                features = networks.synthetic_face_features(16, self.opt.feat_num, seed=0)
+            else:
+                raise FileNotFoundError('face features table not found: %s' % path)
+        table, self.face_rows, self.face_num_images = networks.pack_face_features(features, self.opt.feat_num)
+        self.face_table = table.to(self.device_)
+        return features
 
     # ------------------------------------------------------------------ tensor helpers (CUDA kernels)
     def encode_input(self, input_map, real_image, inst_map=None):
@@ -114,9 +146,12 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
             input_map = ops.onehot_edges(input_map, inst, self.opt.label_nc, self.opt.use_instance)
         elif self.opt.use_instance:
             raise NotImplementedError('use_instance without label_nc')
+        pool_map = None
+        if self.opt.dataset_mode == 'face':
+            pool_map = inst_map.to(self.device_, torch.float32)
         if real_image is not None:
             real_image = real_image.to(self.device_, torch.float32)
-        return input_map, real_image, None
+        return input_map, real_image, pool_map
 
     def build_pyr(self, tensor):
         """base_model.py:122-134."""
@@ -136,10 +171,10 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
     def inference(self, input_A, input_B, inst_A):
         """vid2vid_model_G.py:198-209."""
         with torch.no_grad():
-            real_A, real_B, _ = self.encode_input(input_A, input_B, inst_A)
+            real_A, real_B, pool_map = self.encode_input(input_A, input_B, inst_A)
             self.is_first_frame = self.fake_B_prev is None
             if self.is_first_frame:
-                self.fake_B_prev = self.generate_first_frame(real_A, real_B)
+                self.fake_B_prev = self.generate_first_frame(real_A, real_B, pool_map)
             real_A = self.build_pyr(real_A)
             self.fake_B_feat = self.flow_feat = self.fake_B_fg_feat = None
             for s in range(self.n_scales):
@@ -158,6 +193,9 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         (computed on the device; util/util.py:48-71 does it on the CPU after copying the float frame back)."""
         import ctypes as C
         from . import _lib as L
+        if self.opt.dataset_mode == 'face' and self.use_single_G:
+            raise ValueError('inference_stream does not take the real frames that the face first-frame generator needs '
+                             '(use_single_G with dataset_mode face): use inference()')
         tG = self.opt.n_frames_G
         H, W = label_frame.shape[-2:]
         dev = self.device_
@@ -217,7 +255,10 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         elif self.opt.use_single_G:
             if self.opt.use_instance:
                 real_A = real_A[:, :, :self.opt.label_nc, :, :]
-            frames = [self.netG_i.forward(real_A[:, i].contiguous(), None).unsqueeze(1) for i in range(tG - 1)]
+            frames = []
+            for i in range(tG - 1):
+                feat_map = self.get_face_features(real_B[:, i], pool_map[:, i]) if self.opt.dataset_mode == 'face' else None
+                frames.append(self.netG_i.forward(real_A[:, i].contiguous(), feat_map).unsqueeze(1))
             fake_B_prev = torch.cat(frames, dim=1)
         else:
             raise ValueError('Please specify the method for generating the first frame')
@@ -225,6 +266,15 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         if not self.opt.isTrain:
             fake_B_prev = [B[0] for B in fake_B_prev]
         return fake_B_prev
+
+    def get_face_features(self, real_image, inst):
+        """vid2vid_model_G.py:290-320: the Encoder's pooled features, then the nearest row of the features table (over the
+        labels present in `inst`; absent labels do not count, where the reference reads uninitialised memory for them)
+        painted over the part map.  One chosen index per call, from the first occurrence of each label over the whole batch.
+        self.face_chosen keeps the (1,) int32 device tensor of the index."""
+        feat = self.netE.forward(real_image.contiguous(), inst.contiguous())
+        feat_map, self.face_chosen = ops.face_features(feat, inst.contiguous(), self.face_table, self.face_rows, self.face_num_images)
+        return feat_map
 
     # ------------------------------------------------------------------ training forward
     def init_train(self):

@@ -44,13 +44,19 @@ def get_norm_layer(norm_type='instance'):
 
 def define_G(input_nc, output_nc, prev_output_nc, ngf, which_model_netG, n_downsampling, norm, scale, gpu_ids=[],
              opt=[]):
-    """models/networks.py:32-59 (face-only `*_with_features` / `encoder` variants are out of scope)."""
+    """models/networks.py:32-59 (`local_with_features` is not built: no vid2vid code path uses it)."""
     norm_layer = get_norm_layer(norm_type=norm)
     if which_model_netG == 'global':
         netG = GlobalGenerator(input_nc, output_nc, ngf, n_downsampling, opt.n_blocks, norm_layer)
     elif which_model_netG == 'local':
         netG = LocalEnhancer(input_nc, output_nc, ngf, n_downsampling, opt.n_blocks, opt.n_local_enhancers,
                              opt.n_blocks_local, norm_layer)
+    elif which_model_netG == 'global_with_features':
+        netG = Global_with_z(input_nc, output_nc, opt.feat_num, ngf, n_downsampling, opt.n_blocks, norm_layer)
+    elif which_model_netG == 'encoder':
+        netG = Encoder(input_nc, output_nc, ngf, n_downsampling, norm_layer)
+    elif which_model_netG == 'local_with_features':
+        raise NotImplementedError('Generator model name [local_with_features] (Local_with_z) is not implemented')
     elif which_model_netG == 'composite':
         netG = CompositeGenerator(opt, input_nc, output_nc, prev_output_nc, ngf, n_downsampling, opt.n_blocks,
                                   opt.fg, opt.no_flow, norm_layer)
@@ -628,6 +634,141 @@ class GlobalGenerator(_Planned):
         out = torch.empty((N, self.output_nc, H, W), device=input.device, dtype=torch.float32)
         plan.run([input, out], self.use_cuda_graph)
         return out
+
+
+class Global_with_z(_Planned):
+    """models/networks.py:421-467: a pix2pixHD global generator whose nz-channel feature map z is concatenated in at four
+    places: with the input, in front of the residual blocks and of the upsampling path (z average-pooled n_downsample_G
+    times), and in front of the 7x7 tanh head.  One plan: the input-side concatenation is the caller's torch.cat, the
+    other three are concat nodes (forward only: the first-frame generator runs under no_grad)."""
+
+    def __init__(self, input_nc, output_nc, nz, ngf=64, n_downsample_G=3, n_blocks=9, norm_layer=nn.BatchNorm2d,
+                 padding_type='reflect'):
+        super().__init__()
+        self.n_downsample_G = n_downsample_G
+        self.input_nc, self.output_nc, self.nz = input_nc, output_nc, nz
+        cm = lambda c: min(1024, c)
+        model_downsample = _stem(input_nc + nz, ngf, norm_layer)
+        for i in range(n_downsample_G):
+            model_downsample += _down(cm(ngf * 2 ** i), cm(ngf * 2 ** (i + 1)), norm_layer)
+        mult = 2 ** n_downsample_G
+        model_resnet = [ResnetBlock(cm(ngf * mult) + nz, padding_type=padding_type, norm_layer=norm_layer) for _ in range(n_blocks)]
+        model_upsample = []
+        for i in range(n_downsample_G):
+            mult = 2 ** (n_downsample_G - i)
+            model_upsample += _up(cm(ngf * mult) + (nz * 2 if i == 0 else 0), cm(ngf * mult // 2), norm_layer)
+        self.model_downsample = nn.Sequential(*model_downsample)
+        self.model_resnet = nn.Sequential(*model_resnet)
+        self.model_upsample = nn.Sequential(*model_upsample)
+        self.model_upsample_conv = nn.Sequential(*_head(ngf + nz, output_nc, nn.Tanh()))
+        self.downsample = nn.AvgPool2d(3, stride=2, padding=[1, 1], count_include_pad=False)
+
+    def _z_dims(self, H, W):
+        for _ in range(self.n_downsample_G):
+            H, W = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+        return H, W
+
+    def _describe(self, plan, N, H, W):
+        """slot 0 = cat([x, z]) (N, input_nc + nz, H, W), slot 1 = z average-pooled n_downsample_G times, slot 2 = output."""
+        cin = self.input_nc + self.nz
+        v_xz = plan.input(0, N, cin, 0, cin, H, W)
+        v_z = plan.input(0, N, cin, self.input_nc, self.nz, H, W)
+        v_zd = plan.input(1, N, self.nz, 0, self.nz, *self._z_dims(H, W))
+        down = emit_seq(plan, self.model_downsample, v_xz)                              # :461
+        res = emit_seq(plan, self.model_resnet, plan.concat([down, v_zd]))              # :462
+        up = emit_seq(plan, self.model_upsample, plan.concat([res, v_zd]))              # :463
+        emit_head(plan, self.model_upsample_conv, plan.concat([up, v_z]), (2, self.output_nc, 1.0))   # :464
+
+    def forward(self, x, z):
+        from . import ops
+        self._require_cuda(x, z)
+        if self._wants_grad(x, z):
+            raise NotImplementedError('Global_with_z has no backward (the first-frame generator runs under no_grad)')
+        N, _, H, W = x.shape
+        if x.shape[1] != self.input_nc or tuple(z.shape) != (N, self.nz, H, W) or H % 2 ** self.n_downsample_G or W % 2 ** self.n_downsample_G:
+            raise ValueError('Global_with_z: x %s / z %s do not fit (%d + %d channels, sides divisible by %d)' % (
+                tuple(x.shape), tuple(z.shape), self.input_nc, self.nz, 2 ** self.n_downsample_G))
+        z = z.contiguous()
+        z_down = z
+        for _ in range(self.n_downsample_G):
+            z_down = ops.avgpool3s2(z_down)
+        xz = torch.cat([x, z], dim=1)
+        plan = self._get_plan(('GZ', N, H, W), x.device, lambda p: self._describe(p, N, H, W))
+        out = torch.empty((N, self.output_nc, H, W), device=x.device, dtype=torch.float32)
+        plan.run([xz, z_down, out], self.use_cuda_graph)
+        return out
+
+
+class Encoder(_Planned):
+    """models/networks.py:595-632: stem 7x7, n_downsampling stride-2 convs, as many transposed convs and a 7x7 tanh head
+    (InstanceNorm throughout), then the instance-wise average pooling over the id map `inst` (ops.instance_mean, in place on
+    the head output).  The ids must be integers in [0, n_ids): the face part maps hold 0 .. 6."""
+
+    n_ids = 7        # face parts (data/face_dataset.py); a larger value only costs another pass per 8 ids
+
+    def __init__(self, input_nc, output_nc, ngf=32, n_downsampling=4, norm_layer=nn.BatchNorm2d):
+        super().__init__()
+        self.input_nc, self.output_nc = input_nc, output_nc
+        model = _stem(input_nc, ngf, norm_layer)
+        for i in range(n_downsampling):
+            model += _down(ngf * 2 ** i, ngf * 2 ** (i + 1), norm_layer)
+        for i in range(n_downsampling):
+            mult = 2 ** (n_downsampling - i)
+            model += _up(ngf * mult, int(ngf * mult / 2), norm_layer)
+        model += _head(ngf, output_nc, nn.Tanh())
+        self.model = nn.Sequential(*model)
+
+    def _describe(self, plan, N, H, W):
+        mods = list(self.model)
+        v = emit_seq(plan, mods[:-3], plan.input(0, N, self.input_nc, 0, self.input_nc, H, W))
+        emit_head(plan, mods[-3:], v, (1, self.output_nc, 1.0))
+
+    def forward(self, input, inst):
+        from . import ops
+        self._require_cuda(input, inst)
+        if self._wants_grad(input):
+            raise NotImplementedError('Encoder has no backward (the face first frame runs under no_grad)')
+        input = input.contiguous()
+        N, _, H, W = input.shape
+        plan = self._get_plan(('E', N, H, W), input.device, lambda p: self._describe(p, N, H, W))
+        out = torch.empty((N, self.output_nc, H, W), device=input.device, dtype=torch.float32)
+        plan.run([input, out], self.use_cuda_graph)
+        return ops.instance_mean(out, inst.contiguous(), self.n_ids, out=out)
+
+
+# ------------------------------------------------------------------------------------ face features table
+FACE_LABELS = 7          # face parts of the edge2face part map (data/face_dataset.py)
+
+
+def synthetic_face_features(num_images, feat_num=16, seed=0, n_labels=FACE_LABELS):
+    """A seeded stand-in for checkpoints/edge2face_single/features.npy: {label: (num_images, feat_num + 1) array}, the
+    first feat_num columns uniform in [-1, 1] (the range of the Encoder's tanh means), the last (which the lookup never
+    reads) the row index.  The values are fp32-exact, stored as float64 (numpy float64 scalars are Python floats, which the
+    reference's element-wise copy into a FloatTensor accepts).  Depends only on the arguments."""
+    g = torch.Generator().manual_seed(seed)
+    out = {}
+    for label in range(n_labels):
+        f = torch.rand((num_images, feat_num), generator=g, dtype=torch.float64) * 2 - 1
+        out[label] = torch.cat([f, torch.arange(num_images, dtype=torch.float64)[:, None]], 1).float().double().numpy()
+    return out
+
+
+def pack_face_features(features, feat_num):
+    """features.npy's {label: (rows, feat_num + 1)} dict -> (table (n_labels, max_rows, feat_num + 1) fp32 CPU tensor, rows
+    per label, num_images).  num_images is features[6].shape[0], as the reference takes it (vid2vid_model_G.py:298)."""
+    labels = sorted(int(k) for k in features)
+    if labels != list(range(len(labels))):
+        raise ValueError('features table labels must be 0 .. n-1, got %s' % labels)
+    arrs = [torch.as_tensor(features[k], dtype=torch.float32) for k in labels]
+    if any(a.dim() != 2 or a.shape[1] < feat_num + 1 for a in arrs):
+        raise ValueError('features table rows need feat_num + 1 = %d columns' % (feat_num + 1))
+    rows = [a.shape[0] for a in arrs]
+    table = torch.zeros(len(arrs), max(rows), feat_num + 1)
+    for k, a in enumerate(arrs):
+        table[k, :a.shape[0]] = a[:, :feat_num + 1]
+    if len(rows) < FACE_LABELS:
+        raise ValueError('features table has %d labels; the face parts are %d' % (len(rows), FACE_LABELS))
+    return table, rows, rows[6]
 
 
 class LocalEnhancer(_Planned):

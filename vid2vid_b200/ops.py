@@ -4,6 +4,7 @@ operator surface (same class names / argument meaning / output-ownership rules):
   Correlation / Resample2d / ChannelNorm  <- models/flownet2_pytorch/networks/*_package/*.py
   resample(image, flow)                   <- BaseModel.resample (models/base_model.py:189-196)
   onehot_edges / avgpool3s2 / fg_mask     <- Vid2VidModelG.encode_input / build_pyr / compute_mask
+  instance_mean / face_features           <- Encoder.forward's pooling / Vid2VidModelG.get_face_features (edge2face)
 
 CUDA fp32 contiguous tensors only; errors from the library raise RuntimeError (the reference's
 wrapper raises via AT_ERROR, correlation_cuda.cc:81-83).  No CPU fallback.
@@ -232,6 +233,40 @@ def avgpool2(x):
     if torch.is_grad_enabled() and x.requires_grad:
         return AvgPool2Function.apply(x)
     return _avgpool2_fwd(x)
+
+
+def instance_mean(x, inst, n_ids, out=None):
+    """Encoder.forward's instance-wise average pooling (models/networks.py:617-632): x (N, C, H, W), inst (N, 1, H, W) float
+    ids, integers in [0, n_ids) (anything else raises).  Returns `out` (a new tensor, or x itself for an in-place pass) with
+    every value replaced by the mean of its channel over the pixels of its image that share its id.  Deterministic."""
+    _chk(x, inst, out)
+    N, C, H, W = x.shape
+    if inst.numel() != N * H * W:
+        raise ValueError('instance_mean: id map %s does not match features %s' % (tuple(inst.shape), tuple(x.shape)))
+    if out is None:
+        out = torch.empty_like(x)
+    with _on(x):
+        _ck(L.lib().v2v_instance_mean(_p(x), _p(inst), _p(out), N, C, H, W, int(n_ids), _st(x)))
+    return out
+
+
+def face_features(pooled, inst, table, rows, num_images):
+    """get_face_features's nearest-neighbour lookup (models/vid2vid_model_G.py:290-320): pooled (N, feat_num, H, W) Encoder
+    output, inst (N, 1, H, W) part labels, table (n_labels, max_rows, feat_num + 1) the packed features.npy, rows the
+    per-label row counts (host ints).  Returns (feat_map (N, feat_num, H, W), chosen (1,) int32 device tensor)."""
+    _chk(pooled, inst, table)
+    N, F_, H, W = pooled.shape
+    n_labels, max_rows, stride = table.shape
+    if inst.numel() != N * H * W or len(rows) != n_labels:
+        raise ValueError('face_features: part map %s / rows %d do not match features %s / table %s' % (
+            tuple(inst.shape), len(rows), tuple(pooled.shape), tuple(table.shape)))
+    out = torch.empty_like(pooled)
+    chosen = torch.empty(1, dtype=torch.int32, device=pooled.device)
+    arr = (C.c_int * n_labels)(*[int(r) for r in rows])
+    with _on(pooled):
+        _ck(L.lib().v2v_face_features(_p(pooled), _p(inst), _p(table), arr, n_labels, max_rows, int(num_images), F_, stride, _p(out),
+                                      C.c_void_p(chosen.data_ptr()), N, H, W, _st(pooled)))
+    return out, chosen
 
 
 def fg_mask(real_As, ts, fg_labels):
