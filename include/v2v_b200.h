@@ -120,6 +120,12 @@ int v2v_resample_backward(const float* image, const float* flow, const float* gr
  * columns the floor drops). */
 int v2v_avgpool2(const float* in, float* out, int P, int H, int W, v2v_stream_t stream);
 int v2v_avgpool2_backward(const float* grad_out, float* grad_in, int P, int H, int W, v2v_stream_t stream);
+/* Vid2VidModelD.get_face_region's pixel search (models/vid2vid_model_D.py:215-230) over the whole batch: real_A (N,C,H,W),
+ * C >= 3 (else V2V_ERR_INVALID).  Face pixels: real_A[:,2] > 0.9, or with openpose_only
+ * 0.19 < c0 < 0.21 && c1 < -0.99 && -0.61 < c2 < -0.59, compared in fp32 against the fp32-rounded constants.
+ * box: 5 device int32, reset by this call, then {found (0/1), ymin, ymax, xmin, xmax} of the face pixels (inclusive;
+ * {0, INT_MAX, -1, INT_MAX, -1} when none).  Deterministic (integer atomics). */
+int v2v_face_region(const float* real_A, int N, int C, int H, int W, int openpose_only, int* box, v2v_stream_t stream);
 
 /* The edge2face first-frame generator's non-conv steps (models/vid2vid_model_G.py:231-320), deterministic (no float atomics).
  * Both read the id map as floats and require every value to be an integer in range: anything else is V2V_ERR_INVALID

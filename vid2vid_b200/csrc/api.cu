@@ -28,6 +28,7 @@ cudaError_t launch_avgpool3s2_bwd(const float*, float*, int, int, int, cudaStrea
 cudaError_t launch_resample_bwd(const float*, const float*, const float*, float*, float*, int, int, int, int, int, cudaStream_t);
 cudaError_t launch_avgpool2(const float*, float*, int, int, int, cudaStream_t);
 cudaError_t launch_avgpool2_bwd(const float*, float*, int, int, int, cudaStream_t);
+cudaError_t launch_face_region(const float*, int, int, int, int, int, int*, cudaStream_t);
 struct FgLabels { int v[16]; };
 cudaError_t launch_fg_mask(const float*, float*, int, int, int, int, int, int, FgLabels, int, cudaStream_t);
 }  // namespace v2v
@@ -212,6 +213,12 @@ int v2v_resample_backward(const float* image, const float* flow, const float* gr
   API_REQUIRE(image && flow && grad_out && (grad_image || grad_flow), "resample backward: bad arguments");
   API_CUDA(launch_resample_bwd(image, flow, grad_out, grad_image, grad_flow, N, C, H, W, align_corners,
                                reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+int v2v_face_region(const float* real_A, int N, int C, int H, int W, int openpose_only, int* box, v2v_stream_t stream) {
+  API_REQUIRE(real_A && box && N > 0 && H > 0 && W > 0, "face_region: bad arguments");
+  API_REQUIRE(C >= 3, "face_region: the face predicate reads channels 0-2, got %d channels", C);
+  API_CUDA(launch_face_region(real_A, N, C, H, W, openpose_only, box, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
 

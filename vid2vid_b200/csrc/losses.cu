@@ -4,6 +4,9 @@
 //                criterionFeat) -- forward sum and backward in one pass each
 //   mse_const    mean (x - t)^2 against a constant label (GANLoss with use_lsgan, networks.py:764-774)
 //   avgpool3s2_bwd, resample_bwd  (gradients wrt image and flow of BaseModel.resample, base_model.py:189-196)
+//   face_region  the face bounding box the face discriminator crops (vid2vid_model_D.py:149-162,215-230)
+#include <climits>
+
 #include "ptx.cuh"
 #include "v2v_internal.h"
 
@@ -130,10 +133,61 @@ __global__ void resample_bwd_kernel(const float* __restrict__ img, const float* 
   }
 }
 
+// Face region of the pose demo's face discriminator (Vid2VidModelD.get_face_region, vid2vid_model_D.py:215-230): the bounding
+// box of the pixels of the whole batch that satisfy the face predicate, box = {found, ymin, ymax, xmin, xmax}.  The predicate
+// compares in fp32 against the fp32-rounded constants, as PyTorch compares an fp32 tensor with a Python float.  Each warp
+// reduces its pixels, each block combines its warps in shared memory, and one thread per block merges the block's box into
+// `box` with integer atomics: min / max / or, so the result does not depend on the order.
+__device__ __forceinline__ bool face_pixel(const float* p, size_t HW, int openpose_only) {
+  if (!openpose_only) return p[2 * HW] > 0.9f;
+  const float c0 = p[0], c1 = p[HW], c2 = p[2 * HW];
+  return c0 > 0.19f && c0 < 0.21f && c1 < -0.99f && c2 > -0.61f && c2 < -0.59f;
+}
+__global__ void face_region_reset_kernel(int* box) {
+  box[0] = 0; box[1] = INT_MAX; box[2] = -1; box[3] = INT_MAX; box[4] = -1;
+}
+__global__ void __launch_bounds__(256) face_region_kernel(const float* __restrict__ a, int N, int C, int H, int W, int openpose_only,
+                                                          int* box) {
+  __shared__ int s_box[5];
+  if (threadIdx.x == 0) { s_box[0] = 0; s_box[1] = INT_MAX; s_box[2] = -1; s_box[3] = INT_MAX; s_box[4] = -1; }
+  __syncthreads();
+  const size_t HW = (size_t)H * W, total = (size_t)N * HW;
+  int ymin = INT_MAX, ymax = -1, xmin = INT_MAX, xmax = -1;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t n = i / HW, pix = i - n * HW;
+    if (face_pixel(a + n * C * HW + pix, HW, openpose_only)) {
+      const int y = (int)(pix / W), x = (int)(pix - (size_t)y * W);
+      ymin = min(ymin, y); ymax = max(ymax, y); xmin = min(xmin, x); xmax = max(xmax, x);
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    ymin = min(ymin, __shfl_xor_sync(0xffffffffu, ymin, o));
+    ymax = max(ymax, __shfl_xor_sync(0xffffffffu, ymax, o));
+    xmin = min(xmin, __shfl_xor_sync(0xffffffffu, xmin, o));
+    xmax = max(xmax, __shfl_xor_sync(0xffffffffu, xmax, o));
+  }
+  if ((threadIdx.x & 31) == 0 && ymax >= 0) {
+    s_box[0] = 1;
+    atomicMin(s_box + 1, ymin); atomicMax(s_box + 2, ymax); atomicMin(s_box + 3, xmin); atomicMax(s_box + 4, xmax);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && s_box[0]) {
+    atomicOr(box, 1);
+    atomicMin(box + 1, s_box[1]); atomicMax(box + 2, s_box[2]); atomicMin(box + 3, s_box[3]); atomicMax(box + 4, s_box[4]);
+  }
+}
+
 static inline int grid1d(size_t total) {
   size_t b = (total + 255) / 256;
   const size_t cap = 132 * 8;
   return (int)(b < cap ? (b ? b : 1) : cap);
+}
+
+cudaError_t launch_face_region(const float* real_A, int N, int C, int H, int W, int openpose_only, int* box, cudaStream_t s) {
+  face_region_reset_kernel<<<1, 1, 0, s>>>(box);
+  face_region_kernel<<<grid1d((size_t)N * H * W), 256, 0, s>>>(real_A, N, C, H, W, openpose_only, box);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_l1_fwd(const float* a, const float* b, const float* m, int N, int C, int H, int W, double* sum_ws, float* out,

@@ -5,6 +5,7 @@ operator surface (same class names / argument meaning / output-ownership rules):
   resample(image, flow)                   <- BaseModel.resample (models/base_model.py:189-196)
   onehot_edges / avgpool3s2 / fg_mask     <- Vid2VidModelG.encode_input / build_pyr / compute_mask
   instance_mean / face_features           <- Encoder.forward's pooling / Vid2VidModelG.get_face_features (edge2face)
+  face_region                             <- Vid2VidModelD.get_face_region's pixel search (pose face discriminator)
 
 CUDA fp32 contiguous tensors only; errors from the library raise RuntimeError (the reference's
 wrapper raises via AT_ERROR, correlation_cuda.cc:81-83).  No CPU fallback.
@@ -267,6 +268,36 @@ def face_features(pooled, inst, table, rows, num_images):
         _ck(L.lib().v2v_face_features(_p(pooled), _p(inst), _p(table), arr, n_labels, max_rows, int(num_images), F_, stride, _p(out),
                                       C.c_void_p(chosen.data_ptr()), N, H, W, _st(pooled)))
     return out, chosen
+
+
+class FaceRegion:
+    """The face box of ops.face_region on its way to the host: one 20-byte copy into pinned memory, queued behind the
+    search kernel.  get() waits for that copy only (not for work queued after it) and returns (ymin, ymax, xmin, xmax) as
+    host ints, inclusive, or None when no pixel matched."""
+
+    def __init__(self, box):
+        self.host = torch.empty(5, dtype=torch.int32, pin_memory=True)
+        self.host.copy_(box, non_blocking=True)
+        self.event = torch.cuda.Event()
+        self.event.record(torch.cuda.current_stream(box.device))
+
+    def get(self):
+        self.event.synchronize()
+        found, ymin, ymax, xmin, xmax = self.host.tolist()
+        return (ymin, ymax, xmin, xmax) if found else None
+
+
+def face_region(real_A, openpose_only=False):
+    """The pixel search of Vid2VidModelD.get_face_region (models/vid2vid_model_D.py:215-230) over the whole batch real_A
+    (N, C >= 3, H, W): face pixels are real_A[:, 2] > 0.9, or with openpose_only 0.19 < c0 < 0.21, c1 < -0.99,
+    -0.61 < c2 < -0.59 (fp32 comparisons).  Launches the kernel and the copy of its result; returns a FaceRegion."""
+    real_A = real_A.contiguous()
+    _chk(real_A)
+    N, Ch, H, W = real_A.shape
+    box = torch.empty(5, dtype=torch.int32, device=real_A.device)
+    with _on(real_A):
+        _ck(L.lib().v2v_face_region(_p(real_A), N, Ch, H, W, int(bool(openpose_only)), C.c_void_p(box.data_ptr()), _st(real_A)))
+        return FaceRegion(box)
 
 
 def fg_mask(real_As, ts, fg_labels):
