@@ -87,13 +87,18 @@ TENSOR_UNITS = [
     ('t_head_tanh', lambda: NW._stem(8, 64, BN), (1, 8, 12, 40), lambda: NW._head(64, 3, nn.Tanh()), 1.0),
     ('t_head_flow', lambda: NW._stem(8, 128, BN), (1, 8, 12, 40), lambda: NW._head(128, 2), 20.0),
     ('t_head_both_narrow', lambda: NW._stem(8, 32, BN), (1, 8, 12, 40), lambda: NW._head(32, 3, nn.Tanh()), 1.0),       # dY padded to 64 channels
+    # training shapes of cfg3's coarse scale: enough (tap, M, N) units to fill the SMs without splitting K, so each unit walks
+    # every row chunk through the stage ring (1024 @ 32x64: ksplit 1, 32 chunks; 512 @ 64x128: ksplit 2, 64 chunks)
+    ('t_resblock1024_ksplit1', lambda: [NW.ResnetBlock(1024, 'reflect', BN)], (1, 1024, 32, 64)),
+    ('t_resblock512_64x128', lambda: [NW.ResnetBlock(512, 'reflect', BN)], (1, 512, 64, 128)),
 ]
 
 
 @pytest.mark.parametrize('unit', TENSOR_UNITS, ids=[u[0] for u in TENSOR_UNITS])
 def test_tensor_core_backward_units(unit, monkeypatch):
-    """Gradients of the tensor-core backward (data gradient as a forward conv + fold, weight gradient with pixels as the K
-    dimension) against fp64 autograd, and against the fp32 SIMT backward kernels of the same plan description."""
+    """The training plan's forward against fp64, then the gradients of the tensor-core backward (data gradient as a forward
+    conv + fold, weight gradient with pixels as the K dimension) against fp64 autograd, and against the fp32 SIMT backward
+    kernels of the same plan description."""
     name, build, shape = unit[:3]
     head, scale = (unit[3], unit[4]) if len(unit) > 3 else (None, 1.0)
     make = lambda: NW.SequentialRunner(build(), head(), scale) if head else NW.SequentialRunner(build())
@@ -101,6 +106,7 @@ def test_tensor_core_backward_units(unit, monkeypatch):
     runner = det_fill_(make(), seed=5).cuda()
     runner.precision = 'precise'
     names, ours, refs, out, ref = _grads(runner, x)
+    _cmp(name + ' forward', out.detach(), ref.detach(), tol=3e-4, l2=1e-4)
     monkeypatch.setenv('V2V_BWD', 'simt')
     simt = det_fill_(make(), seed=5).cuda()
     simt.precision = 'precise'
@@ -192,6 +198,7 @@ def test_head_gradients(name, build, head, scale, shape):
     runner.precision = 'precise'
     x = torch.randn(*shape, generator=torch.Generator().manual_seed(2)).cuda()
     names, ours, refs, out, ref = _grads(runner, x)
+    _cmp(name + ' forward', out.detach(), ref.detach(), tol=3e-4, l2=1e-4)
     for n, o, r in zip(names, ours, refs):
         if n.endswith('.bias') and r.abs().max().item() < 1e-6 * max(1.0, scale):
             continue

@@ -1779,11 +1779,11 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
              "%s{\"kind\":%d,\"Cin\":%d,\"Cout\":%d,\"k\":[%d,%d],\"stride\":%d,\"transposed\":%d,\"in\":%d,\"TH\":%d,\"TW\":%d,"
              "\"R\":%d,\"groups\":%d,\"phases\":%d,\"grid\":[%d,%d],\"out\":[%d,%d],"
              "\"BN\":%d,\"kc\":%d,\"MG\":%d,\"CG\":%d,\"SG\":%d,\"resident\":%d,\"EG\":%d,\"units\":%d,\"split\":%d,\"ring2\":%d,\"TB\":%d,\"SBr\":%d,"
-             "\"grad\":%d}",
+             "\"p2d\":%d,\"a_exact\":%d,\"headkx\":%d,\"grad\":%d}",
              first ? "" : ",", (int)op.kind, op.conv.Cin, op.conv.Cout, op.conv.kh, op.conv.kw, op.conv.stride, op.conv.transposed,
              op.value_in, g.TH, g.TW, g.R, g.n_groups, g.n_phases, g.grid_h, g.grid_w, g.out_h, g.out_w,
              kp.BN, kp.kc, kp.MG, kp.CG, kp.SG, kp.b_resident, kp.EG, kp.total_units, kp.split, kp.ring2, kp.TB, kp.SBr,
-             (int)P->op_live[&op - P->gops.data()]);
+             g.patch2d_kc > 0 ? 1 : 0, kp.a_exact, kp.headkx, (int)P->op_live[&op - P->gops.data()]);
     s += t;
     first = false;
   }

@@ -952,7 +952,8 @@ def build_netG(opt, s):
 class SequentialRunner(_Planned):
     """Runs a list of supported layer containers (conv / norm / activation units, ResnetBlocks, transposed
     convs; optionally a trailing small-Cout head) through the plan runtime: fp32 NCHW in -> fp32 NCHW out.
-    Used by the per-kernel parity tests and handy for porting other vid2vid sub-networks."""
+    Used by the per-kernel parity tests and handy for porting other vid2vid sub-networks.  The head is a Conv2d, optionally
+    behind a ReflectionPad2d and followed by an activation (the 7x7 image / flow heads, the discriminators' 4x4 logit layer)."""
 
     def __init__(self, mods, head_mods=None, head_scale=1.0):
         super().__init__()
@@ -960,11 +961,18 @@ class SequentialRunner(_Planned):
         self.head = nn.Sequential(*head_mods) if head_mods else None
         self.head_scale = head_scale
 
+    # As CompositeGenerator.input_exact_bf16: set only when every input element is exact in bf16 (one-hot labels, 0/1 edge
+    # maps); precise plans then skip the lo half of the input (two MMAs per K block of the first conv instead of three).
+    input_exact_bf16 = False
+
+    def _head_conv(self):
+        return next(m for m in self.head if isinstance(m, nn.Conv2d))
+
     def _describe(self, plan, N, C, H, W):
-        v = plan.input(0, N, C, 0, C, H, W)
+        v = plan.input(0, N, C, 0, C, H, W, exact_bf16=self.input_exact_bf16)
         v = emit_seq(plan, self.seq, v)
         if self.head is not None:
-            emit_head(plan, self.head, v, (1, self.head[1].out_channels, self.head_scale))
+            emit_head(plan, self.head, v, (1, self._head_conv().out_channels, self.head_scale))
         else:
             plan.export(v, 1)
 
@@ -972,13 +980,10 @@ class SequentialRunner(_Planned):
         self._require_cuda(x)
         x = x.contiguous()
         N, C, H, W = x.shape
-        key = ('SR', N, C, H, W)
+        key = ('SR', N, C, H, W, bool(self.input_exact_bf16))
         plan = self._get_plan(key, x.device, lambda p: self._describe(p, N, C, H, W))
         if self.head is not None:
-            oc, oh, ow = self.head[1].out_channels, H, W
-            if len(self.seq):
-                last = plan.describe()['values'][-1]
-                oh, ow = last['H'], last['W']
+            oc, (oh, ow) = self._head_conv().out_channels, plan.describe()['convs'][-1]['out']
         else:
             last = plan.describe()['values'][-1]
             oc, oh, ow = last['C'], last['H'], last['W']
