@@ -8,7 +8,8 @@
 //   norm_bwd     train-mode BatchNorm + (Leaky)ReLU backward (two passes: per-channel sums, then apply) and the norm-less
 //                bias + activation unit; residual / skip addends receive the incoming gradient
 //   head_bwd     tanh / sigmoid / scale heads: caller gradient planes (fp32 NCHW) -> dense NHWC dz
-//   composite_bwd  warp + blend + fg composite (networks.py:219-221,228-230): grads of raw, flow, weight, fg
+//   composite_bwd  warp + blend + fg composite (networks.py:219-221,228-230): grads of raw, flow, weight, fg and, when the
+//                caller asks for it, of the warped previous frame (grid_sample's input gradient, scattered with fp32 atomics)
 //   grad import / export between caller fp32 NCHW gradient tensors and the dense NHWC gradient buffers
 #include "ptx.cuh"
 #include "v2v_internal.h"
@@ -366,6 +367,13 @@ __device__ __forceinline__ Bil warp_coords_bwd(int x, int y, float fx, float fy,
   return b;
 }
 
+// PREV: also accumulate the gradient of the warped previous frame, grid_sample's input gradient of
+// g_final * (1 - mask) * (1 - weight), into the last three channels of d_prev.  Several pixels may sample the same source
+// pixel (all of them, at the border, when a flow leaves the frame) and there is no inverse map, so the four corner updates
+// are fp32 atomics: d_prev is reproducible to ~1e-7 relative, not bit for bit.  As ATen's safe_add_2d, a corner whose
+// contribution is zero (the clamped x1 / y1 at the border carry weight 0) issues no update.  Plans that need no img_prev
+// gradient run PREV = false, which is the kernel without that code.
+template <bool PREV>
 __global__ void __launch_bounds__(256) composite_bwd_kernel(CompositeBwd p) {
   const size_t HW = (size_t)p.H * p.W, total = (size_t)p.N * HW;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
@@ -403,6 +411,16 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(CompositeBwd p) {
         dfx += g * (1.f - w) * dwarp_dx * b.dsx;
         dfy += g * (1.f - w) * dwarp_dy * b.dsy;
         p.d_raw[((size_t)n * 3 + c) * HW + pix] = g * w + gr[c] * om;
+        if (PREV) {
+          float* dp = p.d_prev + ((size_t)n * p.prev_C + (p.prev_C - 3) + c) * HW;
+          const float gp = g * (1.f - w);
+          const float u00 = gp * ((1.f - b.wx) * (1.f - b.wy)), u01 = gp * (b.wx * (1.f - b.wy));
+          const float u10 = gp * ((1.f - b.wx) * b.wy), u11 = gp * (b.wx * b.wy);
+          if (u00 != 0.f) atomicAdd(dp + (size_t)b.y0 * p.W + b.x0, u00);
+          if (u01 != 0.f) atomicAdd(dp + (size_t)b.y0 * p.W + b.x1, u01);
+          if (u10 != 0.f) atomicAdd(dp + (size_t)b.y1 * p.W + b.x0, u10);
+          if (u11 != 0.f) atomicAdd(dp + (size_t)b.y1 * p.W + b.x1, u11);
+        }
       }
       p.d_weight[(size_t)n * HW + pix] = dw;
       p.d_flow[((size_t)n * 2) * HW + pix] = dfx;
@@ -552,7 +570,8 @@ cudaError_t launch_head_bwd(const HeadBwd& p, cudaStream_t s) {
   return cudaGetLastError();
 }
 cudaError_t launch_composite_bwd(const CompositeBwd& p, cudaStream_t s) {
-  composite_bwd_kernel<<<grid1d((size_t)p.N * p.H * p.W), 256, 0, s>>>(p);
+  if (p.d_prev && p.use_warp) composite_bwd_kernel<true><<<grid1d((size_t)p.N * p.H * p.W), 256, 0, s>>>(p);
+  else composite_bwd_kernel<false><<<grid1d((size_t)p.N * p.H * p.W), 256, 0, s>>>(p);
   return cudaGetLastError();
 }
 cudaError_t launch_grad_import(const float* g, float* dst, int N, int C_src, int c_off, int C, int H, int W, cudaStream_t s) {

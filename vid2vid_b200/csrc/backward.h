@@ -44,6 +44,7 @@ struct CompositeBwd {
   const float* raw; const float* flow; const float* weight; const float* prev; const float* mask;   // forward tensors (raw = head output)
   const float* g_final; const float* g_rawout;                                                      // incoming gradients (may be null)
   float* d_raw; float* d_flow; float* d_weight; float* d_fg;                                          // written
+  float* d_prev;   // img_prev gradient (fp32 NCHW, prev_C channels), accumulated into its last 3 channels; may be null
 };
 
 // Tensor-core weight gradient (csrc/wgrad_umma.cu): G[tap][m][n] = sum_pixels OUT[pixel][m] * IN[pixel @ tap][n]

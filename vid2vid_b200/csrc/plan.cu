@@ -1040,6 +1040,10 @@ static int run_backward(v2v_plan* P, void* const* io, void* const* gio, const st
         b.g_rawout = c.s_raw_out >= 0 ? reinterpret_cast<const float*>(gio[c.s_raw_out]) : nullptr;
         b.d_raw = P->gslot[c.s_raw]; b.d_flow = c.s_flow >= 0 ? P->gslot[c.s_flow] : nullptr;
         b.d_weight = c.s_weight >= 0 ? P->gslot[c.s_weight] : nullptr; b.d_fg = c.s_fg >= 0 ? P->gslot[c.s_fg] : nullptr;
+        // img_prev's gradient through the warp goes straight into the caller's (zero-filled) gradient tensor.  The slot's
+        // G_INPUT op precedes the composite in the graph, so this walk reaches it afterwards; its export of the stem's data
+        // gradient adds (+=) onto the warp term and must never overwrite it.
+        b.d_prev = (c.use_warp && c.s_prev >= 0) ? reinterpret_cast<float*>(gio[c.s_prev]) : nullptr;
         V2V_CUDA(launch_composite_bwd(b, s));
         break;
       }

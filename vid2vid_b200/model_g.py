@@ -5,6 +5,7 @@ generate_first_frame / compute_mask / build_pyr), with every tensor op routed to
 Inference only in this round (the reference's own `inference` runs under torch.no_grad,
 vid2vid_model_G.py:199); the training forward needs the backward kernels (DESIGN.md, next rows).
 """
+import contextlib
 import os
 
 import torch
@@ -283,12 +284,12 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         self.n_gpus = 1                                                    # one process per GPU (vid2vid_model_G.py:57-61 with n_gpus_gen = 1)
         self.n_frames_per_gpu = min(getattr(opt, 'max_frames_per_gpu', 1), opt.n_frames_total - opt.n_frames_G + 1)
         self.n_frames_load = self.n_gpus * self.n_frames_per_gpu
-        self.n_frames_bp = min(getattr(opt, 'max_frames_backpropagate', 1), self.n_frames_load)
-        self.finetune_all = True                                           # niter_fix_global == 0 (:66-68)
-        params = []
-        for s in range(self.n_scales):
-            params += list(getattr(self, 'netG' + str(s)).parameters())
-        beta1, beta2, lr = (0, 0.9, opt.lr / 2) if opt.TTUR else (opt.beta1, 0.999, opt.lr)       # :74-83
+        self.n_frames_bp = 1                                               # :58; update_training_batch raises it
+        # :66-72: with --niter_fix_global only the finest scale trains until update_fixed_params
+        self.finetune_all = getattr(opt, 'niter_fix_global', 0) == 0
+        scales = range(self.n_scales) if self.finetune_all else [self.n_scales - 1]
+        params = [p for s in scales for p in getattr(self, 'netG' + str(s)).parameters()]
+        beta1, beta2, lr = (0.0, 0.9, opt.lr / 2) if opt.TTUR else (opt.beta1, 0.999, opt.lr)       # :74-83
         self.old_lr = opt.lr
         self.optimizer_G = _adam(params, lr=lr, betas=(beta1, beta2))
         return self
@@ -328,14 +329,13 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
                 fake_B_prevs_reshaped = fake_B_prevs.reshape(bs, -1, h, w)
                 mask_F = self.compute_mask(real_As, t + tG - 1) if self.opt.fg else None
                 use_raw_only = self.opt.no_first_img and is_first_frame
-                fake_B, flow, weight, fake_B_raw, fake_B_feat, flow_feat, fake_B_fg_feat = getattr(self, 'netG' + str(s)).forward(
-                    real_As_reshaped, fake_B_prevs_reshaped, mask_F, fake_B_feat, flow_feat, fake_B_fg_feat, use_raw_only)
-                if s != n_scales - 1 and not self.finetune_all:
-                    fake_B, fake_B_feat = fake_B.detach(), fake_B_feat.detach()
-                    if flow is not None:
-                        flow, flow_feat = flow.detach(), flow_feat.detach()
-                    if fake_B_fg_feat is not None:
-                        fake_B_fg_feat = fake_B_fg_feat.detach()
+                # :181-186 detaches a frozen coarser scale's outputs; running it without autograd gives the same values from
+                # the inference plan (batch statistics and the running-statistics update included), with no saved
+                # statistics and no gradient buffers
+                frozen = s != n_scales - 1 and not self.finetune_all
+                with torch.no_grad() if frozen else contextlib.nullcontext():
+                    fake_B, flow, weight, fake_B_raw, fake_B_feat, flow_feat, fake_B_fg_feat = getattr(self, 'netG' + str(s)).forward(
+                        real_As_reshaped, fake_B_prevs_reshaped, mask_F, fake_B_feat, flow_feat, fake_B_fg_feat, use_raw_only)
                 fake_B_pyr[si] = cat(fake_B_pyr[si], fake_B.unsqueeze(1))
                 if s == n_scales - 1:
                     fake_Bs_raw = cat(fake_Bs_raw, fake_B_raw.unsqueeze(1))
