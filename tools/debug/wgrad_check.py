@@ -1,5 +1,5 @@
 """Tensor-core backward vs the fp32 SIMT backward on single conv units: per-tap / per-channel-block error of dW and the
-error of dX.  Usage: python tools/debug/wgrad_check.py [unit ...]   (V2V_WG_DESC=lbo,sbo overrides the descriptor strides)"""
+error of dX.  Usage: python tools/debug/wgrad_check.py [unit ...]"""
 import os, sys
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), '..', '..'))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))

@@ -33,5 +33,4 @@ for n in names:
             ms = [p[1] for p in prof if p[0] == 1]
             macs = [p[2] for p in prof if p[0] == 1]
             best = ms if best is None else [min(a, b) for a, b in zip(best, ms)]
-    print('%-14s dbg=%s eg=%s res=%s conv_ms=%s TF=%s' % (n, os.environ.get('V2V_DBG', '0'), os.environ.get('V2V_EG', '-'), os.environ.get('V2V_B_RESIDENT', '1'),
-          ['%.4f' % m for m in best], ['%.1f' % (2 * a / (m * 1e-3) / 1e12) for a, m in zip(macs, best)]), flush=True)
+    print('%-14s conv_ms=%s TF=%s' % (n, ['%.4f' % m for m in best], ['%.1f' % (2 * a / (m * 1e-3) / 1e12) for a, m in zip(macs, best)]), flush=True)

@@ -162,7 +162,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_prologue();          // everything above overlaps the previous kernel's tail; nothing above touches global memory
 
   const int a_tx = p.PW * p.PH * p.row_bytes;
   const int b_tx = p.BN * p.row_bytes;
@@ -273,7 +272,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const uint32_t a_wrap = (uint32_t)(((p.PW - p.RW) * p.row_bytes) >> 4);     // to the next patch row
     const uint32_t row16 = (uint32_t)(p.row_bytes >> 4), prow16 = (uint32_t)((p.PW * p.row_bytes) >> 4);
     const uint32_t sB_u32 = smem_u32(sBres);
-    const bool do_stats = (p.epi == EPI_RAW_STATS) && (p.stats != nullptr) && !(p.dbg & 1);
+    const bool do_stats = (p.epi == EPI_RAW_STATS) && (p.stats != nullptr);
     const int nchunks = p.BN / 32;
     const int tw_shift = __ffs(p.TW) - 1;                 // TW is a power of two
     const int ry = row >> tw_shift, rx = row & (p.TW - 1);
@@ -512,7 +511,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 v[j] = (col0 + j < p.Cout) ? apply_act(v[j] + b, p.act, p.lrelu_slope) : 0.f;
               }
             }
-            if (valid && !(p.dbg & 2)) {
+            if (valid) {
               if (dstf) {                                // precise plan: fp32 raw output
 #pragma unroll
                 for (int qv = 0; qv < 8; ++qv)
@@ -588,13 +587,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 }
 
-bool pdl_enabled() {
-  // opt-in (V2V_PDL=1): the early-launched blocks of the elementwise kernels sit in griddepcontrol.wait holding thread slots
-  // the persistent conv CTAs then wait for
-  static const bool on = [] { const char* e = getenv("V2V_PDL"); return e && e[0] == '1'; }();
-  return on;
-}
-
 int device_sm_count() {
   static int n = 0;
   if (!n) {
@@ -614,7 +606,8 @@ static cudaError_t launch_bn_mg(const CUtensorMap& tmA, const CUtensorMap& tmB, 
     if (e != cudaSuccess) return e;
     configured = smem;
   }
-  return launch_pdl(conv_umma_kernel<BN, MG>, dim3(p.grid), dim3(kThreads), smem, stream, tmA, tmB, p);
+  conv_umma_kernel<BN, MG><<<p.grid, kThreads, smem, stream>>>(tmA, tmB, p);
+  return cudaGetLastError();
 }
 
 size_t conv_umma_smem_bytes(const ConvKernelParams& p) {

@@ -23,7 +23,6 @@ __device__ __forceinline__ int reflect_i(int i, int n) {
 template <int CT>
 __global__ void __launch_bounds__(256) import_nchw_kernel(ImportParams p) {
   __shared__ float tile[CT][129];
-  pdl_prologue();
   const float* src = p.direct ? p.direct : reinterpret_cast<const float*>(p.io[p.slot]);
   const ActDesc& o = p.out;
   const int Wpad = o.W + o.pad_l + o.pad_r, Hpad = o.H + o.pad_t + o.pad_b;
@@ -97,7 +96,6 @@ __global__ void __launch_bounds__(256) import_nchw_kernel(ImportParams p) {
 // block (32, 8): tile of 128 x positions x 32 channels at one (n, y).
 __global__ void __launch_bounds__(256) export_nchw_kernel(ExportParams p) {
   __shared__ float tile[32][129];
-  pdl_prologue();
   float* dst = p.direct ? p.direct : reinterpret_cast<float*>(p.io[p.slot]);
   const ActDesc& a = p.in;
   const int xt = blockIdx.x * 128;
@@ -170,7 +168,6 @@ __global__ void pack_weights_kernel(PackParams p) {
 
 // torch.cat along channels: one thread per (padded pixel of out, source channel), channel fastest.
 __global__ void __launch_bounds__(256) act_copy_kernel(CopyParams p) {
-  pdl_prologue();
   const ActDesc& o = p.out;
   const ActDesc& a = p.in;
   const int Wpad = o.W + o.pad_l + o.pad_r, Hpad = o.H + o.pad_t + o.pad_b, C = a.Cvalid;
@@ -209,7 +206,8 @@ cudaError_t launch_act_copy(const CopyParams& p, cudaStream_t stream) {
   const size_t total = (size_t)p.out.N * (p.out.H + p.out.pad_t + p.out.pad_b) * (p.out.W + p.out.pad_l + p.out.pad_r) * p.in.Cvalid;
   size_t b = (total + 255) / 256;
   if (b > 132 * 16) b = 132 * 16;
-  return launch_pdl(act_copy_kernel, dim3((unsigned)(b ? b : 1)), dim3(256), 0, stream, p);
+  act_copy_kernel<<<(unsigned)(b ? b : 1), 256, 0, stream>>>(p);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_bias_affine(float* scale, float* shift, const float* bias, int N, int C, int stride, cudaStream_t stream) {
@@ -223,10 +221,10 @@ cudaError_t launch_import_nchw(const ImportParams& p, cudaStream_t stream) {
   dim3 block(32, 8);
   if (o.C <= 16) {
     dim3 grid((Wpad + 127) / 128, Hpad * o.N, 1);
-    return launch_pdl(import_nchw_kernel<16>, grid, block, 0, stream, p);
+    import_nchw_kernel<16><<<grid, block, 0, stream>>>(p);
   } else {
     dim3 grid((Wpad + 127) / 128, Hpad * o.N, (o.C + 63) / 64);
-    return launch_pdl(import_nchw_kernel<64>, grid, block, 0, stream, p);
+    import_nchw_kernel<64><<<grid, block, 0, stream>>>(p);
   }
   return cudaGetLastError();
 }
@@ -234,7 +232,8 @@ cudaError_t launch_import_nchw(const ImportParams& p, cudaStream_t stream) {
 cudaError_t launch_export_nchw(const ExportParams& p, cudaStream_t stream) {
   const ActDesc& a = p.in;
   dim3 grid((a.W + 127) / 128, a.H * a.N, (a.Cvalid + 31) / 32), block(32, 8);
-  return launch_pdl(export_nchw_kernel, grid, block, 0, stream, p);
+  export_nchw_kernel<<<grid, block, 0, stream>>>(p);
+  return cudaGetLastError();
 }
 
 // Tiled variant for plain convs (forward packing and the data-gradient packing of stride-1 convs): a block stages a
@@ -292,8 +291,7 @@ cudaError_t launch_pack_weights(const PackParams& p, cudaStream_t stream) {
   const int taps = p.kh * p.kw;
   bool natural = !p.transposed && !p.headkx && p.ntaps == taps;
   for (int t = 0; t < taps && natural; ++t) natural = (p.tap_ky[t] * p.kw + p.tap_kx[t] == t);
-  static const bool tiled_ok = [] { const char* e = getenv("V2V_PACK_TILED"); return !(e && e[0] == '0'); }();
-  if (natural && tiled_ok) {
+  if (natural) {
     const int tstride = taps | 1;
     int TC = 32;
     while (TC > 4 && (size_t)TC * (32 * tstride + 1) * sizeof(float) > 40 * 1024) TC >>= 1;

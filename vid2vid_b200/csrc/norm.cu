@@ -17,7 +17,6 @@ namespace v2v {
 // Stand-alone finalisation (one thread per channel): only the grid-stride fallback of the normalise pass needs the scale /
 // shift arrays ahead of time; the row-segment kernel computes them in its block prologue (see finalize.cuh).
 __global__ void __launch_bounds__(128) stats_finalize_kernel(FinalizeParams p) {
-  pdl_prologue();
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= p.C) return;
   channel_side_effects(p, c);
@@ -109,7 +108,6 @@ __device__ __forceinline__ void apply_item(const ApplyParams& p, int vecs, int W
 }
 
 __global__ void __launch_bounds__(256) norm_apply_kernel(ApplyParams p) {
-  pdl_prologue();
   const int vecs = p.out.C / 8;
   const int Hpad = p.out.H + p.out.pad_t + p.out.pad_b, Wpad = p.out.W + p.out.pad_l + p.out.pad_r;
   const unsigned total = (unsigned)p.out.N * Hpad * Wpad * vecs;        // < 2^31 checked by the launcher
@@ -147,7 +145,6 @@ template <int NADD, bool PREC>
 __global__ void __launch_bounds__(256) norm_apply_rows_kernel(ApplyParams p, int xt, int ppb) {
   constexpr int NB = PREC ? 2 : 4;          // items per batch
   constexpr int NW = PREC ? 2 : 1;          // 16-byte words per item and tensor
-  pdl_prologue();
   const int vecs = p.out.C >> 3;
   const int t = threadIdx.x;
   const bool idle = t >= ppb * vecs;                 // (idle threads still take part in the prologue barrier)
@@ -267,15 +264,15 @@ static inline int grid_for(long long total, int block) {
 }
 
 cudaError_t launch_stats_finalize(const FinalizeParams& p, cudaStream_t stream) {
-  return launch_pdl(stats_finalize_kernel, dim3((p.C + 127) / 128), dim3(128), 0, stream, p);
+  stats_finalize_kernel<<<(p.C + 127) / 128, 128, 0, stream>>>(p);
+  return cudaGetLastError();
 }
 
 // true: the row-segment kernel (which derives scale / shift in its prologue) handles this launch; false: grid-stride fallback
 bool norm_apply_uses_rows(const ApplyParams& p) {
-  static const int variant = [] { const char* e = getenv("V2V_APPLY"); return e ? atoi(e) : 1; }();
   const int vecs = p.out.C / 8;
   const int Hpad = p.out.H + p.out.pad_t + p.out.pad_b;
-  return variant == 1 && vecs <= 256 && (long long)p.out.N * Hpad <= 65535;
+  return vecs <= 256 && (long long)p.out.N * Hpad <= 65535;
 }
 
 cudaError_t launch_norm_apply(const ApplyParams& p, cudaStream_t stream) {
@@ -291,15 +288,18 @@ cudaError_t launch_norm_apply(const ApplyParams& p, cudaStream_t stream) {
     const int xt = ppb * 8;                         // 8 items per thread
     dim3 grid((Wpad + xt - 1) / xt, p.out.N * Hpad);
     if (prec) {
-      if (p.n_add == 0) return launch_pdl(norm_apply_rows_kernel<0, true>, grid, dim3(256), 0, stream, p, xt, ppb);
-      if (p.n_add == 1) return launch_pdl(norm_apply_rows_kernel<1, true>, grid, dim3(256), 0, stream, p, xt, ppb);
-      return launch_pdl(norm_apply_rows_kernel<2, true>, grid, dim3(256), 0, stream, p, xt, ppb);
+      if (p.n_add == 0) norm_apply_rows_kernel<0, true><<<grid, 256, 0, stream>>>(p, xt, ppb);
+      else if (p.n_add == 1) norm_apply_rows_kernel<1, true><<<grid, 256, 0, stream>>>(p, xt, ppb);
+      else norm_apply_rows_kernel<2, true><<<grid, 256, 0, stream>>>(p, xt, ppb);
+    } else {
+      if (p.n_add == 0) norm_apply_rows_kernel<0, false><<<grid, 256, 0, stream>>>(p, xt, ppb);
+      else if (p.n_add == 1) norm_apply_rows_kernel<1, false><<<grid, 256, 0, stream>>>(p, xt, ppb);
+      else norm_apply_rows_kernel<2, false><<<grid, 256, 0, stream>>>(p, xt, ppb);
     }
-    if (p.n_add == 0) return launch_pdl(norm_apply_rows_kernel<0, false>, grid, dim3(256), 0, stream, p, xt, ppb);
-    if (p.n_add == 1) return launch_pdl(norm_apply_rows_kernel<1, false>, grid, dim3(256), 0, stream, p, xt, ppb);
-    return launch_pdl(norm_apply_rows_kernel<2, false>, grid, dim3(256), 0, stream, p, xt, ppb);
+  } else {
+    norm_apply_kernel<<<grid_for(total, 256), 256, 0, stream>>>(p);
   }
-  return launch_pdl(norm_apply_kernel, dim3(grid_for(total, 256)), dim3(256), 0, stream, p);
+  return cudaGetLastError();
 }
 
 }  // namespace v2v

@@ -60,8 +60,6 @@ static inline size_t round_up_sz(size_t a, size_t b) { return (a + b - 1) / b * 
 // padded channel count of an activation buffer: one K block of min(C,64) channels per shared-memory row
 static thread_local int g_pad_min = 0;     // set while a backward sub-plan is being described (build_backward_units)
 static inline int pad_channels(int c) {
-  const char* e = getenv("V2V_KC64");
-  if (e && e[0] == '1') return round_up(c, 64);
   const int r = c <= 16 ? 16 : (c <= 32 ? 32 : round_up(c, 64));
   return std::max(r, g_pad_min);
 }
@@ -76,8 +74,7 @@ struct ConvGeom {
   int TH, TW, R;
   int RW;                 // taps per patch row: tap r of a group reads the patch shifted by (r / RW) rows, (r % RW) columns
   int patch2d_kc;         // > 0: 16x8 pixel tiles, ONE activation patch of (16+kh-1) x (8+kw-1) pixels serves all kh*kw taps;
-  int patch2d_bn;         //      K block / N tile / weight residency chosen together with the geometry (they decide the fit)
-  int patch2d_resident;
+  int patch2d_bn;         //      K block / N tile chosen together with the geometry (they decide the fit)
   int headkx;             // > 0 (= kw): small-Cout head evaluated as a GEMM over (kx, channel) columns (taps over ky only)
   int n_groups, n_phases;
   ConvGroup groups[V2V_MAX_TAPS];
@@ -85,9 +82,13 @@ struct ConvGeom {
 };
 
 
-static inline int round_up_i(int a, int b) { return round_up(a, b); }
 static const int kSmemBudget = 188 * 1024;      // operand slots + resident weights (227 KB - 36.5 KB epilogue staging - alignment - barriers)
 static const int kResidentMax = 150 * 1024;
+
+// Bytes of one shared-memory operand slot, each of its sp halves 1 KB aligned: the activation patch of `pixels` pixels for
+// one K block of kc channels (A), and the weights of `taps` taps x an N tile of bn x kc (B).
+static inline int a_slot_bytes(int sp, int pixels, int kc) { return sp * round_up(pixels * kc * 2, 1024); }
+static inline int b_slot_bytes(int sp, int taps, int bn, int kc) { return sp * round_up(taps * bn * kc * 2, 1024); }
 
 // 2-D patch mode (stride-1 filters): a tile of 16 rows x 8 pixels makes every 8-row core-matrix group of the A operand
 // one tile row, so the operand of tap (ky, kx) is the SAME shared-memory patch of (16+kh-1) x (8+kw-1) pixels read with
@@ -95,32 +96,22 @@ static const int kResidentMax = 150 * 1024;
 // ~1.4x (3x3) instead of 3x (row tiles with horizontal reuse) or 9x (one box per tap).  Feasible when a step's weights
 // (all taps of one K block) fit next to the patch, double buffered, or the whole (phase, N tile) weight set stays resident.
 // sp = 2 for precise plans: every operand slot holds a hi and a lo half, so all byte counts double.
-static bool choose_patch2d(const v2v_conv_desc& c, bool head, int N, int grid_h, int grid_w, int sp, int* kc_out, int* bn_out, int* res_out) {
-  const char* e = getenv("V2V_PATCH2D");
-  if (e && e[0] == '0') return false;
+static bool choose_patch2d(const v2v_conv_desc& c, bool head, int N, int grid_h, int grid_w, int sp, int* kc_out, int* bn_out) {
   if (c.transposed || c.stride != 1 || c.kh * c.kw == 1 || grid_w < 8) return false;
   const long long tiles = (long long)((grid_w + 7) / 8) * ((grid_h + 15) / 16);
   if (tiles * 128 * 4 > (long long)grid_h * grid_w * 5) return false;          // > 25 % masked rows: keep row tiles
-  const int Cp = pad_channels(c.Cin), taps = c.kh * c.kw, PH = 16 + c.kh - 1, PW = 8 + c.kw - 1;
-  const int bn0 = head ? 16 : std::min(128, round_up_i(c.Cout, 32));
+  const int Cp = pad_channels(c.Cin), taps = c.kh * c.kw, patch_px = (16 + c.kh - 1) * (8 + c.kw - 1);
+  const int bn0 = head ? 16 : std::min(128, round_up(c.Cout, 32));
   const long long m_total = tiles * N;
   const int sms = device_sm_count();
   const int kc_max = std::min(Cp, 64);
-  // (1) resident weights with the natural N tile, (2) with a halved N tile when a CTA walks >= 4 M tiles (streaming the
-  // weights again for every tile costs more L2 traffic than the second pass over the activations)
-  for (int pass = 0; pass < 2; ++pass) {
-    const int bn = pass == 0 ? bn0 : bn0 / 2;
-    // (pass 2 is opt-in: it has not been measured to pay off)
-    static const bool half_ok = [] { const char* e = getenv("V2V_P2D_HALF"); return e && e[0] == '1'; }();
-    if (pass == 1 && (!half_ok || bn0 < 128 || m_total < 4LL * sms)) break;
-    if (m_total <= sms) break;
+  // resident weights with the natural N tile, when a CTA walks several M tiles
+  if (m_total > sms) {
     // precise plans also try 32-channel K blocks: the resident weight set is the same size, the two patch stages halve
     for (int kc = kc_max; kc >= (sp == 2 ? 32 : kc_max); kc >>= 1) {
-      if (Cp % kc) continue;
-      const long long res_bytes = (long long)sp * (Cp / kc) * round_up_i(taps * bn * kc * 2, 1024);
-      const int patch = sp * round_up_i(PH * PW * kc * 2, 1024);
-      if (res_bytes <= kResidentMax && kSmemBudget - res_bytes >= 2 * patch) {
-        *kc_out = kc; *bn_out = bn; *res_out = 1;
+      const long long res_bytes = (long long)(Cp / kc) * b_slot_bytes(sp, taps, bn0, kc);
+      if (res_bytes <= kResidentMax && kSmemBudget - res_bytes >= 2 * a_slot_bytes(sp, patch_px, kc)) {
+        *kc_out = kc; *bn_out = bn0;
         return true;
       }
     }
@@ -132,11 +123,11 @@ static bool choose_patch2d(const v2v_conv_desc& c, bool head, int N, int grid_h,
   if (m_total >= 4LL * sms) return false;
   // (precise plans: halve the N tile before going below 32-channel K blocks; 32-byte rows ingest badly)
   for (int bn = bn0; bn >= (sp == 2 && !head ? std::min(bn0, 64) : bn0); bn >>= 1)
-    for (int kc = kc_max; kc >= 32; kc >>= 1) {
-      if (Cp % kc) continue;
-      const int patch = sp * round_up_i(PH * PW * kc * 2, 1024), bstep = sp * round_up_i(taps * bn * kc * 2, 1024);
-      if (2 * (patch + bstep) <= kSmemBudget) { *kc_out = kc; *bn_out = bn; *res_out = 0; return true; }
-    }
+    for (int kc = kc_max; kc >= 32; kc >>= 1)
+      if (2 * (a_slot_bytes(sp, patch_px, kc) + b_slot_bytes(sp, taps, bn, kc)) <= kSmemBudget) {
+        *kc_out = kc; *bn_out = bn;
+        return true;
+      }
   return false;
 }
 
@@ -166,8 +157,7 @@ static int conv_geometry(const v2v_conv_desc& c, int head, int N, int H, int W, 
   g->TH = 128 / g->TW;
   g->R = 1;
   int ng = 0;
-  static const bool headkx_ok = [] { const char* e = getenv("V2V_HEADKX"); return !(e && e[0] == '0'); }();
-  if (head == 2 && headkx_ok && !c.transposed && c.stride == 1 && c.kw >= 3 && c.kw <= 8 && c.Cout <= 4 && c.kw * c.Cout <= 32 &&
+  if (head == 2 && !c.transposed && c.stride == 1 && c.kw >= 3 && c.kw <= 8 && c.Cout <= 4 && c.kw * c.Cout <= 32 &&
       c.kh <= 8 && g->grid_w >= 32) {
     // Small-Cout heads (7x7, 2-3 channels) are MMA-issue bound as N = 16 convolutions: 49 taps x K blocks of ~40-cycle MMAs per
     // 128 pixels.  As a GEMM with N = kw * Cout columns per INPUT pixel and taps over the kh filter rows only, a tile issues
@@ -181,7 +171,7 @@ static int conv_geometry(const v2v_conv_desc& c, int head, int N, int H, int W, 
     g->headkx = c.kw;
     g->groups[ng++] = ConvGroup{0, 0, 0, 0, 0, 0};
     g->phases[0] = ConvPhase{0, ng, 0, 0};
-  } else if (allow_reuse && choose_patch2d(c, head != 0, N, g->grid_h, g->grid_w, sp, &g->patch2d_kc, &g->patch2d_bn, &g->patch2d_resident)) {
+  } else if (allow_reuse && choose_patch2d(c, head != 0, N, g->grid_h, g->grid_w, sp, &g->patch2d_kc, &g->patch2d_bn)) {
     g->n_phases = 1;
     g->TH = 16; g->TW = 8;
     g->R = c.kh * c.kw; g->RW = c.kw;
@@ -341,7 +331,6 @@ struct v2v_plan {
   int impl = V2V_IMPL_UMMA;
   int precise = 0;            // V2V_PREC_BF16X3: split activations / weights, fp32 raw tensors, 3 MMAs per K block
   int sp() const { return precise ? 2 : 1; }
-  bool allow_reuse = true;
   bool lowered = false, finalized = false;
   bool train = false;          // keep what the backward needs (batch statistics) and allocate gradient buffers
   void* garena = nullptr; size_t garena_bytes = 0;
@@ -498,7 +487,7 @@ static int lower(v2v_plan* P) {
   for (auto& op : P->gops) {
     if (op.kind == G_CONV || op.kind == G_CONV_ACT || op.kind == G_HEAD) {
       Value& vin = P->values[op.value_in];
-      int rc = conv_geometry(op.conv, op.kind == G_HEAD ? (P->impl == V2V_IMPL_UMMA ? 2 : 1) : 0, vin.N, vin.H, vin.W, P->allow_reuse,
+      int rc = conv_geometry(op.conv, op.kind == G_HEAD ? (P->impl == V2V_IMPL_UMMA ? 2 : 1) : 0, vin.N, vin.H, vin.W, true,
                              P->sp(), &op.geom);
       if (rc) return rc;
       op.req_index = add_req(vin, conv_req(op.conv, op.geom));
@@ -533,208 +522,185 @@ static int lower(v2v_plan* P) {
   return 0;
 }
 
-static void fill_conv_params(v2v_plan* P, GOp& op) {
-  const Value& vin = P->values[op.value_in];
+static int max_phase_groups(const ConvGeom& g) {
+  int m = 0;
+  for (int i = 0; i < g.n_phases; ++i) m = std::max(m, g.phases[i].group_end - g.phases[i].group_begin);
+  return m;
+}
+
+// The configuration of one conv_umma_kernel launch that fill_conv_params derives every other kernel parameter from.
+struct ConvTiling {
+  int kc, BN, MG;          // K block, N tile, M tiles accumulated side by side per weight pass
+  int b_resident;          // the weights of one (phase, N tile) stay in shared memory
+  int ring2, TB, SBr;      // decoupled operand rings: taps per weight chunk, weight slots
+  int CG, SG;              // K-loop steps per commit group, group slots
+};
+
+// Chooses the tiling from the conv, its geometry and the tile grid / patch extent already in kp.  The rules apply in order;
+// each later rule refines what the earlier ones chose.
+static ConvTiling choose_tiling(const v2v_plan* P, const GOp& op, const ConvKernelParams& kp) {
   const ConvGeom& g = op.geom;
-  ConvKernelParams& kp = op.kp;
-  memset(&kp, 0, sizeof(kp));
-  kp.N = vin.N; kp.TH = g.TH; kp.TW = g.TW;
-  kp.headkx = g.headkx;
-  kp.tile_dx = g.headkx ? g.TW - (g.headkx - 1) : g.TW;
-  kp.tiles_x = (g.grid_w + kp.tile_dx - 1) / kp.tile_dx; kp.tiles_y = (g.grid_h + g.TH - 1) / g.TH;
-  kp.grid_h = g.grid_h; kp.grid_w = g.grid_w;
-  kp.Cout = op.conv.Cout;
-  kp.BN = op.kind == G_HEAD ? (g.headkx ? 32 : 16) : std::min(128, round_up(op.conv.Cout, 32));
-  kp.Cp = pad_channels(op.conv.Cin);
-  kp.kc = std::min(kp.Cp, 64);
-  kp.MG = 1;
-  const int sp = P->sp();
-  kp.split = P->precise;
-  kp.a_exact = (P->precise && vin.exact_bf16) ? 1 : 0;
-  const bool p2d = g.patch2d_kc > 0;
-  if (p2d) { kp.kc = g.patch2d_kc; if (op.kind != G_HEAD) kp.BN = g.patch2d_bn; }
+  const v2v_conv_desc& c = op.conv;
+  const bool head = op.kind == G_HEAD, p2d = g.patch2d_kc > 0;
+  const int sp = P->sp(), sms = device_sm_count(), budget = kSmemBudget;
+  const int Cp = kp.Cp, kc_nat = std::min(Cp, 64), bn_nat = std::min(128, round_up(c.Cout, 32));
+  const int m_tiles = kp.N * kp.tiles_x * kp.tiles_y;
+  auto a_slot = [&](int kc) { return a_slot_bytes(sp, kp.PW * kp.PH, kc); };
+  ConvTiling t{};
+  t.kc = kc_nat; t.BN = head ? (g.headkx ? 32 : 16) : bn_nat; t.MG = 1;
+  if (p2d) { t.kc = g.patch2d_kc; if (!head) t.BN = g.patch2d_bn; }
   if (g.headkx) {
     // K block of a kx-GEMM head: the largest whose patch ring (2 stages) fits next to the resident weight set, or, failing
     // that, whose two streamed stages fit
-    for (int kc = std::min(kp.Cp, 64); kc >= 16; kc >>= 1) {
-      if (kp.Cp % kc) continue;
-      const int a_sl = sp * round_up(g.TW * (g.TH + op.conv.kh - 1) * kc * 2, 1024), b_sl = sp * round_up(g.R * kp.BN * kc * 2, 1024);
-      const long long res = (long long)(kp.Cp / kc) * b_sl;
-      kp.kc = kc;
-      if ((res <= kResidentMax && kSmemBudget - res >= 2 * a_sl) || 2 * (a_sl + b_sl) <= kSmemBudget) break;
+    for (; t.kc > 16; t.kc >>= 1) {
+      const int a_sl = a_slot(t.kc), b_sl = b_slot_bytes(sp, g.R, t.BN, t.kc);
+      const long long res = (long long)(Cp / t.kc) * b_sl;
+      if ((res <= kResidentMax && budget - res >= 2 * a_sl) || 2 * (a_sl + b_sl) <= budget) break;
     }
   }
-  const int m_tiles = kp.N * kp.tiles_x * kp.tiles_y;
   // M blocking for row-tile filters whose weights must be streamed (the 7x7 stems over the 108-channel label input):
   // per M tile such a layer pulls taps*Cp*BN*2 bytes of weights through L2 -> SM (802 KB for 108->48, 13 GB per launch at
   // 2048x1024), more than an SM ingests at the full MMA rate.  MG = 2 consecutive x tiles accumulate side by side in
   // registers and share every weight tile, within the accumulator budget V2V_MAX_ACC_COLS.  64-byte rows (32-channel K
-  // blocks) cost TMA request rate, so they are used only where they buy an exact N tile (Cout = 96).  V2V_FORCE=kc,bn,mg
-  // overrides the choice for timing experiments.
+  // blocks) cost TMA request rate, so they are used only where they buy an exact N tile (Cout = 96).
   bool mblock = false;
-  if (!p2d && !op.conv.transposed && op.conv.stride == 1 && g.R >= 5 && g.n_phases == 1 && op.kind != G_HEAD &&
-      m_tiles >= 4 * device_sm_count() &&
-      (long long)sp * op.conv.kh * op.conv.kw * kp.Cp * std::min(64, kp.BN) * 2 > kResidentMax) {   // cannot stay resident
-    int c_kc = std::min(kp.Cp, 64), c_bn = std::min(64, round_up(op.conv.Cout, 32)), c_mg = 2;
-    if (round_up(op.conv.Cout, 32) == 96 && kp.Cp % 32 == 0) { c_kc = 32; c_bn = 96; }
-    c_mg = std::max(1, std::min(c_mg, V2V_MAX_ACC_COLS / c_bn));      // (the exact 96-wide N tile leaves room for one tile)
-    if (const char* ef = getenv("V2V_FORCE")) sscanf(ef, "%d,%d,%d", &c_kc, &c_bn, &c_mg);      // timing experiments
-    const char* em = getenv("V2V_MG");
-    if (em && atoi(em) == 0) c_mg = 0;                                                           // V2V_MG=0: off
+  if (!p2d && !c.transposed && c.stride == 1 && g.R >= 5 && g.n_phases == 1 && !head && m_tiles >= 4 * sms &&
+      (long long)sp * c.kh * c.kw * Cp * std::min(64, t.BN) * 2 > kResidentMax) {   // cannot stay resident
+    int c_kc = kc_nat, c_bn = std::min(64, round_up(c.Cout, 32));
+    if (round_up(c.Cout, 32) == 96 && Cp % 32 == 0) { c_kc = 32; c_bn = 96; }
+    const int c_mg = std::min(2, V2V_MAX_ACC_COLS / c_bn);      // (the exact 96-wide N tile leaves room for one tile)
     // precise plans double every slot: fall back through smaller K blocks / N tiles until two stages fit
     const int cand[4][3] = {{c_kc, c_bn, c_mg}, {32, c_bn, c_mg}, {32, 64, c_mg}, {32, 64, 1}};
     for (int ci = 0; ci < (sp == 2 ? 4 : 1) && !mblock; ++ci) {
       const int t_kc = cand[ci][0], t_bn = cand[ci][1], t_mg = cand[ci][2];
-      if (t_mg < 1 || kp.Cp % t_kc || t_bn % 32 || t_bn > 128 || kp.tiles_x % t_mg || t_mg * std::max(32, t_bn) > V2V_MAX_ACC_COLS) continue;
-      const int a_slot = sp * round_up((g.TW + g.R - 1) * g.TH * t_kc * 2, 1024), b_slot = sp * round_up(g.R * t_bn * t_kc * 2, 1024);   // (never a head)
-      if (2 * (t_mg * a_slot + b_slot) <= kSmemBudget) { kp.kc = t_kc; kp.BN = t_bn; kp.MG = t_mg; mblock = true; }
+      if (Cp % t_kc || kp.tiles_x % t_mg) continue;
+      if (2 * (t_mg * a_slot(t_kc) + b_slot_bytes(sp, g.R, t_bn, t_kc)) <= budget) { t.kc = t_kc; t.BN = t_bn; t.MG = t_mg; mblock = true; }
     }
   }
-  kp.cblocks = kp.Cp / kp.kc;
-  kp.row_bytes = kp.kc * 2; kp.kmma = kp.kc / 16;
-  kp.layout_type = kp.kc == 64 ? 2 : (kp.kc == 32 ? 4 : 6);
-  kp.R = g.R; kp.RW = g.RW;
-  // patch extent in pixels; 8-row core-matrix groups of the A operand are SBO bytes apart: the canonical 8 rows for
-  // row tiles, one patch row (PW pixels) in 2-D patch mode
-  kp.PW = p2d ? g.TW + op.conv.kw - 1 : (g.headkx ? g.TW : g.TW + g.R - 1);
-  kp.PH = p2d ? g.TH + op.conv.kh - 1 : (g.headkx ? g.TH + op.conv.kh - 1 : g.TH);
-  kp.sbo_bytes = 8 * kp.row_bytes;
-  kp.sbo_a_bytes = p2d ? kp.PW * kp.row_bytes : 8 * kp.row_bytes;
-  kp.a_half_bytes = round_up(kp.PW * kp.PH * kp.row_bytes, 1024);
-  kp.a_slot_bytes = sp * kp.a_half_bytes;
-  kp.EG = 1;                   // the two consumer warpgroups of conv_umma_kernel drain every tile together
-  // shared-memory budget: 227 KB - epilogue staging - alignment slack - barriers
-  const int budget = kSmemBudget;
-  // a weight slot holds the R taps served by one activation patch; keep >= 2 slots + 3 patches in the budget
-  if (sp == 2 && !p2d && !mblock && g.R > 1 && !g.headkx) {
-    // precise plans: every slot doubles.  N tiles below 64 make the (3x) MMAs issue bound, so try (K block, N tile) in the
-    // order (kc, BN), (kc, BN/2 >= 64), (32, BN), (32, BN/2 >= 64) before falling through to the generic halving
-    const int bn0 = kp.BN, kc0 = kp.kc;
-    bool ok = false;
-    for (int t = 0; t < 4 && !ok; ++t) {
-      const int t_kc = (t & 2) ? 32 : kc0, t_bn = (t & 1) ? bn0 / 2 : bn0;
-      if (t_kc > kc0 || kp.Cp % t_kc || ((t & 1) && (t_bn < 64 || t_bn % 32))) continue;
-      const int a_sl = sp * round_up(kp.PW * kp.PH * t_kc * 2, 1024);
-      if (2 * sp * g.R * t_bn * t_kc * 2 + 3 * a_sl <= budget) {
-        kp.kc = t_kc; kp.BN = t_bn; ok = true;
-        kp.cblocks = kp.Cp / kp.kc; kp.row_bytes = kp.kc * 2; kp.kmma = kp.kc / 16;
-        kp.layout_type = kp.kc == 64 ? 2 : (kp.kc == 32 ? 4 : 6);
-        kp.sbo_bytes = 8 * kp.row_bytes; kp.sbo_a_bytes = 8 * kp.row_bytes;
-        kp.a_half_bytes = round_up(kp.PW * kp.PH * kp.row_bytes, 1024); kp.a_slot_bytes = sp * kp.a_half_bytes;
+  if (!p2d && !mblock && g.R > 1) {
+    // a weight slot holds the R taps served by one activation patch; keep >= 2 slots + 3 patches in the budget
+    auto fits = [&](int kc, int bn) { return 2 * sp * g.R * bn * kc * 2 + 3 * a_slot(kc) <= budget; };
+    if (sp == 2 && !g.headkx) {
+      // precise plans: every slot doubles.  N tiles below 64 make the (3x) MMAs issue bound, so try (K block, N tile) in the
+      // order (kc, BN), (kc, BN/2 >= 64), (32, BN), (32, BN/2 >= 64) before falling through to the generic halving
+      const int bn0 = t.BN, kc0 = t.kc;
+      for (int i = 0; i < 4; ++i) {
+        const int t_kc = (i & 2) ? 32 : kc0, t_bn = (i & 1) ? bn0 / 2 : bn0;
+        if (t_kc > kc0 || ((i & 1) && (t_bn < 64 || t_bn % 32))) continue;
+        if (fits(t_kc, t_bn)) { t.kc = t_kc; t.BN = t_bn; break; }
       }
     }
+    while (t.BN > 32 && !fits(t.kc, t.BN)) t.BN = std::max(32, t.BN / 2 / 32 * 32);
   }
-  while (!p2d && !mblock && g.R > 1 && kp.BN > 32 && 2 * sp * g.R * kp.BN * kp.row_bytes + 3 * kp.a_slot_bytes > budget)
-    kp.BN = std::max(32, kp.BN / 2 / 32 * 32);
   // Precise convs whose 128-wide N tile gives at most one work unit per SM (the 512->512 and 1024->1024 3x3 convs at 32x64,
   // 64 and 128 units of one M tile each) take a 64-wide tile instead.  Each unit then streams 48 instead of 64 KB per K step,
   // so three stages fit where two did, and the stage pipeline, not the MMA rate, is what bounds these layers: one round of
   // half-width units fills the SMs the 64-unit layers left idle, and two rounds of them beat one round of full-width units
   // (1024->1024: 0.278 against 0.348 ms on an H100 SXM).  Splitting N changes no output's sum, and a CTA's units belong to
   // different (N tile) keys, so it still adds the statistics of exactly one M tile per channel and flush.
-  if (sp == 2 && !p2d && !mblock && op.kind != G_HEAD && g.n_phases == 1 && kp.BN == 128 && kp.Cout % 128 == 0 &&
-      (long long)kp.N * kp.tiles_x * kp.tiles_y * (kp.Cout / 128) <= device_sm_count())
-    kp.BN = 64;
-  kp.b_half_bytes = round_up(g.R * kp.BN * kp.row_bytes, 1024);
-  kp.b_slot_bytes = sp * kp.b_half_bytes;
-  kp.n_tiles = (kp.Cout + kp.BN - 1) / kp.BN;
-  kp.m_total = kp.N * (kp.tiles_x / kp.MG) * kp.tiles_y;       // M units: MG consecutive x tiles each
-  kp.total_tiles = kp.m_total * kp.n_tiles * g.n_phases;
-  int max_phase_groups = 0;
-  for (int i = 0; i < g.n_phases; ++i) max_phase_groups = std::max(max_phase_groups, g.phases[i].group_end - g.phases[i].group_begin);
-  const int nB = max_phase_groups * kp.cblocks;                 // weight slots of one (phase, N tile)
-  const char* er = getenv("V2V_B_RESIDENT");
-  const bool allow_res = !(er && er[0] == '0');
-  const int sms = device_sm_count();
+  if (sp == 2 && !p2d && !mblock && !head && g.n_phases == 1 && t.BN == 128 && c.Cout % 128 == 0 &&
+      (long long)m_tiles * (c.Cout / 128) <= sms)
+    t.BN = 64;
   // resident weights pay off when a CTA walks several M tiles with the same weights
-  const bool many_m = kp.m_total > sms;
-  kp.b_resident = (allow_res && many_m && (long long)nB * kp.b_slot_bytes <= kResidentMax &&
-                   budget - nB * kp.b_slot_bytes >= 2 * kp.a_slot_bytes) ? 1 : 0;
-  if (kp.MG > 1) kp.b_resident = 0;
-  if (p2d && !kp.b_resident && 2 * (kp.a_slot_bytes + kp.b_slot_bytes) > budget) {
-    set_error("internal: 2-D patch conv does not fit (a %d b %d)", kp.a_slot_bytes, kp.b_slot_bytes);
-  }
-  kp.SB = kp.b_resident ? nB : 0;
+  const int nB = max_phase_groups(g) * (Cp / t.kc);            // weight slots of one (phase, N tile)
+  const int b_slot = b_slot_bytes(sp, g.R, t.BN, t.kc);
+  t.b_resident = (t.MG == 1 && m_tiles > sms && (long long)nB * b_slot <= kResidentMax &&
+                  budget - nB * b_slot >= 2 * a_slot(t.kc)) ? 1 : 0;
+  if (p2d && !t.b_resident && 2 * (a_slot(t.kc) + b_slot) > budget)
+    set_error("internal: 2-D patch conv does not fit (a %d b %d)", a_slot(t.kc), b_slot);
   // Decoupled operand rings for streamed-weight layers whose coupled stages forced a narrow K block or N tile (see
   // ConvKernelParams::ring2): 64-byte rows cost TMA request rate and narrow N tiles cost MMA issue slots.
-  kp.ring2 = 0;
-  {
-    static const bool ring2_ok = [] { const char* e = getenv("V2V_RING2"); return !(e && e[0] == '0'); }();
-    const int kc_nat = std::min(kp.Cp, 64), bn_nat = std::min(128, round_up(op.conv.Cout, 32));
-    // Precise plans only: bf16 plans and the exact-input finest stem keep the coupled stages (fewer barrier round trips
-    // per MMA).
-    if (ring2_ok && sp == 2 && !kp.a_exact && P->impl == V2V_IMPL_UMMA && !kp.b_resident && g.R >= 3 && !g.headkx && g.n_phases == 1 &&
-        op.kind != G_HEAD && (kp.kc < kc_nat || kp.BN < bn_nat)) {
-      const int nhA = 2;
-      const int a_half = round_up(kp.PW * kp.PH * kc_nat * 2, 1024);
-      bool found = false;
-      int f_bn = 0, f_mg = 0, f_tb = 0, f_sbr = 0;
-      // N tile: the natural one unless that leaves SMs idle (512->512 @32x64: 64 tiles of 128 columns)
-      const long long units_nat = (long long)kp.N * kp.tiles_x * kp.tiles_y * ((op.conv.Cout + bn_nat - 1) / bn_nat);
-      const int bns[2] = {bn_nat, bn_nat / 2}, mgs[2] = {kp.MG, 1};
-      const bool too_few = units_nat * 5 < (long long)sms * 3;      // then the coupled path with a halved N tile fills the SMs
-      for (int bi = 0; bi < 2 && !found && !too_few; ++bi) {
-        const int bn = bns[bi];
-        if (bn < 32 || bn % 32 || (bi == 1 && bn < 64)) continue;
-        for (int mi = 0; mi < 2 && !found; ++mi) {
-          const int mg = mgs[mi];
-          if (mg < 1 || kp.tiles_x % mg || mg * std::max(32, bn) > V2V_MAX_ACC_COLS || (mi == 1 && mgs[0] == 1)) continue;
-          // taps per weight chunk: as many as leave >= 3 chunks in flight (every chunk costs a commit group and a barrier
-          // round trip: fewer, longer chunks)
-          for (int tb = std::min(g.R, 4); tb >= 1 && !found; --tb) {
-            const int chunk = sp * round_up(tb * bn * kc_nat * 2, 1024);
-            const int sbr = (budget - 2 * mg * nhA * a_half) / chunk;
-            if (sbr >= 3) { found = true; f_bn = bn; f_mg = mg; f_tb = tb; f_sbr = std::min(8, sbr); }
-          }
+  // Precise plans only: bf16 plans and the exact-input finest stem keep the coupled stages (fewer barrier round trips
+  // per MMA).
+  if (sp == 2 && !kp.a_exact && P->impl == V2V_IMPL_UMMA && !t.b_resident && g.R >= 3 && !g.headkx && g.n_phases == 1 &&
+      !head && (t.kc < kc_nat || t.BN < bn_nat)) {
+    // N tile: the natural one unless that leaves SMs idle (512->512 @32x64: 64 tiles of 128 columns)
+    const long long units_nat = (long long)m_tiles * ((c.Cout + bn_nat - 1) / bn_nat);
+    const int bns[2] = {bn_nat, bn_nat / 2}, mgs[2] = {t.MG, 1};
+    const bool too_few = units_nat * 5 < (long long)sms * 3;      // then the coupled path with a halved N tile fills the SMs
+    for (int bi = 0; bi < 2 && !t.ring2 && !too_few; ++bi) {
+      const int bn = bns[bi];
+      if (bi == 1 && (bn < 64 || bn % 32)) continue;
+      for (int mi = 0; mi < 2 && !t.ring2; ++mi) {
+        const int mg = mgs[mi];
+        if (kp.tiles_x % mg || mg * std::max(32, bn) > V2V_MAX_ACC_COLS || (mi == 1 && mgs[0] == 1)) continue;
+        // taps per weight chunk: as many as leave >= 3 chunks in flight (every chunk costs a commit group and a barrier
+        // round trip: fewer, longer chunks)
+        for (int tb = std::min(g.R, 4); tb >= 1 && !t.ring2; --tb) {
+          const int sbr = (budget - 2 * mg * a_slot(kc_nat)) / b_slot_bytes(sp, tb, bn, kc_nat);
+          if (sbr >= 3) { t.ring2 = 1; t.kc = kc_nat; t.BN = bn; t.MG = mg; t.TB = tb; t.SBr = std::min(8, sbr); t.CG = 1; t.SG = 2; }
         }
-      }
-      if (found) {
-        kp.ring2 = 1; kp.kc = kc_nat; kp.BN = f_bn; kp.MG = f_mg; kp.TB = f_tb; kp.SBr = f_sbr;
-        kp.cblocks = kp.Cp / kp.kc; kp.row_bytes = kp.kc * 2; kp.kmma = kp.kc / 16;
-        kp.layout_type = kp.kc == 64 ? 2 : (kp.kc == 32 ? 4 : 6);
-        kp.sbo_bytes = 8 * kp.row_bytes; kp.sbo_a_bytes = p2d ? kp.PW * kp.row_bytes : 8 * kp.row_bytes;
-        kp.a_half_bytes = a_half; kp.a_slot_bytes = nhA * a_half;
-        kp.b_half_bytes = round_up(kp.TB * kp.BN * kp.row_bytes, 1024); kp.b_slot_bytes = sp * kp.b_half_bytes;
-        kp.n_tiles = (kp.Cout + kp.BN - 1) / kp.BN;
-        kp.m_total = kp.N * (kp.tiles_x / kp.MG) * kp.tiles_y;
-        kp.total_tiles = kp.m_total * kp.n_tiles * g.n_phases;
-        kp.b_resident = 0; kp.SB = 0; kp.CG = 1; kp.SG = 2; kp.SA = 2;
       }
     }
   }
   // Commit groups: CG consecutive K-loop steps share one barrier pair and one wgmma commit group, so that the barrier
   // round trips are paid once per group; `est` is a step's MMA work in cycle-like units (small-N MMAs are floored).
-  if (!kp.ring2) {
-    const int slot = kp.MG * kp.a_slot_bytes + (kp.b_resident ? 0 : kp.b_slot_bytes);
-    const int avail = budget - (kp.b_resident ? nB * kp.b_slot_bytes : 0);
+  if (!t.ring2) {
+    const int slot = t.MG * a_slot(t.kc) + (t.b_resident ? 0 : b_slot);
+    const int avail = budget - (t.b_resident ? nB * b_slot : 0);
     const int nslots = std::max(2, avail / slot);
-    const int steps = max_phase_groups * kp.cblocks;
-    const int est = (kp.split ? (kp.a_exact ? 2 : 3) : 1) * kp.MG * g.R * kp.kmma * std::max(40, kp.BN / 2);
-    int cg;
-    if (steps * est <= 6000 && 2 * steps <= nslots) cg = steps;           // one group per tile, double buffered
+    const int steps = nB;
+    const int est = (sp == 2 ? (kp.a_exact ? 2 : 3) : 1) * t.MG * g.R * (t.kc / 16) * std::max(40, t.BN / 2);
+    if (steps * est <= 6000 && 2 * steps <= nslots) t.CG = steps;           // one group per tile, double buffered
     else {
-      cg = std::max(1, std::min({(1500 + est - 1) / est, steps, nslots / 2}));
-      if (nslots / cg < 3 && cg > 1) cg = std::max(1, nslots / 3);
+      t.CG = std::max(1, std::min({(1500 + est - 1) / est, steps, nslots / 2}));
+      if (nslots / t.CG < 3 && t.CG > 1) t.CG = std::max(1, nslots / 3);
     }
-    const char* ec = getenv("V2V_CG");
-    if (ec) cg = std::max(1, std::min(atoi(ec), nslots / 2));
-    kp.CG = cg;
-    kp.SG = std::max(2, std::min(8, nslots / cg));
-    kp.SA = kp.SG * kp.CG;     // (informational)
+    t.SG = std::max(2, std::min(8, nslots / t.CG));
   }
-  { const char* dg = getenv("V2V_DBG"); kp.dbg = dg ? atoi(dg) : 0; }
-  kp.mg_total = kp.m_total;
-  kp.total_units = kp.m_total * kp.n_tiles * g.n_phases;
-  kp.grid = std::min(kp.total_units, device_sm_count());
+  return t;
+}
+
+static void fill_conv_params(v2v_plan* P, GOp& op) {
+  const Value& vin = P->values[op.value_in];
+  const ConvGeom& g = op.geom;
+  const v2v_conv_desc& c = op.conv;
+  const bool p2d = g.patch2d_kc > 0;
+  const int sp = P->sp();
+  ConvKernelParams& kp = op.kp;
+  memset(&kp, 0, sizeof(kp));
+  // geometry: the tile grid and the A patch extent in pixels
+  kp.N = vin.N; kp.TH = g.TH; kp.TW = g.TW;
+  kp.headkx = g.headkx;
+  kp.tile_dx = g.headkx ? g.TW - (g.headkx - 1) : g.TW;
+  kp.tiles_x = (g.grid_w + kp.tile_dx - 1) / kp.tile_dx; kp.tiles_y = (g.grid_h + g.TH - 1) / g.TH;
+  kp.grid_h = g.grid_h; kp.grid_w = g.grid_w;
+  kp.Cout = c.Cout;
+  kp.Cp = pad_channels(c.Cin);
+  kp.R = g.R; kp.RW = g.RW;
+  kp.PW = p2d ? g.TW + c.kw - 1 : (g.headkx ? g.TW : g.TW + g.R - 1);
+  kp.PH = p2d || g.headkx ? g.TH + c.kh - 1 : g.TH;
+  kp.split = P->precise;
+  kp.a_exact = (P->precise && vin.exact_bf16) ? 1 : 0;
   kp.num_phases = g.n_phases;
   memcpy(kp.phases, g.phases, sizeof(kp.phases));
   memcpy(kp.groups, g.groups, sizeof(kp.groups));
+  // the choice, and every field that follows from it
+  const ConvTiling t = choose_tiling(P, op, kp);
+  kp.kc = t.kc; kp.BN = t.BN; kp.MG = t.MG; kp.b_resident = t.b_resident;
+  kp.ring2 = t.ring2; kp.TB = t.TB; kp.SBr = t.SBr; kp.CG = t.CG; kp.SG = t.SG;
+  kp.cblocks = kp.Cp / kp.kc;
+  kp.row_bytes = kp.kc * 2; kp.kmma = kp.kc / 16;
+  kp.layout_type = kp.kc == 64 ? 2 : (kp.kc == 32 ? 4 : 6);
+  // 8-row core-matrix groups of the A operand are SBO bytes apart: the canonical 8 rows for row tiles, one patch row (PW
+  // pixels) in 2-D patch mode
+  kp.sbo_bytes = 8 * kp.row_bytes;
+  kp.sbo_a_bytes = p2d ? kp.PW * kp.row_bytes : 8 * kp.row_bytes;
+  kp.a_half_bytes = a_slot_bytes(1, kp.PW * kp.PH, kp.kc);
+  kp.a_slot_bytes = sp * kp.a_half_bytes;
+  kp.b_half_bytes = b_slot_bytes(1, kp.ring2 ? kp.TB : g.R, kp.BN, kp.kc);   // a ring2 weight slot holds TB taps
+  kp.b_slot_bytes = sp * kp.b_half_bytes;
+  kp.SB = kp.b_resident ? max_phase_groups(g) * kp.cblocks : 0;
+  kp.n_tiles = (kp.Cout + kp.BN - 1) / kp.BN;
+  kp.m_total = kp.N * (kp.tiles_x / kp.MG) * kp.tiles_y;       // M units: MG consecutive x tiles each
+  kp.total_units = kp.m_total * kp.n_tiles * g.n_phases;
+  kp.grid = std::min(kp.total_units, device_sm_count());
   kp.oy_mul = kp.ox_mul = g.mul;
   kp.out_H = g.out_h; kp.out_W = g.out_w;
-  kp.bias = op.conv.bias;
+  kp.bias = c.bias;
   kp.lrelu_slope = op.slope;
   kp.act = op.act;
-  op.Cp = kp.Cp; op.Ktotal = (g.headkx ? op.conv.kh : op.conv.kh * op.conv.kw) * kp.Cp;
+  op.Cp = kp.Cp; op.Ktotal = (g.headkx ? c.kh : c.kh * c.kw) * kp.Cp;
   kp.Khalf = op.Ktotal;
 }
 
@@ -753,10 +719,6 @@ static int pack_one(const GOp& op, cudaStream_t stream) {
 }
 
 static int run_xop(v2v_plan* P, const XOp& x, cudaStream_t s) {
-  // V2V_SKIP (timing experiments only, results are wrong): bit mask of XOp kinds left out of the frame, to measure what
-  // each kind costs inside the captured graph (CUDA events around single launches over-state tiny kernels)
-  static const int skip = [] { const char* e = getenv("V2V_SKIP"); return e ? atoi(e) : 0; }();
-  if (skip & (1 << (int)x.kind)) return 0;
   switch (x.kind) {
     case X_IMPORT: V2V_CUDA(launch_import_nchw(x.imp, s)); break;
     case X_EXPORT: V2V_CUDA(launch_export_nchw(x.exp, s)); break;
@@ -871,7 +833,7 @@ static int build_backward_units(v2v_plan* P, cudaStream_t stream) {
     struct PadReset { ~PadReset() { g_pad_min = 0; } } pad_reset;
     v2v_plan* C = nullptr;
     int rc = v2v_plan_create(P->device, P->impl, &C); if (rc) return rc;
-    C->precise = P->precise; C->allow_reuse = P->allow_reuse;
+    C->precise = P->precise;
     u.child = C;
     GOp gi; gi.kind = G_RAWIN; gi.ext_raw = dy; gi.ext_C = dy_C;
     gi.value_out = new_value(C, vin.N, oh, ow, c.Cout);
@@ -896,11 +858,9 @@ static int build_backward_units(v2v_plan* P, cudaStream_t stream) {
     const ActDesc& a_out = u.mode == 2 ? a_x : a_dy;
     const ActDesc& a_in = u.mode == 2 ? a_dy : a_x;
     const int kp = std::min(a_out.Wp, a_in.Wp) >= 64 ? 64 : (std::min(a_out.Wp, a_in.Wp) >= 32 ? 32 : (std::min(a_out.Wp, a_in.Wp) >= 16 ? 16 : 0));
-    const char* ewg = getenv("V2V_WGRAD");
-    const bool wg_ok = !(ewg && !strcmp(ewg, "simt"));
     const bool wide_out = a_out.C % 64 == 0, wide_in = a_in.C % 64 == 0;
     const bool narrow_ok_out = a_out.C == 16 || a_out.C == 32, narrow_ok_in = a_in.C == 16 || a_in.C == 32;
-    if (wg_ok && kp > 0 && ((wide_out && (wide_in || narrow_ok_in)) || (wide_in && narrow_ok_out)) && !a_out.parity && a_out.split == a_in.split &&
+    if (kp > 0 && ((wide_out && (wide_in || narrow_ok_in)) || (wide_in && narrow_ok_out)) && !a_out.parity && a_out.split == a_in.split &&
         c.kh * c.kw <= V2V_MAX_TAPS) {
       WgradParams& w = u.wg;
       w.N = vin.N; w.gh = u.mode == 2 ? vin.H : oh; w.gw = u.mode == 2 ? vin.W : ow;
@@ -1124,10 +1084,6 @@ int v2v_plan_create(int device, int conv_impl, v2v_plan** out) {
   v2v_plan* p = new v2v_plan();
   p->device = device;
   p->impl = conv_impl;
-  const char* e = getenv("V2V_TAP_REUSE");
-  p->allow_reuse = !(e && e[0] == '0');
-  const char* ei = getenv("V2V_CONV_IMPL");
-  if (ei && !strcmp(ei, "simt")) p->impl = V2V_IMPL_SIMT;
   *out = p;
   return 0;
 }
@@ -1207,7 +1163,7 @@ static int check_conv(v2v_plan* p, int value_in, const v2v_conv_desc* c) {
 int v2v_g_conv(v2v_plan* p, int value_in, const v2v_conv_desc* c, int* raw_out) {
   int rc = check_conv(p, value_in, c); if (rc) return rc;
   V2V_REQUIRE(raw_out, V2V_ERR_INVALID, "null raw_out");
-  ConvGeom g; rc = conv_geometry(*c, 0, p->values[value_in].N, p->values[value_in].H, p->values[value_in].W, p->allow_reuse, p->sp(), &g); if (rc) return rc;
+  ConvGeom g; rc = conv_geometry(*c, 0, p->values[value_in].N, p->values[value_in].H, p->values[value_in].W, true, p->sp(), &g); if (rc) return rc;
   GOp op; op.kind = G_CONV; op.value_in = value_in; op.conv = *c;
   Raw r{}; r.N = p->values[value_in].N; r.H = g.out_h; r.W = g.out_w; r.C = c->Cout; r.conv_op = (int)p->gops.size();
   p->raws.push_back(r);
@@ -1248,7 +1204,7 @@ int v2v_g_norm_act(v2v_plan* p, int raw_in, const v2v_norm_desc* norm, int act, 
 int v2v_g_conv_act(v2v_plan* p, int value_in, const v2v_conv_desc* c, int act, float slope, int* value_out) {
   int rc = check_conv(p, value_in, c); if (rc) return rc;
   V2V_REQUIRE(value_out, V2V_ERR_INVALID, "null value_out");
-  ConvGeom g; rc = conv_geometry(*c, 0, p->values[value_in].N, p->values[value_in].H, p->values[value_in].W, p->allow_reuse, p->sp(), &g); if (rc) return rc;
+  ConvGeom g; rc = conv_geometry(*c, 0, p->values[value_in].N, p->values[value_in].H, p->values[value_in].W, true, p->sp(), &g); if (rc) return rc;
   GOp op; op.kind = G_CONV_ACT; op.value_in = value_in; op.conv = *c; op.act = act; op.slope = slope;
   op.value_out = new_value(p, p->values[value_in].N, g.out_h, g.out_w, c->Cout);
   p->gops.push_back(op);
@@ -1545,7 +1501,7 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
           ap.n_add = 0;
           for (int k = 0; k < 2; ++k) if (op.add[k] >= 0) ap.add[ap.n_add++] = P->acts[P->values[op.add[k]].bufs[0]];
           ap.out = P->acts[vo.bufs[m]]; ap.pad_mode = P->act_pad_mode[vo.bufs[m]];
-          ap.fused = 0; ap.update_running = 0; ap.fin = fp;
+          ap.fin = fp;
           if (has_norm) {
             // Train-mode side effects (running statistics; the scale / shift / mean / rstd arrays the backward and the
             // grid-stride fallback read) happen ONCE per (raw, slice), however many normalise passes read it (two output
@@ -1558,9 +1514,8 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
             if (first) {
               // scale / shift come from the tail of the producing tensor-core launch (last-CTA finalisation, conv_umma.cu); the
               // SIMT cross-check implementation and a third slice of one raw use a stats_finalize launch instead
-              static const bool tail_ok = [] { const char* e = getenv("V2V_FUSED_FIN"); return !(e && e[0] == '0'); }();
               GOp& prod = P->gops[r.conv_op];
-              if (tail_ok && P->impl == V2V_IMPL_UMMA && prod.kp.n_fin < 2) {
+              if (P->impl == V2V_IMPL_UMMA && prod.kp.n_fin < 2) {
                 prod.kp.fin[prod.kp.n_fin++] = side;
                 prod.kp.fin_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<uint8_t*>(r.stats) + (size_t)r.N * 2 * r.C * sizeof(stat_t));
               } else {
@@ -1788,15 +1743,25 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
     GOp tmp = op;                                  // kernel configuration (host-only logic; no device state needed)
     fill_conv_params(const_cast<v2v_plan*>(P), tmp);
     const ConvKernelParams& kp = tmp.kp;
+    // EG: epilogue groups per tile, always 1 (the two consumer warpgroups of conv_umma_kernel drain every tile together)
     snprintf(t, sizeof(t),
              "%s{\"kind\":%d,\"Cin\":%d,\"Cout\":%d,\"k\":[%d,%d],\"stride\":%d,\"transposed\":%d,\"in\":%d,\"TH\":%d,\"TW\":%d,"
              "\"R\":%d,\"groups\":%d,\"phases\":%d,\"grid\":[%d,%d],\"out\":[%d,%d],"
-             "\"BN\":%d,\"kc\":%d,\"MG\":%d,\"CG\":%d,\"SG\":%d,\"resident\":%d,\"EG\":%d,\"units\":%d,\"split\":%d,\"ring2\":%d,\"TB\":%d,\"SBr\":%d,"
-             "\"p2d\":%d,\"a_exact\":%d,\"headkx\":%d,\"grad\":%d}",
+             "\"BN\":%d,\"kc\":%d,\"MG\":%d,\"CG\":%d,\"SG\":%d,\"resident\":%d,\"EG\":1,\"units\":%d,\"split\":%d,\"ring2\":%d,\"TB\":%d,\"SBr\":%d,"
+             "\"p2d\":%d,\"a_exact\":%d,\"headkx\":%d,\"grad\":%d,",
              first ? "" : ",", (int)op.kind, op.conv.Cin, op.conv.Cout, op.conv.kh, op.conv.kw, op.conv.stride, op.conv.transposed,
              op.value_in, g.TH, g.TW, g.R, g.n_groups, g.n_phases, g.grid_h, g.grid_w, g.out_h, g.out_w,
-             kp.BN, kp.kc, kp.MG, kp.CG, kp.SG, kp.b_resident, kp.EG, kp.total_units, kp.split, kp.ring2, kp.TB, kp.SBr,
+             kp.BN, kp.kc, kp.MG, kp.CG, kp.SG, kp.b_resident, kp.total_units, kp.split, kp.ring2, kp.TB, kp.SBr,
              g.patch2d_kc > 0 ? 1 : 0, kp.a_exact, kp.headkx, (int)P->op_live[&op - P->gops.data()]);
+    s += t;
+    // the derived launch parameters the kernel reads (ctas: persistent CTAs launched; smem: dynamic shared memory)
+    snprintf(t, sizeof(t),
+             "\"tiles_x\":%d,\"tiles_y\":%d,\"tile_dx\":%d,\"Cp\":%d,\"cblocks\":%d,\"row_bytes\":%d,\"kmma\":%d,\"layout_type\":%d,"
+             "\"sbo_bytes\":%d,\"sbo_a_bytes\":%d,\"RW\":%d,\"PW\":%d,\"PH\":%d,\"a_half_bytes\":%d,\"a_slot_bytes\":%d,"
+             "\"b_half_bytes\":%d,\"b_slot_bytes\":%d,\"SB\":%d,\"n_tiles\":%d,\"m_total\":%d,\"ctas\":%d,\"Khalf\":%d,\"smem\":%zu}",
+             kp.tiles_x, kp.tiles_y, kp.tile_dx, kp.Cp, kp.cblocks, kp.row_bytes, kp.kmma, kp.layout_type, kp.sbo_bytes,
+             kp.sbo_a_bytes, kp.RW, kp.PW, kp.PH, kp.a_half_bytes, kp.a_slot_bytes, kp.b_half_bytes, kp.b_slot_bytes, kp.SB,
+             kp.n_tiles, kp.m_total, kp.grid, kp.Khalf, conv_umma_smem_bytes(kp));
     s += t;
     first = false;
   }

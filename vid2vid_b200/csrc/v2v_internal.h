@@ -113,11 +113,11 @@ struct ConvKernelParams {
   int R, RW;                         // taps served per A patch (1 = none); taps per patch row (tap r: row r / RW, column r % RW)
   int PW, PH;                        // patch extent in pixels (TMA box)
   int sbo_a_bytes;                   // A operand 8-row group stride: 8*row_bytes (row tiles) or PW*row_bytes (2-D patch)
-  int a_slot_bytes, b_slot_bytes, SA, SB;
+  int a_slot_bytes, b_slot_bytes, SB;  // bytes per A / B slot (both halves), resident B slots
   int b_resident;                    // 1: SB == B tiles of one (phase, n-tile): loaded once per key, kept in smem
-  int n_tiles, m_total, total_tiles; // N tiles, M tiles (N * tiles_x * tiles_y), all tiles incl. phases
+  int n_tiles, m_total;              // N tiles, M units (N * tiles_x / MG * tiles_y)
   int CG, SG;                        // K-loop steps per barrier / commit group, group slots in the ring
-  int MG, mg_total, total_units;     // M tiles accumulated side by side per weight pass (work unit), units per key, all units
+  int MG, total_units;               // M tiles accumulated side by side per weight pass (work unit), all units
   int num_phases;
   int split;                         // precise plan: A and B slots hold a hi and a lo half; 3 MMAs per (tap, K block)
   int a_half_bytes, b_half_bytes;    // byte offset of the lo half inside an A / B slot
@@ -152,8 +152,6 @@ struct ConvKernelParams {
   int stats_C;
   const float* bias;                 // may be null
   const float* bias2; int Cout1;     // fused heads: channels >= Cout1 take bias2[j - Cout1]
-  int dbg;                           // timing experiments only (V2V_DBG): bit0 skip stats, bit1 skip output stores
-  int EG;                            // epilogue groups (always 1: both consumer warpgroups drain every tile)
   int grid;                          // CTAs launched (persistent); also the stats partial rows per (phase, image)
   // EPI_HEAD_F32: per output channel destination = io[head_slot] + head_off (+ n * head_bstride),
   // activation and scale.  Caller pointers are read from the device IO table at run time.
@@ -172,6 +170,7 @@ cudaError_t launch_conv_umma(const CUtensorMap& tmA, const CUtensorMap& tmB, con
                              cudaStream_t stream);
 cudaError_t launch_conv_simt(const ActDesc& in, const bf16* wpacked, int Ktotal, const ConvKernelParams& p,
                              cudaStream_t stream);
+size_t conv_umma_smem_bytes(const ConvKernelParams& p);   // dynamic shared memory of one conv_umma_kernel launch
 
 
 // ---------------------------------------------------------------------------------------
@@ -186,8 +185,6 @@ struct ApplyParams {
   ActDesc add[2];          // interior is read (any padding / parity)
   ActDesc out;
   int pad_mode;            // PadMode of out's halo
-  int fused;               // (unused: a block-prologue variant was slower than reading the arrays)
-  int update_running;
   FinalizeParams fin;
 };
 
@@ -289,20 +286,5 @@ cudaError_t launch_feature_l1(const FeatL1Params& p, cudaStream_t stream);
 cudaError_t launch_feature_l1_bwd(const FeatL1Params& p, const float* g, float* gx, cudaStream_t stream);
 int feature_l1_blocks(const ActDesc& x);
 int device_sm_count();
-
-
-// Host side of PDL: launch with the programmatic-stream-serialization attribute (captured into the CUDA graph as a
-// programmatic dependency) when V2V_PDL=1; plain serialised launches otherwise (the default, see pdl_enabled()).
-bool pdl_enabled();
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
-}
 
 }  // namespace v2v

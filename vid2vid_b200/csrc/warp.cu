@@ -48,7 +48,6 @@ __device__ __forceinline__ float bilerp(const float* pl, const Bilerp& b, int W)
 }
 
 __global__ void composite_kernel(CompositeParams p) {
-  pdl_prologue();
   const size_t HW = (size_t)p.H * p.W;
   const size_t total = (size_t)p.N * HW;
   float* raw = reinterpret_cast<float*>(p.io[p.s_raw]);          // in: tanh head output; out: composited
@@ -101,7 +100,6 @@ __global__ void composite_kernel(CompositeParams p) {
 // loads / stores with no per-pixel index division (grid = x blocks, rows, images); the warp gathers stay scalar (they hit
 // L2: neighbouring pixels sample neighbouring texels).  Same per-pixel arithmetic as composite_kernel -> identical results.
 __global__ void __launch_bounds__(128) composite_vec4_kernel(CompositeParams p) {
-  pdl_prologue();
   const int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * 4, y = blockIdx.y, n = blockIdx.z;
   if (x0 >= p.W) return;
   const size_t HW = (size_t)p.H * p.W, pix = (size_t)y * p.W + x0;
@@ -176,10 +174,10 @@ static inline int grid1d(size_t total) {
 }
 
 cudaError_t launch_composite(const CompositeParams& p, cudaStream_t stream) {
-  static const bool vec_ok = [] { const char* e = getenv("V2V_COMPOSITE_VEC"); return !(e && e[0] == '0'); }();
-  if (vec_ok && p.W % 4 == 0 && p.H <= 65535 && p.N <= 65535)
-    return launch_pdl(composite_vec4_kernel, dim3((p.W / 4 + 127) / 128, p.H, p.N), dim3(128), 0, stream, p);
-  return launch_pdl(composite_kernel, dim3(grid1d((size_t)p.N * p.H * p.W)), dim3(256), 0, stream, p);
+  if (p.W % 4 == 0 && p.H <= 65535 && p.N <= 65535)
+    composite_vec4_kernel<<<dim3((p.W / 4 + 127) / 128, p.H, p.N), 128, 0, stream>>>(p);
+  else
+    composite_kernel<<<grid1d((size_t)p.N * p.H * p.W), 256, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
