@@ -30,6 +30,7 @@
 // The kernel contains no call (no printf, no division slow path, see mbar_wait in ptx.cuh): ptxas would otherwise
 // serialise every wgmma, and the commit groups below would never overlap.
 #include <cstdlib>
+#include <type_traits>
 #include "ptx.cuh"
 #include "wgmma.cuh"
 #include "v2v_internal.h"
@@ -109,7 +110,9 @@ struct UnitIter {
 
 // All MMAs of one (tap, K block) for the MG accumulators: KMMA K=16 steps x the operand passes of the arithmetic mode
 // (precise plans: A_hi*B_hi + A_lo*B_hi + A_hi*B_lo, the lo halves a_half / b_half bytes further in the same slots).
-template <int BN, int MG>
+// W < BN (a tail N tile) multiplies only the first W columns: the m64nWk16 fragment is the first W / 2 registers of the
+// m64nBNk16 one (column block b of 8 is registers 4b .. 4b + 3, see wgmma.cuh).
+template <int BN, int W, int MG>
 __device__ __forceinline__ void mma_tap(float (&acc)[MG][BN / 2], uint64_t ad, uint64_t bd, uint32_t a_tile16, int kmma, int ps_step,
                                         uint32_t a_half16, uint32_t b_half16, uint32_t first) {
 #pragma unroll
@@ -118,14 +121,14 @@ __device__ __forceinline__ void mma_tap(float (&acc)[MG][BN / 2], uint64_t ad, u
     for (int ps = 0; ps < 3; ps += ps_step) {
       const uint64_t a = ad + (uint64_t)j * a_tile16 + (ps == 1 ? a_half16 : 0u), b = bd + (ps == 2 ? b_half16 : 0u);
       for (int k = 0; k < kmma; ++k) {
-        Wgmma<BN>::template mma<0, 0>(acc[j], a + 2 * k, b + 2 * k, f);      // +32 bytes along K per MMA
+        Wgmma<W>::template mma<0, 0>(*reinterpret_cast<float(*)[W / 2]>(&acc[j][0]), a + 2 * k, b + 2 * k, f);   // +32 bytes along K per MMA
         f = 1u;
       }
     }
   }
 }
 
-template <int BN, int MG>
+template <int BN, int BNT, int MG>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ ConvKernelParams p) {
@@ -358,65 +361,84 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       un.next(p);
       const bool last_of_key = !un.valid(p) || un.key != key;
       const int nsteps = (ph.group_end - ph.group_begin) * p.cblocks;
+      const bool tail = BNT != BN && n0 + BN > p.Cout;
 
       // ---------------- MMAs
       if (p.b_resident && first_of_key) mbar_wait(bres_full, gen);
 #pragma unroll
       for (int j = 0; j < MG; ++j) wgmma_fence_operands(acc[j]);
       wgmma_fence();
-      uint32_t first = 0;
-      if (p.ring2) {
-        // K loop: steps (tap group, K block); per step ONE patch slot (MG tiles) from the A ring and ceil(R / TB) weight
-        // chunks from the B ring; tap r of the step reads the patch advanced by (r / RW) * PW + (r % RW) rows.
-        const int RH = p.R / p.RW;
-        for (int st = 0; st < nsteps; ++st) {
-          mbar_wait(&g_full[as], apar);
-          const uint32_t a_base16 = (smem_u32(sG + (size_t)as * p.MG * p.a_slot_bytes) & 0x3FFFF) >> 4;
-          uint32_t bchunk16 = 0;
-          int tin = 0, r = 0;
-          for (int ky = 0; ky < RH; ++ky) {
-            for (int kx = 0; kx < p.RW; ++kx, ++r) {
-              if (tin == 0) {
-                mbar_wait(&b_full[bs], bpar);
-                bchunk16 = ((sB_u32 + (uint32_t)bs * (uint32_t)p.b_slot_bytes) & 0x3FFFF) >> 4;
-              }
-              mma_tap<BN, MG>(acc, a_d0 + a_base16 + (uint32_t)ky * prow16 + (uint32_t)kx * row16, b_d0 + bchunk16 + (uint32_t)tin * b_step,
-                              a_tile16, p.kmma, ps_step, a_half16, b_half16, first);
-              first = 1u;
-              if (++tin == p.TB || r == p.R - 1) {             // chunks hold TB taps; the last one of a step may be short
-                tin = 0;
-                commit_and_retire_previous(r == p.R - 1 ? as : -1, bs);      // the patch slot retires with the step's last chunk
-                if (++bs == p.SBr) { bs = 0; bpar ^= 1; }
-                wgmma_fence();
-              }
-            }
-          }
-          if (++as == p.SG) { as = 0; apar ^= 1; }
-        }
-      } else {
-        for (int s0 = 0; s0 < nsteps; s0 += p.CG) {
-          const int n = min(p.CG, nsteps - s0);
-          mbar_wait(&g_full[gs], gpar);
-          const uint32_t base = smem_u32(sG + (size_t)gs * group_bytes);
-          for (int i = 0; i < n; ++i) {
-            const uint32_t b_base = p.b_resident ? sB_u32 + (s0 + i) * p.b_slot_bytes
-                                                 : base + p.CG * p.MG * p.a_slot_bytes + i * p.b_slot_bytes;
-            const uint32_t a_base = base + i * p.MG * p.a_slot_bytes;
-            uint32_t al = (a_base & 0x3FFFF) >> 4, bl = (b_base & 0x3FFFF) >> 4;
-            // tap r reads the patch shifted by (r / RW) patch rows and (r % RW) pixels
-            for (int r0 = 0; r0 < p.R; r0 += p.RW, al += a_wrap) {
-              for (int r = 0; r < p.RW; ++r, al += a_step, bl += b_step) {
-                mma_tap<BN, MG>(acc, a_d0 + al, b_d0 + bl, a_tile16, p.kmma, ps_step, a_half16, b_half16, first);
+      // The K loop at one MMA width W, the full or the tail tile's, chosen once per unit: choosing it per MMA inside the
+      // wgmma chain made the 108->48 stem 23 % slower than the full-width MMAs.
+      auto k_loop = [&](auto width) {
+        constexpr int W = decltype(width)::value;
+        uint32_t first = 0;
+        int cb = 0;                                       // K block of the current step: the last one issues kmma_last steps
+        if (p.ring2) {
+          // K loop: steps (tap group, K block); per step ONE patch slot (MG tiles) from the A ring and ceil(R / TB) weight
+          // chunks from the B ring; tap r of the step reads the patch advanced by (r / RW) * PW + (r % RW) rows.
+          const int RH = p.R / p.RW;
+          for (int st = 0; st < nsteps; ++st) {
+            mbar_wait(&g_full[as], apar);
+            const uint32_t a_base16 = (smem_u32(sG + (size_t)as * p.MG * p.a_slot_bytes) & 0x3FFFF) >> 4;
+            uint32_t bchunk16 = 0;
+            int tin = 0, r = 0;
+            const int kk = cb == p.cblocks - 1 ? p.kmma_last : p.kmma;
+            if (++cb == p.cblocks) cb = 0;
+            for (int ky = 0; ky < RH; ++ky) {
+              for (int kx = 0; kx < p.RW; ++kx, ++r) {
+                if (tin == 0) {
+                  mbar_wait(&b_full[bs], bpar);
+                  bchunk16 = ((sB_u32 + (uint32_t)bs * (uint32_t)p.b_slot_bytes) & 0x3FFFF) >> 4;
+                }
+                mma_tap<BN, W, MG>(acc, a_d0 + a_base16 + (uint32_t)ky * prow16 + (uint32_t)kx * row16, b_d0 + bchunk16 + (uint32_t)tin * b_step,
+                                     a_tile16, kk, ps_step, a_half16, b_half16, first);
                 first = 1u;
+                if (++tin == p.TB || r == p.R - 1) {             // chunks hold TB taps; the last one of a step may be short
+                  tin = 0;
+                  commit_and_retire_previous(r == p.R - 1 ? as : -1, bs);      // the patch slot retires with the step's last chunk
+                  if (++bs == p.SBr) { bs = 0; bpar ^= 1; }
+                  wgmma_fence();
+                }
               }
             }
+            if (++as == p.SG) { as = 0; apar ^= 1; }
           }
-          commit_and_retire_previous(gs, -1);              // the whole group slot retires with these MMAs
-          if (++gs == p.SG) { gs = 0; gpar ^= 1; }
-          wgmma_fence();
+        } else {
+          for (int s0 = 0; s0 < nsteps; s0 += p.CG) {
+            const int n = min(p.CG, nsteps - s0);
+            mbar_wait(&g_full[gs], gpar);
+            const uint32_t base = smem_u32(sG + (size_t)gs * group_bytes);
+            for (int i = 0; i < n; ++i) {
+              const uint32_t b_base = p.b_resident ? sB_u32 + (s0 + i) * p.b_slot_bytes
+                                                   : base + p.CG * p.MG * p.a_slot_bytes + i * p.b_slot_bytes;
+              const uint32_t a_base = base + i * p.MG * p.a_slot_bytes;
+              uint32_t al = (a_base & 0x3FFFF) >> 4, bl = (b_base & 0x3FFFF) >> 4;
+              const int kk = cb == p.cblocks - 1 ? p.kmma_last : p.kmma;
+              if (++cb == p.cblocks) cb = 0;
+              // tap r reads the patch shifted by (r / RW) patch rows and (r % RW) pixels
+              for (int r0 = 0; r0 < p.R; r0 += p.RW, al += a_wrap) {
+                for (int r = 0; r < p.RW; ++r, al += a_step, bl += b_step) {
+                  mma_tap<BN, W, MG>(acc, a_d0 + al, b_d0 + bl, a_tile16, kk, ps_step, a_half16, b_half16, first);
+                  first = 1u;
+                }
+              }
+            }
+            commit_and_retire_previous(gs, -1);              // the whole group slot retires with these MMAs
+            if (++gs == p.SG) { gs = 0; gpar ^= 1; }
+            wgmma_fence();
+          }
         }
-      }
+      };
+      if (tail) k_loop(std::integral_constant<int, BNT>());
+      else k_loop(std::integral_constant<int, BN>());
       drain();
+      if (tail) {                                         // columns the tail MMAs did not write: padded output channels are zero
+#pragma unroll
+        for (int j = 0; j < MG; ++j)
+#pragma unroll
+          for (int i = BNT / 2; i < BN / 2; ++i) acc[j][i] = 0.f;
+      }
       __syncwarp();
       mbar_arrive_if(bres_empty, lane == 0 && p.b_resident && last_of_key);
 
@@ -598,16 +620,24 @@ int device_sm_count() {
   return n;
 }
 
-template <int BN, int MG>
+template <int BN, int BNT, int MG>
 static cudaError_t launch_bn_mg(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvKernelParams& p, size_t smem, cudaStream_t stream) {
   static size_t configured = 0;
   if (smem > configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<BN, MG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<BN, BNT, MG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     configured = smem;
   }
-  conv_umma_kernel<BN, MG><<<p.grid, kThreads, smem, stream>>>(tmA, tmB, p);
+  conv_umma_kernel<BN, BNT, MG><<<p.grid, kThreads, smem, stream>>>(tmA, tmB, p);
   return cudaGetLastError();
+}
+
+// The tail N tile's MMA width: its valid columns rounded up to 16 where a kernel instantiation has that width (the 7x7
+// stems over the 108-channel label input: 48 outputs in a 64-wide tile, 192 outputs in 128-wide tiles), else the full tile.
+int conv_umma_tail_width(const ConvKernelParams& p) {
+  const int w = (p.Cout - (p.n_tiles - 1) * p.BN + 15) / 16 * 16;
+  if ((p.BN == 64 && w == 48 && p.MG == 2) || (p.BN == 128 && w == 64 && p.MG == 1)) return w;
+  return p.BN;
 }
 
 size_t conv_umma_smem_bytes(const ConvKernelParams& p) {
@@ -621,14 +651,17 @@ cudaError_t launch_conv_umma(const CUtensorMap& tmA, const CUtensorMap& tmB, con
                              cudaStream_t stream) {
   const size_t smem = conv_umma_smem_bytes(p);
   // the N tile and the M blocking fix the accumulator registers: one instantiation per plan choice (V2V_MAX_ACC_COLS)
+  // (and the tail tile's MMA width BNt, conv_umma_tail_width)
   switch (p.BN * 4 + p.MG) {
-    case 16 * 4 + 1: return launch_bn_mg<16, 1>(tmA, tmB, p, smem, stream);
-    case 32 * 4 + 1: return launch_bn_mg<32, 1>(tmA, tmB, p, smem, stream);
-    case 32 * 4 + 2: return launch_bn_mg<32, 2>(tmA, tmB, p, smem, stream);
-    case 64 * 4 + 1: return launch_bn_mg<64, 1>(tmA, tmB, p, smem, stream);
-    case 64 * 4 + 2: return launch_bn_mg<64, 2>(tmA, tmB, p, smem, stream);
-    case 96 * 4 + 1: return launch_bn_mg<96, 1>(tmA, tmB, p, smem, stream);
-    case 128 * 4 + 1: return launch_bn_mg<128, 1>(tmA, tmB, p, smem, stream);
+    case 16 * 4 + 1: return launch_bn_mg<16, 16, 1>(tmA, tmB, p, smem, stream);
+    case 32 * 4 + 1: return launch_bn_mg<32, 32, 1>(tmA, tmB, p, smem, stream);
+    case 32 * 4 + 2: return launch_bn_mg<32, 32, 2>(tmA, tmB, p, smem, stream);
+    case 64 * 4 + 1: return launch_bn_mg<64, 64, 1>(tmA, tmB, p, smem, stream);
+    case 64 * 4 + 2: return p.BNt == 48 ? launch_bn_mg<64, 48, 2>(tmA, tmB, p, smem, stream)
+                                        : launch_bn_mg<64, 64, 2>(tmA, tmB, p, smem, stream);
+    case 96 * 4 + 1: return launch_bn_mg<96, 96, 1>(tmA, tmB, p, smem, stream);
+    case 128 * 4 + 1: return p.BNt == 64 ? launch_bn_mg<128, 64, 1>(tmA, tmB, p, smem, stream)
+                                         : launch_bn_mg<128, 128, 1>(tmA, tmB, p, smem, stream);
     default: return cudaErrorInvalidConfiguration;
   }
 }

@@ -692,6 +692,8 @@ static void fill_conv_params(v2v_plan* P, GOp& op) {
   kp.b_slot_bytes = sp * kp.b_half_bytes;
   kp.SB = kp.b_resident ? max_phase_groups(g) * kp.cblocks : 0;
   kp.n_tiles = (kp.Cout + kp.BN - 1) / kp.BN;
+  kp.kmma_last = std::min(kp.kmma, std::max(1, (c.Cin - (kp.cblocks - 1) * kp.kc + 15) / 16));
+  kp.BNt = conv_umma_tail_width(kp);
   kp.m_total = kp.N * (kp.tiles_x / kp.MG) * kp.tiles_y;       // M units: MG consecutive x tiles each
   kp.total_units = kp.m_total * kp.n_tiles * g.n_phases;
   kp.grid = std::min(kp.total_units, device_sm_count());
@@ -1756,10 +1758,10 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
     s += t;
     // the derived launch parameters the kernel reads (ctas: persistent CTAs launched; smem: dynamic shared memory)
     snprintf(t, sizeof(t),
-             "\"tiles_x\":%d,\"tiles_y\":%d,\"tile_dx\":%d,\"Cp\":%d,\"cblocks\":%d,\"row_bytes\":%d,\"kmma\":%d,\"layout_type\":%d,"
+             "\"tiles_x\":%d,\"tiles_y\":%d,\"tile_dx\":%d,\"Cp\":%d,\"cblocks\":%d,\"row_bytes\":%d,\"kmma\":%d,\"kmma_last\":%d,\"BNt\":%d,\"layout_type\":%d,"
              "\"sbo_bytes\":%d,\"sbo_a_bytes\":%d,\"RW\":%d,\"PW\":%d,\"PH\":%d,\"a_half_bytes\":%d,\"a_slot_bytes\":%d,"
              "\"b_half_bytes\":%d,\"b_slot_bytes\":%d,\"SB\":%d,\"n_tiles\":%d,\"m_total\":%d,\"ctas\":%d,\"Khalf\":%d,\"smem\":%zu}",
-             kp.tiles_x, kp.tiles_y, kp.tile_dx, kp.Cp, kp.cblocks, kp.row_bytes, kp.kmma, kp.layout_type, kp.sbo_bytes,
+             kp.tiles_x, kp.tiles_y, kp.tile_dx, kp.Cp, kp.cblocks, kp.row_bytes, kp.kmma, kp.kmma_last, kp.BNt, kp.layout_type, kp.sbo_bytes,
              kp.sbo_a_bytes, kp.RW, kp.PW, kp.PH, kp.a_half_bytes, kp.a_slot_bytes, kp.b_half_bytes, kp.b_slot_bytes, kp.SB,
              kp.n_tiles, kp.m_total, kp.grid, kp.Khalf, conv_umma_smem_bytes(kp));
     s += t;

@@ -109,6 +109,9 @@ struct ConvKernelParams {
   int Cout, BN;                      // valid output channels, N tile (16/32/64/128)
   int Cp, cblocks;                   // padded input channels, K blocks per tap (Cp / kc)
   int kc, row_bytes, kmma;           // channels per K block (16/32/64), smem row bytes (2*kc), MMAs per row (kc/16)
+  int kmma_last;                     // MMAs per row of the last K block: those that reach a real input channel (< Cin; the
+                                     // packed weights of the channels [Cin, Cp) are zero, so the skipped products are too)
+  int BNt;                           // MMA width of the last N tile: its valid columns rounded up to 16 (or BN)
   int layout_type, sbo_bytes;        // smem-descriptor swizzle code (6/4/2: 32B/64B/128B) and 8-row group stride (8*row_bytes)
   int R, RW;                         // taps served per A patch (1 = none); taps per patch row (tap r: row r / RW, column r % RW)
   int PW, PH;                        // patch extent in pixels (TMA box)
@@ -171,6 +174,7 @@ cudaError_t launch_conv_umma(const CUtensorMap& tmA, const CUtensorMap& tmB, con
 cudaError_t launch_conv_simt(const ActDesc& in, const bf16* wpacked, int Ktotal, const ConvKernelParams& p,
                              cudaStream_t stream);
 size_t conv_umma_smem_bytes(const ConvKernelParams& p);   // dynamic shared memory of one conv_umma_kernel launch
+int conv_umma_tail_width(const ConvKernelParams& p);      // ConvKernelParams::BNt of a conv_umma_kernel launch
 
 
 // ---------------------------------------------------------------------------------------
