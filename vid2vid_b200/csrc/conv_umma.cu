@@ -16,17 +16,23 @@
 // One CTA per SM walks tiles t = blockIdx.x, += gridDim.x (M fastest, so co-running CTAs share weights in L2).
 //   warps 0-7   two consumer warpgroups: warpgroup h issues the m64nBNk16 wgmmas of rows [64 h, 64 h + 64) of every M tile
 //               (MG tiles side by side, accumulators in registers), keeping one commit group in flight and handing each
-//               operand slot back to the producer as soon as the MMAs that read it have retired.  Both then drain the
-//               accumulators through a 128 x 64 fp32 shared-memory staging tile, so that in the epilogue thread
-//               (warp q = 0..3, lane) owns pixel row 32 q + lane and warps q / q + 4 take alternate 32-channel chunks:
+//               operand slot back to the producer as soon as the MMAs that read it have retired.  They then stage the
+//               accumulators through a 128 x 64 fp32 shared-memory staging tile, 64 columns at a time, into the epilogue:
+//               thread (warp q = 0..3 of warpgroup hc, lane) owns pixel row 32 q + lane and the two warpgroups take
+//               alternate 32-channel chunks:
 //     EPI_RAW_STATS : bf16 NHWC raw output + per-channel (sum, sumsq) of the tile for the following
 //                     Batch/InstanceNorm (deterministic fixed-point atomics)
 //     EPI_HEAD_F32  : bias + tanh/sigmoid/scale -> fp32 NCHW planes (the 7x7 image/flow/weight heads)
 //     EPI_ACT_BF16  : bias + (leaky)ReLU -> interior of the next layer's padded NHWC buffer
+//               and, in the last CTA to finish, the statistics finalisation.
 //   warps 8-11  producer warpgroup: one elected lane of warp 8 issues every TMA, warps 9-11 leave at once
-// Registers: the 384-thread block launches at 168 registers per thread (65536 / 384); setmaxnreg then lowers the
-// producer warpgroup to kProducerRegs and raises the two consumer warpgroups to kConsumerRegs (128 * 40 + 256 * 232 <=
-// 65536), so that the accumulators and the epilogue of every instantiation fit without spilling.
+//   warps 12-19 (ASYNC only) two epilogue warpgroups that run the epilogue instead of the consumers: they walk the same
+//               units, and each 64-column handoff goes stg_empty -> stage -> stg_full, so the consumers start the next unit's
+//               MMAs while the epilogue warpgroups store this one.  conv_umma_async_epilogue chooses per launch.
+// Registers: the 384-thread kernel launches at 168 registers per thread (65536 / 384); setmaxnreg lowers the producer
+// warpgroup to kProducerRegs and raises the consumers, which hold the accumulators and the epilogue, to kConsumerRegs
+// (128 * 40 + 256 * 232 <= 65536).  The ASYNC kernel launches 640 threads at 96 (65536 / 640, in steps of 8) and raises
+// the consumers to kConsumerRegsAsync (128 * 40 + 256 * 96 + 256 * 120 <= 640 * 96): at 96 the BN 128 consumers spill.
 // The kernel contains no call (no printf, no division slow path, see mbar_wait in ptx.cuh): ptxas would otherwise
 // serialise every wgmma, and the commit groups below would never overlap.
 #include <cstdlib>
@@ -39,8 +45,12 @@
 namespace v2v {
 
 static constexpr int kConsumerThreads = 256;              // two warpgroups
-static constexpr int kThreads = kConsumerThreads + 128;   // + the producer warpgroup
-static constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+static constexpr int kEpilogueThreads = 256;              // the two warpgroups that run the epilogue: consumers or epilogue warps
+// + the producer warpgroup, + the epilogue warpgroups in the ASYNC kernel
+constexpr int conv_threads(bool async) { return kConsumerThreads + 128 + (async ? kEpilogueThreads : 0); }
+// The consumers that run the epilogue themselves hold it and the accumulators (128 * 40 + 256 * 232 <= 65536); without it
+// they name no register above R92, so the ASYNC kernel keeps their launch share (65536 / 640 = 96 in steps of 8).
+static constexpr int kProducerRegs = 40, kConsumerRegs = 232, kConsumerRegsAsync = 120;
 static constexpr int kStgStride = 65;                     // floats per staging row: row-wise and column-wise walks are conflict free
 static constexpr int kStgFloats = 128 * kStgStride;       // 128 pixel rows x 64 accumulator columns
 static constexpr int kRedFloats = 4 * 2 * 128;            // [warp quarter][sum|sumsq][128 columns] running column sums
@@ -128,8 +138,8 @@ __device__ __forceinline__ void mma_tap(float (&acc)[MG][BN / 2], uint64_t ad, u
   }
 }
 
-template <int BN, int BNT, int MG>
-__global__ void __launch_bounds__(kThreads, 1)
+template <int BN, int BNT, int MG, bool ASYNC>
+__global__ void __launch_bounds__(conv_threads(ASYNC), 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ ConvKernelParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -147,10 +157,13 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* bars = reinterpret_cast<uint64_t*>(racc + kRedFloats);
   uint64_t* g_full = bars;
   uint64_t* g_empty = g_full + p.SG;
-  uint64_t* bres_full = g_empty + p.SG;
-  uint64_t* bres_empty = bres_full + 1;
-  uint64_t* b_full = bres_empty + 1;        // ring2: weight ring barriers [8] + [8]
+  uint64_t* stg_full = g_empty + p.SG;      // staging tile handoff: consumers -> epilogue warpgroups
+  uint64_t* stg_empty = stg_full + 1;       //                       epilogue warpgroups -> consumers
+  uint64_t* b_full = stg_empty + 1;         // ring2: weight ring barriers [8] + [8]
   uint64_t* b_empty = b_full + 8;
+  // a resident weight set and the decoupled weight ring never coexist: the resident set's pair is the ring's first pair
+  uint64_t* bres_full = b_full;
+  uint64_t* bres_empty = b_empty;
   uint32_t* ticket = reinterpret_cast<uint32_t*>(b_empty + 8);
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // (warp-uniform to the compiler)
@@ -160,17 +173,221 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < p.SG; ++i) { mbar_init(&g_full[i], 1); mbar_init(&g_empty[i], n_consumer_warps); }
-    mbar_init(bres_full, 1); mbar_init(bres_empty, n_consumer_warps);
-    if (p.ring2) for (int i = 0; i < p.SBr; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], n_consumer_warps); }
+    for (int i = 0; i < 8; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], n_consumer_warps); }
+    mbar_init(stg_full, n_consumer_warps); mbar_init(stg_empty, kEpilogueThreads / 32);
     fence_barrier_init();
   }
+  for (int i = threadIdx.x; i < kRedFloats; i += conv_threads(ASYNC)) racc[i] = 0.f;
   __syncthreads();
 
   const int a_tx = p.PW * p.PH * p.row_bytes;
   const int b_tx = p.BN * p.row_bytes;
   const int t_first = blockIdx.x, t_step = gridDim.x;
 
-  if (warp >= n_consumer_warps) {
+  // ---------------- the epilogue, run by 256 threads: the consumers themselves, or (ASYNC) the epilogue warpgroups while
+  // the consumers multiply the next unit.  Thread (warp q = 0..3 of warpgroup hc, lane) owns pixel row 32 q + lane of the
+  // staging tile; the two warpgroups take alternate 32-channel chunks.
+  const int q = warp & 3, hc = (warp >> 2) & 1;
+  const int row = q * 32 + lane;
+  const int etid = threadIdx.x - (ASYNC ? kConsumerThreads + 128 : 0);
+  constexpr int nchunks = BN / 32;
+  const int tw_shift = __ffs(p.TW) - 1;                   // TW is a power of two
+  const int ry = row >> tw_shift, rx = row & (p.TW - 1);
+  const bool do_stats = (p.epi == EPI_RAW_STATS) && (p.stats != nullptr);
+  // Statistics: running (sum, sumsq) per (warp quarter, column of the current N tile) in shared memory, flushed onto the
+  // image's statistics row when (phase, N tile, image) changes.  Every (quarter, column) has one writer warp.
+  int acc_key = -1, acc_img = -1, acc_n0 = 0;
+  // flush() publishes the running sums and zeroes them again: thread c owns column c of every quarter.
+  auto flush = [&]() {
+    named_bar_sync(1, kEpilogueThreads);                // every warp has added its last tile
+    if (etid < p.BN) {
+      float s = 0.f, qq = 0.f;
+#pragma unroll
+      for (int w = 0; w < 4; ++w) {
+        s += racc[(w * 2 + 0) * 128 + etid];
+        qq += racc[(w * 2 + 1) * 128 + etid];
+        racc[(w * 2 + 0) * 128 + etid] = 0.f;
+        racc[(w * 2 + 1) * 128 + etid] = 0.f;
+      }
+      // 64-bit fixed-point integer atomics onto the image's single statistics row: order independent (deterministic)
+      if (acc_n0 + etid < p.stats_C) {
+        atomicAdd(&p.stats[((size_t)acc_img * 2 + 0) * p.stats_C + acc_n0 + etid], (stat_t)__float2ll_rn(s * V2V_STAT_SUM_SCALE));
+        atomicAdd(&p.stats[((size_t)acc_img * 2 + 1) * p.stats_C + acc_n0 + etid], (stat_t)__float2ll_rn(qq * V2V_STAT_SQ_SCALE));
+      }
+    }
+    named_bar_sync(1, kEpilogueThreads);                // every column is zero again
+  };
+  // One work unit: handoff(jt, c0) makes accumulator columns [c0, c0 + 64) of tile jt readable in the staging tile, done()
+  // lets it be overwritten again.
+  auto epilogue_unit = [&](const ConvPhase& ph, int key, int y0, int x0, int n0, int n_img, auto handoff, auto done) {
+      const int gy = y0 + ry, gx0 = x0 + rx;
+      const int oy = gy * p.oy_mul + ph.oy_add;
+#pragma unroll
+      for (int jt = 0; jt < MG; ++jt) {                   // the unit's MG tiles sit side by side along x
+        const int gx = gx0 + jt * p.TW;
+        const bool valid = (gy < p.grid_h) && (gx < p.grid_w);
+        const int ox = gx * p.ox_mul + ph.ox_add;
+        bf16* dst = nullptr;
+        float* dstf = nullptr;
+        if (valid && p.epi != EPI_HEAD_F32) {
+          const size_t pix_off = (((size_t)n_img * p.out_H + oy) * p.out_W + ox) * p.out_C;
+          if (p.epi == EPI_RAW_STATS) {
+            if (p.out_f32) dstf = reinterpret_cast<float*>(p.out) + pix_off;
+            else dst = reinterpret_cast<bf16*>(p.out) + pix_off;
+          } else {
+            dst = p.out_act.base + p.out_act.offset(n_img, oy, ox);
+          }
+        }
+        const float* srow = stg + row * kStgStride;
+
+        if (p.epi == EPI_HEAD_F32 && p.headkx) {
+          // kx-GEMM head.  Tile = 4 rows x 32 INPUT pixels: warp quarter q = tile row, lane = pixel, accumulator column
+          // kx * Cout + c.  out(x)[c] = sum_kx D[x + kx][kx * Cout + c] is a sum over the NEXT kw - 1 lanes of the same
+          // warp: warp shuffles.  Lanes 32 - (kw - 1) .. 31 only feed their left neighbours (tiles advance by
+          // tile_dx = 32 - (kw - 1) pixels).
+          handoff(jt, 0);
+          if (hc == 0) {
+            uint32_t r[32];
+#pragma unroll
+            for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(srow[j]);
+            float hacc[4];
+            switch (p.Cout) {
+              case 1: head_shift_sum<1>(r, p.headkx, hacc); break;
+              case 2: head_shift_sum<2>(r, p.headkx, hacc); break;
+              case 3: head_shift_sum<3>(r, p.headkx, hacc); break;
+              default: head_shift_sum<4>(r, p.headkx, hacc); break;
+            }
+            if (valid && rx < p.tile_dx) {
+              const size_t pix = (size_t)oy * p.out_W + ox;
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                if (j < p.Cout) {
+                  float v = hacc[j];
+                  if (p.bias) v += (p.bias2 && j >= p.Cout1) ? __ldg(p.bias2 + j - p.Cout1) : __ldg(p.bias + j);
+                  v = apply_act(v, p.head_act[j], p.lrelu_slope) * p.head_scale[j];
+                  reinterpret_cast<float*>(p.io[p.head_slot[j]])[p.head_off[j] + (size_t)n_img * p.head_bstride[j] + pix] = v;
+                }
+              }
+            }
+          }
+          done();
+          continue;
+        }
+        if (p.epi == EPI_HEAD_F32) {
+          handoff(jt, 0);
+          if (hc == 0 && valid) {
+            const size_t pix = (size_t)oy * p.out_W + ox;
+#pragma unroll
+            for (int j = 0; j < V2V_MAX_HEAD; ++j) {
+              if (j < p.Cout) {
+                float v = srow[j];
+                if (p.bias) v += (p.bias2 && j >= p.Cout1) ? __ldg(p.bias2 + j - p.Cout1) : __ldg(p.bias + j);
+                v = apply_act(v, p.head_act[j], p.lrelu_slope) * p.head_scale[j];
+                reinterpret_cast<float*>(p.io[p.head_slot[j]])[p.head_off[j] + (size_t)n_img * p.head_bstride[j] + pix] = v;
+              }
+            }
+          }
+          done();
+          continue;
+        }
+
+        if (do_stats && (key != acc_key || n_img != acc_img)) {
+          if (acc_key >= 0) flush();
+          acc_key = key; acc_img = n_img; acc_n0 = n0;
+        }
+        // one handoff per 64 staged columns: chunk c0 + hc of 32
+        for (int c0 = 0; c0 < nchunks; c0 += 2) {
+          handoff(jt, c0 * 32);
+          const int c = c0 + hc;
+          if (c < nchunks) {
+            float v[32];
+            const int col0 = n0 + c * 32;
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] = valid ? srow[hc * 32 + j] : 0.f;
+            if (p.epi == EPI_ACT_BF16) {
+#pragma unroll
+              for (int j = 0; j < 32; ++j) {
+                float b = (p.bias && col0 + j < p.Cout) ? __ldg(p.bias + col0 + j) : 0.f;
+                v[j] = (col0 + j < p.Cout) ? apply_act(v[j] + b, p.act, p.lrelu_slope) : 0.f;
+              }
+            }
+            if (valid) {
+              if (dstf) {                                // precise plan: fp32 raw output
+#pragma unroll
+                for (int qv = 0; qv < 8; ++qv)
+                  if (col0 + qv * 4 < p.out_C)
+                    *reinterpret_cast<float4*>(dstf + col0 + qv * 4) = make_float4(v[qv * 4], v[qv * 4 + 1], v[qv * 4 + 2], v[qv * 4 + 3]);
+              } else if (p.epi == EPI_ACT_BF16 && p.out_act.split) {
+#pragma unroll
+                for (int qv = 0; qv < 4; ++qv) {
+                  if (col0 + qv * 8 < p.out_C) {
+                    float lo[8];
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) lo[j] = v[qv * 8 + j] - __bfloat162float(__float2bfloat16_rn(v[qv * 8 + j]));
+                    uint4 pk, pl;
+                    pk.x = pack_bf16x2(v[qv * 8 + 0], v[qv * 8 + 1]); pl.x = pack_bf16x2(lo[0], lo[1]);
+                    pk.y = pack_bf16x2(v[qv * 8 + 2], v[qv * 8 + 3]); pl.y = pack_bf16x2(lo[2], lo[3]);
+                    pk.z = pack_bf16x2(v[qv * 8 + 4], v[qv * 8 + 5]); pl.z = pack_bf16x2(lo[4], lo[5]);
+                    pk.w = pack_bf16x2(v[qv * 8 + 6], v[qv * 8 + 7]); pl.w = pack_bf16x2(lo[6], lo[7]);
+                    *reinterpret_cast<uint4*>(dst + col0 + qv * 8) = pk;
+                    *reinterpret_cast<uint4*>(dst + p.out_act.C + col0 + qv * 8) = pl;
+                  }
+                }
+              } else {
+#pragma unroll
+                for (int qv = 0; qv < 4; ++qv) {
+                  if (col0 + qv * 8 < p.out_C) {
+                    uint4 pk;
+                    pk.x = pack_bf16x2(v[qv * 8 + 0], v[qv * 8 + 1]);
+                    pk.y = pack_bf16x2(v[qv * 8 + 2], v[qv * 8 + 3]);
+                    pk.z = pack_bf16x2(v[qv * 8 + 4], v[qv * 8 + 5]);
+                    pk.w = pack_bf16x2(v[qv * 8 + 6], v[qv * 8 + 7]);
+                    *reinterpret_cast<uint4*>(dst + col0 + qv * 8) = pk;
+                  }
+                }
+              }
+            }
+            if (do_stats) {
+              // column sums over this warp's 32 rows: each lane writes its (masked) row back into the staging tile, then
+              // lane l walks column l down the 32 rows (banks (r + l) mod 32: conflict free)
+              float* sw = stg + hc * 32;
+#pragma unroll
+              for (int j = 0; j < 32; ++j) sw[row * kStgStride + j] = v[j];
+              __syncwarp();
+              float s = 0.f, qq = 0.f;
+#pragma unroll
+              for (int r2 = 0; r2 < 32; ++r2) {
+                const float x = sw[(q * 32 + r2) * kStgStride + lane];
+                s += x;
+                qq = fmaf(x, x, qq);
+              }
+              racc[(q * 2 + 0) * 128 + c * 32 + lane] += s;
+              racc[(q * 2 + 1) * 128 + c * 32 + lane] += qq;
+            }
+          }
+          done();
+        }
+      }
+  };
+  auto epilogue_end = [&]() {
+    if (do_stats && acc_key >= 0) flush();
+
+    __threadfence();                                // this thread's statistics atomics are visible device-wide
+    if (p.n_fin > 0) {
+      // Statistics finalisation by the LAST CTA to get here (ticket counter, zeroed with the statistics rows before every
+      // run): all rows are complete then; every other CTA has exited, nobody waits.  Only these warpgroups wrote statistics.
+      named_bar_sync(1, kEpilogueThreads);
+      if (etid == 0) *ticket = atomicAdd(p.fin_counter, 1u);
+      named_bar_sync(1, kEpilogueThreads);
+      if (*ticket == gridDim.x - 1) {
+        __threadfence();
+        for (int f = 0; f < p.n_fin; ++f)
+          for (int c = etid; c < p.fin[f].C; c += kEpilogueThreads) channel_side_effects(p.fin[f], c);
+      }
+    }
+  };
+
+  if (warp >= n_consumer_warps && warp < n_consumer_warps + 4) {
     setmaxnreg_dec<kProducerRegs>();
     if (warp == n_consumer_warps && elect_one_sync()) {
       // ---------------------------------------------------------- TMA producer (single elected lane)
@@ -258,12 +475,10 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else {
-    // ------------------------------------------------------------ consumers: wgmma issue + epilogue
-    setmaxnreg_inc<kConsumerRegs>();
+  } else if (warp < n_consumer_warps) {
+    // ------------------------------------------------------------ consumers: wgmma issue, accumulators -> staging tile
+    setmaxnreg_inc<ASYNC ? kConsumerRegsAsync : kConsumerRegs>();
     const int wg = warp >> 2;                             // M half of the tile this warpgroup multiplies
-    const int q = warp & 3, hc = wg;                      // epilogue: pixel rows 32 q .. 32 q + 31, chunk parity hc
-    const int row = q * 32 + lane;
     const int ps_step = p.split ? (p.a_exact ? 2 : 1) : 3;    // 3 = one pass (fast), 1 = three passes, 2 = {hi*hi, hi*lo}
     const uint32_t a_half16 = (uint32_t)(p.a_half_bytes >> 4), b_half16 = (uint32_t)(p.b_half_bytes >> 4);
     const uint32_t a_tile16 = (uint32_t)(p.a_slot_bytes >> 4);
@@ -275,10 +490,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const uint32_t a_wrap = (uint32_t)(((p.PW - p.RW) * p.row_bytes) >> 4);     // to the next patch row
     const uint32_t row16 = (uint32_t)(p.row_bytes >> 4), prow16 = (uint32_t)((p.PW * p.row_bytes) >> 4);
     const uint32_t sB_u32 = smem_u32(sBres);
-    const bool do_stats = (p.epi == EPI_RAW_STATS) && (p.stats != nullptr);
-    const int nchunks = p.BN / 32;
-    const int tw_shift = __ffs(p.TW) - 1;                 // TW is a power of two
-    const int ry = row >> tw_shift, rx = row & (p.TW - 1);
 
     float acc[MG][BN / 2];
     // Operand slots retire one commit group late: after committing group k the warpgroup waits for group k - 1 only, so
@@ -302,31 +513,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
       for (int j = 0; j < MG; ++j) wgmma_fence_operands(acc[j]);
     };
-    // Statistics: running (sum, sumsq) per (warp quarter, column of the current N tile) in shared memory, flushed onto the
-    // image's statistics row when (phase, N tile, image) changes.  Every (quarter, column) has one writer warp.
-    int acc_key = -1, acc_img = -1, acc_n0 = 0;
-    // flush() publishes the running sums and zeroes them again: thread c owns column c of every quarter.
-    auto flush = [&]() {
-      named_bar_sync(1, kConsumerThreads);                // every warp has added its last tile
-      const int etid = threadIdx.x;
-      if (etid < p.BN) {
-        float s = 0.f, qq = 0.f;
-#pragma unroll
-        for (int w = 0; w < 4; ++w) {
-          s += racc[(w * 2 + 0) * 128 + etid];
-          qq += racc[(w * 2 + 1) * 128 + etid];
-          racc[(w * 2 + 0) * 128 + etid] = 0.f;
-          racc[(w * 2 + 1) * 128 + etid] = 0.f;
-        }
-        // 64-bit fixed-point integer atomics onto the image's single statistics row: order independent (deterministic)
-        if (acc_n0 + etid < p.stats_C) {
-          atomicAdd(&p.stats[((size_t)acc_img * 2 + 0) * p.stats_C + acc_n0 + etid], (stat_t)__float2ll_rn(s * V2V_STAT_SUM_SCALE));
-          atomicAdd(&p.stats[((size_t)acc_img * 2 + 1) * p.stats_C + acc_n0 + etid], (stat_t)__float2ll_rn(qq * V2V_STAT_SQ_SCALE));
-        }
-      }
-      named_bar_sync(1, kConsumerThreads);                // every column is zero again
-    };
-    for (int i = threadIdx.x; i < kRedFloats; i += kConsumerThreads) racc[i] = 0.f;    // (ordered by the first stage())
     // accumulator columns [c0, c0 + 64) of tile jt -> staging rows (the wgmma fragment layout, see wgmma.cuh)
     auto stage = [&](int jt, int c0) {
 #pragma unroll
@@ -342,8 +528,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           stg[(r0 + 8) * kStgStride + col + 1] = acc[j][b * 4 + 3];
         }
       }
-      named_bar_sync(1, kConsumerThreads);
     };
+    uint32_t stg_par = 0;                                 // ASYNC: handoffs to the epilogue warpgroups
 
     int gs = 0, as = 0, bs = 0;
     uint32_t gpar = 0, gen = 0, apar = 0, bpar = 0;
@@ -442,170 +628,35 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       __syncwarp();
       mbar_arrive_if(bres_empty, lane == 0 && p.b_resident && last_of_key);
 
-      // ---------------- epilogue
-      const int gy = y0 + ry, gx0 = x0 + rx;
-      const int oy = gy * p.oy_mul + ph.oy_add;
+      if (ASYNC) {
+        // hand the accumulators to the epilogue warpgroups, 64 columns at a time, once they have read the previous ones
 #pragma unroll
-      for (int jt = 0; jt < MG; ++jt) {                   // the unit's MG tiles sit side by side along x
-        const int gx = gx0 + jt * p.TW;
-        const bool valid = (gy < p.grid_h) && (gx < p.grid_w);
-        const int ox = gx * p.ox_mul + ph.ox_add;
-        bf16* dst = nullptr;
-        float* dstf = nullptr;
-        if (valid && p.epi != EPI_HEAD_F32) {
-          const size_t pix_off = (((size_t)n_img * p.out_H + oy) * p.out_W + ox) * p.out_C;
-          if (p.epi == EPI_RAW_STATS) {
-            if (p.out_f32) dstf = reinterpret_cast<float*>(p.out) + pix_off;
-            else dst = reinterpret_cast<bf16*>(p.out) + pix_off;
-          } else {
-            dst = p.out_act.base + p.out_act.offset(n_img, oy, ox);
+        for (int jt = 0; jt < MG; ++jt)
+#pragma unroll
+          for (int c0 = 0; c0 < BN; c0 += 64) {
+            mbar_wait(stg_empty, stg_par ^ 1);
+            stg_par ^= 1;
+            stage(jt, c0);
+            __syncwarp();
+            mbar_arrive_if(stg_full, lane == 0);
           }
-        }
-        const float* srow = stg + row * kStgStride;
-
-        if (p.epi == EPI_HEAD_F32 && p.headkx) {
-          // kx-GEMM head.  Tile = 4 rows x 32 INPUT pixels: warp quarter q = tile row, lane = pixel, accumulator column
-          // kx * Cout + c.  out(x)[c] = sum_kx D[x + kx][kx * Cout + c] is a sum over the NEXT kw - 1 lanes of the same
-          // warp: warp shuffles.  Lanes 32 - (kw - 1) .. 31 only feed their left neighbours (tiles advance by
-          // tile_dx = 32 - (kw - 1) pixels).
-          stage(jt, 0);
-          if (hc == 0) {
-            uint32_t r[32];
-#pragma unroll
-            for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(srow[j]);
-            float hacc[4];
-            switch (p.Cout) {
-              case 1: head_shift_sum<1>(r, p.headkx, hacc); break;
-              case 2: head_shift_sum<2>(r, p.headkx, hacc); break;
-              case 3: head_shift_sum<3>(r, p.headkx, hacc); break;
-              default: head_shift_sum<4>(r, p.headkx, hacc); break;
-            }
-            if (valid && rx < p.tile_dx) {
-              const size_t pix = (size_t)oy * p.out_W + ox;
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                if (j < p.Cout) {
-                  float v = hacc[j];
-                  if (p.bias) v += (p.bias2 && j >= p.Cout1) ? __ldg(p.bias2 + j - p.Cout1) : __ldg(p.bias + j);
-                  v = apply_act(v, p.head_act[j], p.lrelu_slope) * p.head_scale[j];
-                  reinterpret_cast<float*>(p.io[p.head_slot[j]])[p.head_off[j] + (size_t)n_img * p.head_bstride[j] + pix] = v;
-                }
-              }
-            }
-          }
-          named_bar_sync(1, kConsumerThreads);
-          continue;
-        }
-        if (p.epi == EPI_HEAD_F32) {
-          stage(jt, 0);
-          if (hc == 0 && valid) {
-            const size_t pix = (size_t)oy * p.out_W + ox;
-#pragma unroll
-            for (int j = 0; j < V2V_MAX_HEAD; ++j) {
-              if (j < p.Cout) {
-                float v = srow[j];
-                if (p.bias) v += (p.bias2 && j >= p.Cout1) ? __ldg(p.bias2 + j - p.Cout1) : __ldg(p.bias + j);
-                v = apply_act(v, p.head_act[j], p.lrelu_slope) * p.head_scale[j];
-                reinterpret_cast<float*>(p.io[p.head_slot[j]])[p.head_off[j] + (size_t)n_img * p.head_bstride[j] + pix] = v;
-              }
-            }
-          }
-          named_bar_sync(1, kConsumerThreads);
-          continue;
-        }
-
-        if (do_stats && (key != acc_key || n_img != acc_img)) {
-          if (acc_key >= 0) flush();
-          acc_key = key; acc_img = n_img; acc_n0 = n0;
-        }
-        for (int c0 = 0; c0 < nchunks; c0 += 2) {
-          stage(jt, c0 * 32);
-          const int c = c0 + hc;
-          if (c < nchunks) {
-            float v[32];
-            const int col0 = n0 + c * 32;
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = valid ? srow[hc * 32 + j] : 0.f;
-            if (p.epi == EPI_ACT_BF16) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                float b = (p.bias && col0 + j < p.Cout) ? __ldg(p.bias + col0 + j) : 0.f;
-                v[j] = (col0 + j < p.Cout) ? apply_act(v[j] + b, p.act, p.lrelu_slope) : 0.f;
-              }
-            }
-            if (valid) {
-              if (dstf) {                                // precise plan: fp32 raw output
-#pragma unroll
-                for (int qv = 0; qv < 8; ++qv)
-                  if (col0 + qv * 4 < p.out_C)
-                    *reinterpret_cast<float4*>(dstf + col0 + qv * 4) = make_float4(v[qv * 4], v[qv * 4 + 1], v[qv * 4 + 2], v[qv * 4 + 3]);
-              } else if (p.epi == EPI_ACT_BF16 && p.out_act.split) {
-#pragma unroll
-                for (int qv = 0; qv < 4; ++qv) {
-                  if (col0 + qv * 8 < p.out_C) {
-                    float lo[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) lo[j] = v[qv * 8 + j] - __bfloat162float(__float2bfloat16_rn(v[qv * 8 + j]));
-                    uint4 pk, pl;
-                    pk.x = pack_bf16x2(v[qv * 8 + 0], v[qv * 8 + 1]); pl.x = pack_bf16x2(lo[0], lo[1]);
-                    pk.y = pack_bf16x2(v[qv * 8 + 2], v[qv * 8 + 3]); pl.y = pack_bf16x2(lo[2], lo[3]);
-                    pk.z = pack_bf16x2(v[qv * 8 + 4], v[qv * 8 + 5]); pl.z = pack_bf16x2(lo[4], lo[5]);
-                    pk.w = pack_bf16x2(v[qv * 8 + 6], v[qv * 8 + 7]); pl.w = pack_bf16x2(lo[6], lo[7]);
-                    *reinterpret_cast<uint4*>(dst + col0 + qv * 8) = pk;
-                    *reinterpret_cast<uint4*>(dst + p.out_act.C + col0 + qv * 8) = pl;
-                  }
-                }
-              } else {
-#pragma unroll
-                for (int qv = 0; qv < 4; ++qv) {
-                  if (col0 + qv * 8 < p.out_C) {
-                    uint4 pk;
-                    pk.x = pack_bf16x2(v[qv * 8 + 0], v[qv * 8 + 1]);
-                    pk.y = pack_bf16x2(v[qv * 8 + 2], v[qv * 8 + 3]);
-                    pk.z = pack_bf16x2(v[qv * 8 + 4], v[qv * 8 + 5]);
-                    pk.w = pack_bf16x2(v[qv * 8 + 6], v[qv * 8 + 7]);
-                    *reinterpret_cast<uint4*>(dst + col0 + qv * 8) = pk;
-                  }
-                }
-              }
-            }
-            if (do_stats) {
-              // column sums over this warp's 32 rows: each lane writes its (masked) row back into the staging tile, then
-              // lane l walks column l down the 32 rows (banks (r + l) mod 32: conflict free)
-              float* sw = stg + hc * 32;
-#pragma unroll
-              for (int j = 0; j < 32; ++j) sw[row * kStgStride + j] = v[j];
-              __syncwarp();
-              float s = 0.f, qq = 0.f;
-#pragma unroll
-              for (int r2 = 0; r2 < 32; ++r2) {
-                const float x = sw[(q * 32 + r2) * kStgStride + lane];
-                s += x;
-                qq = fmaf(x, x, qq);
-              }
-              racc[(q * 2 + 0) * 128 + c * 32 + lane] += s;
-              racc[(q * 2 + 1) * 128 + c * 32 + lane] += qq;
-            }
-          }
-          named_bar_sync(1, kConsumerThreads);             // the staging tile may be overwritten
-        }
+      } else {
+        epilogue_unit(ph, key, y0, x0, n0, n_img,
+                      [&](int jt, int c0) { stage(jt, c0); named_bar_sync(1, kConsumerThreads); },
+                      [&]() { named_bar_sync(1, kConsumerThreads); });   // the staging tile may be overwritten
       }
     }
-    if (do_stats && acc_key >= 0) flush();
-
-    __threadfence();                                // this thread's statistics atomics are visible device-wide
-    if (p.n_fin > 0) {
-      // Statistics finalisation by the LAST CTA to get here (ticket counter, zeroed with the statistics rows before every
-      // run): all rows are complete then; every other CTA has exited, nobody waits.  Only the consumers wrote statistics.
-      named_bar_sync(1, kConsumerThreads);
-      if (threadIdx.x == 0) *ticket = atomicAdd(p.fin_counter, 1u);
-      named_bar_sync(1, kConsumerThreads);
-      if (*ticket == gridDim.x - 1) {
-        __threadfence();
-        for (int f = 0; f < p.n_fin; ++f)
-          for (int c = threadIdx.x; c < p.fin[f].C; c += kConsumerThreads) channel_side_effects(p.fin[f], c);
-      }
-    }
+    if (!ASYNC) epilogue_end();
+  } else if (ASYNC) {
+    // ------------------------------------------------------------ epilogue warpgroups: staging tile -> outputs, statistics
+    uint32_t stg_par = 0;
+    UnitIter un;
+    un.init(p, t_first, t_step);
+    for (; un.valid(p); un.next(p))
+      epilogue_unit(p.phases[un.phase], un.key, un.y0(p), un.x0(p), un.n0(p), un.img,
+                    [&](int, int) { mbar_wait_sleep(stg_full, stg_par); stg_par ^= 1; },
+                    [&]() { __syncwarp(); mbar_arrive_if(stg_empty, lane == 0); });
+    epilogue_end();
   }
 }
 
@@ -620,17 +671,30 @@ int device_sm_count() {
   return n;
 }
 
-template <int BN, int BNT, int MG>
-static cudaError_t launch_bn_mg(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvKernelParams& p, size_t smem, cudaStream_t stream) {
+template <int BN, int BNT, int MG, bool ASYNC>
+static cudaError_t launch_kernel(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvKernelParams& p, size_t smem, cudaStream_t stream) {
   static size_t configured = 0;
   if (smem > configured) {
-    cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<BN, BNT, MG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(conv_umma_kernel<BN, BNT, MG, ASYNC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     configured = smem;
   }
-  conv_umma_kernel<BN, BNT, MG><<<p.grid, kThreads, smem, stream>>>(tmA, tmB, p);
+  conv_umma_kernel<BN, BNT, MG, ASYNC><<<p.grid, conv_threads(ASYNC), smem, stream>>>(tmA, tmB, p);
   return cudaGetLastError();
 }
+
+template <int BN, int BNT, int MG>
+static cudaError_t launch_bn_mg(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvKernelParams& p, size_t smem, cudaStream_t stream) {
+  if constexpr (MG == 1)
+    if (conv_umma_async_epilogue(p)) return launch_kernel<BN, BNT, MG, true>(tmA, tmB, p, smem, stream);
+  return launch_kernel<BN, BNT, MG, false>(tmA, tmB, p, smem, stream);
+}
+
+// Epilogue warpgroups pay where the consumers have a next unit to multiply while a unit is stored: single-tile units (MG 1)
+// and at least two units per CTA.  M-blocked units (the 7x7 stems over the 108-channel input) keep the consumers' epilogue:
+// on the epilogue warpgroups the three-pass stems were 25-32 % slower (tools/time_conv.py, DESIGN §7); so were plans with
+// one unit per CTA, which have nothing to overlap.
+int conv_umma_async_epilogue(const ConvKernelParams& p) { return p.MG == 1 && p.total_units >= 2 * p.grid; }
 
 // The tail N tile's MMA width: its valid columns rounded up to 16 where a kernel instantiation has that width (the 7x7
 // stems over the 108-channel label input: 48 outputs in a 64-wide tile, 192 outputs in 128-wide tiles), else the full tile.
@@ -649,6 +713,8 @@ size_t conv_umma_smem_bytes(const ConvKernelParams& p) {
 
 cudaError_t launch_conv_umma(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvKernelParams& p,
                              cudaStream_t stream) {
+  // the resident weight set's barrier pair is the decoupled weight ring's first pair
+  if (p.b_resident && p.ring2) return cudaErrorInvalidConfiguration;
   const size_t smem = conv_umma_smem_bytes(p);
   // the N tile and the M blocking fix the accumulator registers: one instantiation per plan choice (V2V_MAX_ACC_COLS)
   // (and the tail tile's MMA width BNt, conv_umma_tail_width)

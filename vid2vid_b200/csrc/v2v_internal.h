@@ -175,6 +175,7 @@ cudaError_t launch_conv_simt(const ActDesc& in, const bf16* wpacked, int Ktotal,
                              cudaStream_t stream);
 size_t conv_umma_smem_bytes(const ConvKernelParams& p);   // dynamic shared memory of one conv_umma_kernel launch
 int conv_umma_tail_width(const ConvKernelParams& p);      // ConvKernelParams::BNt of a conv_umma_kernel launch
+int conv_umma_async_epilogue(const ConvKernelParams& p);  // 1: the launch stores its units on epilogue warpgroups
 
 
 // ---------------------------------------------------------------------------------------
