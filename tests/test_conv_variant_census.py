@@ -20,14 +20,15 @@ from vid2vid_b200.plan import Plan
 
 H100_SXM_SMS = 132
 
-Variant = collections.namedtuple('Variant', 'kind patch R multi_phase BN kc MG resident split a_exact ring2 TB headkx')
+Variant = collections.namedtuple('Variant', 'kind patch R multi_phase BN kc MG resident split a_exact ring2 TB headkx async_epi')
 
 
 def variant(c):
     """The fields of a described conv that select a code path of the kernel (the stage / commit-group / unit counts CG, SG,
-    SBr and units only tune it)."""
+    SBr and units only tune it; async_epi selects the 640-thread instantiation whose epilogue warpgroup stores each unit
+    while the consumers multiply the next)."""
     return Variant(c['kind'], c['p2d'], c['R'], int(c['phases'] > 1), c['BN'], c['kc'], c['MG'], c['resident'], c['split'],
-                   c['a_exact'], c['ring2'], c['TB'], c['headkx'])
+                   c['a_exact'], c['ring2'], c['TB'], c['headkx'], c['async_epi'])
 
 
 @pytest.fixture(autouse=True)

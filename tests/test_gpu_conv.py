@@ -174,11 +174,11 @@ def test_head(name, build, head, scale, shape, mode):
 LR01 = lambda: nn.LeakyReLU(0.1, True)
 VARIANT_CASES = [
     ('stem_6_128_ring2_tb4', lambda: NW._stem(6, 128, BN), (1, 6, 160, 512), ['precise'], False),
-    ('stem_6_128_kc16_bn128', lambda: NW._stem(6, 128, BN), (1, 6, 8, 128), ['fast'], False),
-    ('stem_6_64_mg2_kc16', lambda: NW._stem(6, 64, BN), (1, 6, 160, 512), ['precise'], False),
+    ('stem_6_128_kc16_bn128', lambda: NW._stem(6, 128, BN), (1, 6, 256, 512), ['fast'], False),
+    ('stem_6_64_mg2_kc16', lambda: NW._stem(6, 64, BN), (1, 6, 512, 1024), MODES, False),
     ('stem_108_48_exact_mg2', lambda: NW._stem(108, 48, BN), (1, 108, 160, 512), ['precise'], True),
     ('stem_108_96_exact_kc32', lambda: NW._stem(108, 96, BN), (1, 108, 160, 512), ['precise'], True),
-    ('s2_16_32_resident_kc16', lambda: NW._down(16, 32, BN), (1, 16, 160, 512), MODES, False),
+    ('s2_16_32_resident_kc16', lambda: NW._down(16, 32, BN), (1, 16, 1024, 2048), MODES, False),
     ('s2_64_128_resident', lambda: NW._down(64, 128, BN), (1, 64, 160, 512), ['fast'], False),
     ('deconv_32_16_resident', lambda: NW._up(32, 16, BN), (1, 32, 160, 128), MODES, False),
     ('deconv_128_64_resident', lambda: NW._up(128, 64, BN), (1, 128, 160, 128), ['fast'], False),
@@ -195,7 +195,17 @@ VARIANT_CASES = [
      (1, 6, 128, 256), ['precise'], False),
     ('fn_194_64_ring2_tb2', lambda: [nn.Conv2d(194, 64, 3, padding=1), BN(64), LR01()], (1, 194, 128, 256), ['precise'], False),
     ('fn_162_32_stream', lambda: [nn.Conv2d(162, 32, 3, padding=1), BN(32), LR01()], (1, 162, 256, 512), ['precise'], False),
-    ('fn_16_2_kc16_resident', lambda: [nn.Conv2d(16, 2, 3, padding=1), BN(2), LR01()], (1, 16, 128, 256), ['precise'], False),
+    ('fn_16_2_kc16_resident', lambda: [nn.Conv2d(16, 2, 3, padding=1), BN(2), LR01()], (1, 16, 512, 1024), ['precise'], False),
+    # large grids: enough units per CTA for the epilogue warpgroup (async_epi), at the sizes the benchmark runs the layers
+    ('d_first_39_async_512x1024', lambda: [nn.Conv2d(39, 64, 4, stride=2, padding=2), nn.LeakyReLU(0.2, True)], (1, 39, 512, 1024),
+     ['precise'], False),
+    ('d_k4_256_512_ring2_tb1', lambda: [nn.Conv2d(256, 512, 4, stride=1, padding=2), BN(512), nn.LeakyReLU(0.2, True)], (1, 256, 33, 65),
+     ['precise'], False),
+    ('g1_64_128_s2_256x512', lambda: NW._down(64, 128, BN), (1, 64, 512, 1024), MODES, False),
+    ('g2_res32_512x1024', lambda: [NW.ResnetBlock(32, 'reflect', BN)], (1, 32, 512, 1024), MODES, False),
+    ('fn_c1_3_64_k7s2_async', lambda: [nn.Conv2d(3, 64, 7, stride=2, padding=3), BN(64), LR01()], (1, 3, 512, 1024), ['precise'], False),
+    ('fn_6_64_s2_async_512x1024', lambda: [nn.Conv2d(6, 64, 3, padding=1), BN(64), LR01(), nn.Conv2d(64, 64, 3, stride=2, padding=1), BN(64),
+                                            LR01()], (1, 6, 512, 1024), ['precise'], False),
 ]
 
 
@@ -210,10 +220,16 @@ def test_conv_variant(name, build, shape, mode, exact):
 # name, layer list builder, head builder, head scale, input shape, modes
 VARIANT_HEADS = [
     # the finest scale's 16 -> 3 image head: kx-GEMM with a 16-channel K block, resident weights
-    ('head_16_3_headkx_kc16', lambda: NW._stem(8, 16, BN), lambda: NW._head(16, 3, nn.Tanh()), 1.0, (1, 8, 16, 1024), MODES),
+    ('head_16_3_headkx_kc16', lambda: NW._stem(8, 16, BN), lambda: NW._head(16, 3, nn.Tanh()), 1.0, (1, 8, 1024, 2048), MODES),
     # the discriminators' last two layers: 4x4 stride-1 conv on the decoupled rings, then the 1-channel 4x4 logit head
     ('d_last_layers_k4_headkx', lambda: [nn.Conv2d(256, 512, 4, stride=1, padding=2), BN(512), nn.LeakyReLU(0.2, True)],
      lambda: [nn.Conv2d(512, 1, 4, stride=1, padding=2)], 1.0, (1, 256, 33, 129), ['precise']),
+    # the cfg4 generators' encoder / decoder paths at the benchmark's grids, where most layers run the async epilogue
+    ('g0_128_enc_dec_256x512', lambda: NW._down(128, 256, BN) + NW._down(256, 512, BN) + NW._up(512, 256, BN) + NW._up(256, 128, BN),
+     lambda: NW._head(128, 3, nn.Tanh()), 1.0, (1, 128, 256, 512), MODES),
+    ('g0_128_64_up_head_128x256', lambda: NW._up(128, 64, BN), lambda: NW._head(64, 3, nn.Tanh()), 1.0, (1, 128, 128, 256), ['precise']),
+    ('g2_6_32_res64_1024x2048', lambda: NW._stem(6, 32, BN) + NW._down(32, 64, BN) + [NW.ResnetBlock(64, 'reflect', BN)] + NW._up(64, 32, BN),
+     lambda: NW._head(32, 3, nn.Tanh()), 1.0, (1, 6, 1024, 2048), MODES),
 ]
 
 

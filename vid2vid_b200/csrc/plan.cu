@@ -58,11 +58,16 @@ struct DeviceGuard {
 static inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
 static inline size_t round_up_sz(size_t a, size_t b) { return (a + b - 1) / b * b; }
 // padded channel count of an activation buffer: one K block of min(C,64) channels per shared-memory row
-static thread_local int g_pad_min = 0;     // set while a backward sub-plan is being described (build_backward_units)
+static thread_local int g_pad_min = 0;     // a backward sub-plan's pad_min while it is built, lowered or described (PadScope)
 static inline int pad_channels(int c) {
   const int r = c <= 16 ? 16 : (c <= 32 ? 32 : round_up(c, 64));
   return std::max(r, g_pad_min);
 }
+struct PadScope {
+  int prev;
+  explicit PadScope(int m) : prev(g_pad_min) { g_pad_min = m; }
+  ~PadScope() { g_pad_min = prev; }
+};
 
 // ------------------------------------------------------------------------------ conv geometry
 struct ConvGeom {
@@ -312,20 +317,24 @@ using namespace v2v;
 //                       mode 2  transposed conv (s 2)  -> stride-2 conv of dY with the same weight tensor
 //                       mode 3  stride-2 conv          -> transposed conv of dY with the same weight tensor
 //   weight gradient = wgrad_umma_kernel over the two activation buffers the passes above left in place
+// Mode 0: the fp32 SIMT backward (backward.cu) does all of the conv, `simt` says why; wgrad false with mode > 0: it does the
+// weight gradient, `wg_simt` says why.
 struct BwdUnit {
   int gop = -1, mode = 0;
   v2v_plan* child = nullptr;
   int child_raw = -1;
   bool wgrad = false;
+  std::string simt, wg_simt;
   CUtensorMap tmOut{}, tmIn{};
   WgradParams wg{};
   int M = 0, M1 = 0, Nv = 0;
 };
 
 struct v2v_plan {
-  std::vector<BwdUnit> bwd;     // indexed through bwd_of[gop]
-  std::vector<int> bwd_of;
+  std::vector<BwdUnit> bwd;     // one per live conv op of a training plan, in graph order
+  std::vector<int> bwd_of;      // per graph op: its unit in bwd when that runs on the tensor cores (mode > 0), else -1
   float* wg_stage = nullptr;    // staging buffer of the weight-gradient kernel (largest unit)
+  int pad_min = 0;              // minimum padded channel count of every buffer (a backward sub-plan's dY: see choose_backward_unit)
 
   int device = 0;
   int impl = V2V_IMPL_UMMA;
@@ -364,7 +373,7 @@ struct v2v_plan {
 extern "C" int v2v_plan_create(int device, int conv_impl, v2v_plan** out);
 extern "C" int v2v_g_conv(v2v_plan* p, int value_in, const v2v_conv_desc* c, int* raw_out);
 extern "C" int v2v_plan_finalize(v2v_plan* P, v2v_stream_t stream_);
-extern "C" { static int new_value(v2v_plan* p, int N, int H, int W, int C); }
+extern "C" { static int new_value(v2v_plan* p, int N, int H, int W, int C); static int size_arena(v2v_plan* P); }
 
 namespace v2v {
 
@@ -803,105 +812,143 @@ static bool bwd_tensor_enabled() {      // read per plan, so that one process ca
   return !(e && !strcmp(e, "simt"));
 }
 
+// The weight gradient's operands: OUT is the gradient side, IN the activation side.  A transposed conv's data gradient is a
+// stride-2 conv of dY, so there the roles of the forward input x and of dY swap.
+static void wgrad_operands(const v2v_plan* P, const BwdUnit& u, const ActDesc** out, const ActDesc** in) {
+  const v2v_plan* C = u.child;
+  const GOp& op = P->gops[u.gop];
+  const ActDesc* a_dy = &C->acts[C->values[C->gops[0].value_out].bufs[0]];
+  const ActDesc* a_x = &P->acts[P->values[op.value_in].bufs[op.req_index]];
+  *out = u.mode == 2 ? a_x : a_dy;
+  *in = u.mode == 2 ? a_dy : a_x;
+}
+
+// Host-only half of the backward of live conv op i: the data-gradient mode and its sub-plan (built and lowered, no device
+// memory), and the weight-gradient launch or the reason it stays on the SIMT kernel.  u.child, when set, belongs to the
+// caller.  The device half is build_backward_units; v2v_plan_describe reports the same choice without a device.
+static int choose_backward_unit(v2v_plan* P, int i, BwdUnit& u) {
+  const GOp& op = P->gops[i];
+  const v2v_conv_desc& c = op.conv;
+  const Value& vin = P->values[op.value_in];
+  const int oh = op.geom.out_h, ow = op.geom.out_w;
+  char why[200];
+  u.gop = i;
+  if (!P->precise) { u.simt = "bf16 plan"; return 0; }
+  if (P->impl != V2V_IMPL_UMMA) { u.simt = "SIMT conv implementation"; return 0; }
+  if (!bwd_tensor_enabled()) { u.simt = "V2V_BWD=simt"; return 0; }
+  v2v_conv_desc cd{};
+  cd.Cin = c.Cout; cd.Cout = c.Cin; cd.kh = c.kh; cd.kw = c.kw; cd.pad_mode = V2V_PAD_ZERO; cd.weight = c.weight;
+  if (!c.transposed && c.stride == 1 && c.kh == c.kw && c.pad <= c.kh - 1 && (c.pad_mode != V2V_PAD_REFLECT || c.pad < std::min(vin.H, vin.W))) {
+    u.mode = 1; cd.stride = 1; cd.pad = c.kh - 1;
+  } else if (c.transposed && c.Cout2 == 0) {
+    u.mode = 2; cd.stride = 2; cd.pad = c.pad;
+  } else if (!c.transposed && c.stride == 2 && c.Cout2 == 0 && c.kh == c.kw && 2 + 2 * c.pad - c.kh >= 0 && 2 * oh >= vin.H && 2 * ow >= vin.W) {
+    // the transposed conv is asked for exactly 2 oh x 2 ow outputs (output_padding 2 + 2 pad - k; for 4x4 / pad 2 that is one
+    // row more than nn.ConvTranspose2d would accept, the extra rows are simply cropped by fold_add)
+    u.mode = 3; cd.stride = 2; cd.pad = c.pad; cd.transposed = 1; cd.output_padding = 2 + 2 * c.pad - c.kh;
+  } else {
+    snprintf(why, sizeof(why), "no data-gradient mode for k %dx%d stride %d pad %d (mode %d) transposed %d Cout2 %d on %dx%d -> %dx%d",
+             c.kh, c.kw, c.stride, c.pad, c.pad_mode, c.transposed, c.Cout2, vin.H, vin.W, oh, ow);
+    u.simt = why;
+    return 0;
+  }
+  // ---- sub-plan: dY (dense fp32 NHWC, channel stride round_up(Cout, 8)) -> halo-padded split activation -> conv
+  // the weight-gradient GEMM needs >= 64 channels on one side: when the forward input AND output are narrow (the 32 -> 3
+  // foreground head), the sub-plan carries dY padded to 64 channels
+  const int pad_min = (pad_channels(c.Cout) < 64 && pad_channels(c.Cin) < 64) ? 64 : 0;
+  v2v_plan* C = nullptr;
+  int rc = v2v_plan_create(P->device, P->impl, &C); if (rc) return rc;
+  C->precise = P->precise; C->pad_min = pad_min;
+  u.child = C;
+  PadScope scope(pad_min);
+  GOp gi; gi.kind = G_RAWIN; gi.ext_raw = op.kind == G_CONV ? P->raws[op.raw].graw : op.gdz; gi.ext_C = round_up(c.Cout, 8);
+  gi.value_out = new_value(C, vin.N, oh, ow, c.Cout);
+  C->gops.push_back(gi);
+  rc = v2v_g_conv(C, gi.value_out, &cd, &u.child_raw); if (rc) return rc;
+  C->raws[u.child_raw].no_stats = true;
+  if (u.mode == 1) { GOp& co = C->gops.back(); co.pack_dgrad = 1; co.dg_w2 = c.Cout2 > 0 ? c.weight2 : nullptr; co.dg_Cout1 = c.Cout - c.Cout2; }
+  rc = size_arena(C); if (rc) return rc;
+  {
+    const Raw& cr = C->raws[u.child_raw];
+    const int eh = u.mode == 1 ? vin.H + 2 * c.pad : vin.H, ew = u.mode == 1 ? vin.W + 2 * c.pad : vin.W;
+    V2V_REQUIRE(cr.H >= eh && cr.W >= ew && (u.mode == 3 || (cr.H == eh && cr.W == ew)) && cr.C == c.Cin, V2V_ERR_STATE,
+                "internal: data-gradient conv of op %d yields %dx%dx%d, expected %dx%dx%d", i, cr.H, cr.W, cr.C, eh, ew, c.Cin);
+  }
+  // ---- weight gradient on the tensor cores: OUT (gradient side) x IN (activation side) over the driving grid
+  const ActDesc *pa_out, *pa_in;
+  wgrad_operands(P, u, &pa_out, &pa_in);
+  const ActDesc& a_out = *pa_out, &a_in = *pa_in;
+  const int wmin = std::min(a_out.Wp, a_in.Wp);
+  const int kp = wmin >= 64 ? 64 : (wmin >= 32 ? 32 : (wmin >= 16 ? 16 : 0));
+  const bool wide_out = a_out.C % 64 == 0, wide_in = a_in.C % 64 == 0;
+  const bool narrow_ok_out = a_out.C == 16 || a_out.C == 32, narrow_ok_in = a_in.C == 16 || a_in.C == 32;
+  if (kp == 0) snprintf(why, sizeof(why), "operand rows of %d pixels (< 16)", wmin);
+  else if (!((wide_out && (wide_in || narrow_ok_in)) || (wide_in && narrow_ok_out)))
+    snprintf(why, sizeof(why), "padded channels %d (gradient) x %d (activation): neither 64-wide with the other 16 / 32 / 64-wide", a_out.C, a_in.C);
+  else if (a_out.parity) snprintf(why, sizeof(why), "gradient operand in parity planes");
+  else if (a_out.split != a_in.split) snprintf(why, sizeof(why), "operands differ in split");
+  else if (c.kh * c.kw > V2V_MAX_TAPS) snprintf(why, sizeof(why), "%d taps (> %d)", c.kh * c.kw, V2V_MAX_TAPS);
+  else why[0] = 0;
+  if (why[0]) { u.wg_simt = why; return 0; }
+  WgradParams& w = u.wg;
+  w.N = vin.N; w.gh = u.mode == 2 ? vin.H : oh; w.gw = u.mode == 2 ? vin.W : ow;
+  w.KP = kp; w.kmma = kp / 16; w.xsegs = (w.gw + kp - 1) / kp;
+  w.out_padt = a_out.pad_t; w.out_padl = a_out.pad_l;
+  w.swap = wide_out ? 0 : 1;                          // the narrow tensor (16 / 32 channels) always sits on the N side
+  const ActDesc& aA = w.swap ? a_in : a_out;
+  const ActDesc& aB = w.swap ? a_out : a_in;
+  w.a_C = aA.C; w.b_C = aB.C;
+  w.Mblocks = aA.C >= 128 ? 2 : 1;
+  w.b_row = aB.C >= 64 ? 128 : aB.C * 2;
+  w.Nblocks = aB.C >= 128 ? 2 : 1;
+  w.BN = aB.C >= 128 ? 128 : aB.C;
+  w.m_tiles = (aA.C + w.Mblocks * 64 - 1) / (w.Mblocks * 64); w.n_tiles = (aB.C + w.BN - 1) / w.BN;
+  w.ntaps = c.kh * c.kw; w.split = a_out.split; w.Mp = aA.C; w.Np = aB.C;
+  // taps: IN buffer coordinate of grid pixel (y, x).  Stride 1: (y + ky, x + kx); stride 2 (IN in parity planes):
+  // plane (ky & 1, kx & 1), (y + ky / 2, x + kx / 2) -- as conv_geometry lays the forward taps out
+  const bool s2 = (u.mode != 1);
+  for (int ky = 0; ky < c.kh; ++ky)
+    for (int kx = 0; kx < c.kw; ++kx)
+      w.taps[ky * c.kw + kx] = s2 ? WgradTap{(int8_t)(((ky & 1) << 1) | (kx & 1)), (int8_t)(ky >> 1), (int8_t)(kx >> 1), 0}
+                                  : WgradTap{0, (int8_t)ky, (int8_t)kx, 0};
+  V2V_REQUIRE(!s2 || a_in.parity, V2V_ERR_STATE, "internal: stride-2 weight gradient needs a parity-plane operand");
+  const int stage_bytes = (int)wgrad_stage_smem_bytes(w);
+  w.stages = std::max(2, std::min(6, kSmemBudget / stage_bytes));
+  w.chunks_total = w.N * w.gh * w.xsegs;
+  const int base_units = w.ntaps * w.m_tiles * w.n_tiles;
+  const int want = std::max(1, (2 * device_sm_count() + base_units - 1) / base_units);
+  w.chunks_per_unit = std::max(std::min(8, w.chunks_total), (w.chunks_total + want - 1) / want);
+  w.ksplit = (w.chunks_total + w.chunks_per_unit - 1) / w.chunks_per_unit;
+  // parameter gradient [R][Cc][taps]: rows = channels of OUT, columns = channels of IN
+  u.M = u.mode == 2 ? c.Cin : c.Cout; u.M1 = u.mode == 2 ? c.Cin : c.Cout - c.Cout2; u.Nv = u.mode == 2 ? c.Cout : c.Cin;
+  u.wgrad = true;
+  return 0;
+}
+
+// Device half: finalizes each unit's sub-plan, encodes the weight gradient's tensor maps and allocates its stage buffer.
 static int build_backward_units(v2v_plan* P, cudaStream_t stream) {
   P->bwd_of.assign(P->gops.size(), -1);
-  if (!P->precise || P->impl != V2V_IMPL_UMMA || !bwd_tensor_enabled()) return 0;
   size_t stage_max = 0;
   for (size_t i = 0; i < P->gops.size(); ++i) {
     const GOp& op = P->gops[i];
     if (op.kind != G_CONV && op.kind != G_CONV_ACT && op.kind != G_HEAD) continue;
-    if (!P->op_live[i]) continue;                 // forward-only branch: no data-gradient sub-plan
-    const v2v_conv_desc& c = op.conv;
-    const Value& vin = P->values[op.value_in];
-    const int oh = op.geom.out_h, ow = op.geom.out_w;
-    BwdUnit u; u.gop = (int)i;
-    v2v_conv_desc cd{};
-    cd.Cin = c.Cout; cd.Cout = c.Cin; cd.kh = c.kh; cd.kw = c.kw; cd.pad_mode = V2V_PAD_ZERO; cd.weight = c.weight;
-    if (!c.transposed && c.stride == 1 && c.kh == c.kw && c.pad <= c.kh - 1 && (c.pad_mode != V2V_PAD_REFLECT || c.pad < std::min(vin.H, vin.W))) {
-      u.mode = 1; cd.stride = 1; cd.pad = c.kh - 1;
-    } else if (c.transposed && c.Cout2 == 0) {
-      u.mode = 2; cd.stride = 2; cd.pad = c.pad;
-    } else if (!c.transposed && c.stride == 2 && c.Cout2 == 0 && c.kh == c.kw && 2 + 2 * c.pad - c.kh >= 0 && 2 * oh >= vin.H && 2 * ow >= vin.W) {
-      // the transposed conv is asked for exactly 2 oh x 2 ow outputs (output_padding 2 + 2 pad - k; for 4x4 / pad 2 that is one
-      // row more than nn.ConvTranspose2d would accept, the extra rows are simply cropped by fold_add)
-      u.mode = 3; cd.stride = 2; cd.pad = c.pad; cd.transposed = 1; cd.output_padding = 2 + 2 * c.pad - c.kh;
-    } else continue;
-    const float* dy = op.kind == G_CONV ? P->raws[op.raw].graw : op.gdz;
-    const int dy_C = op.kind == G_CONV ? P->raws[op.raw].desc.C : round_up(c.Cout, 8);
-    // ---- sub-plan: dY (dense fp32 NHWC) -> halo-padded split activation -> conv
-    // the weight-gradient GEMM needs >= 64 channels on one side: when the forward input AND output are narrow (the 32 -> 3
-    // foreground head), the sub-plan carries dY padded to 64 channels
-    g_pad_min = (pad_channels(c.Cout) < 64 && pad_channels(c.Cin) < 64) ? 64 : 0;
-    struct PadReset { ~PadReset() { g_pad_min = 0; } } pad_reset;
-    v2v_plan* C = nullptr;
-    int rc = v2v_plan_create(P->device, P->impl, &C); if (rc) return rc;
-    C->precise = P->precise;
-    u.child = C;
-    GOp gi; gi.kind = G_RAWIN; gi.ext_raw = dy; gi.ext_C = dy_C;
-    gi.value_out = new_value(C, vin.N, oh, ow, c.Cout);
-    C->gops.push_back(gi);
-    rc = v2v_g_conv(C, gi.value_out, &cd, &u.child_raw);
-    if (!rc) {
-      C->raws[u.child_raw].no_stats = true;
-      if (u.mode == 1) { GOp& co = C->gops.back(); co.pack_dgrad = 1; co.dg_w2 = c.Cout2 > 0 ? c.weight2 : nullptr; co.dg_Cout1 = c.Cout - c.Cout2; }
-      rc = v2v_plan_finalize(C, reinterpret_cast<v2v_stream_t>(stream));
-    }
-    if (rc) { P->bwd.push_back(u); return rc; }
+    if (!P->op_live[i]) continue;                 // forward-only branch: no backward
+    P->bwd.emplace_back();                        // owns the sub-plan from here on, also when a step below fails
+    BwdUnit& u = P->bwd.back();
+    int rc = choose_backward_unit(P, (int)i, u); if (rc) return rc;
+    if (!u.mode) continue;
     {
-      const Raw& cr = C->raws[u.child_raw];
-      const int eh = u.mode == 1 ? vin.H + 2 * c.pad : vin.H, ew = u.mode == 1 ? vin.W + 2 * c.pad : vin.W;
-      V2V_REQUIRE(cr.H >= eh && cr.W >= ew && (u.mode == 3 || (cr.H == eh && cr.W == ew)) && cr.C == c.Cin, V2V_ERR_STATE,
-                  "internal: data-gradient conv of op %d yields %dx%dx%d, expected %dx%dx%d", (int)i, cr.H, cr.W, cr.C, eh, ew, c.Cin);
+      PadScope scope(u.child->pad_min);
+      rc = v2v_plan_finalize(u.child, reinterpret_cast<v2v_stream_t>(stream)); if (rc) return rc;
     }
-    // ---- weight gradient on the tensor cores: OUT (gradient side) x IN (activation side) over the driving grid
-    g_pad_min = 0;
-    const ActDesc& a_dy = C->acts[C->values[gi.value_out].bufs[0]];
-    const ActDesc& a_x = P->acts[vin.bufs[op.req_index]];
-    const ActDesc& a_out = u.mode == 2 ? a_x : a_dy;
-    const ActDesc& a_in = u.mode == 2 ? a_dy : a_x;
-    const int kp = std::min(a_out.Wp, a_in.Wp) >= 64 ? 64 : (std::min(a_out.Wp, a_in.Wp) >= 32 ? 32 : (std::min(a_out.Wp, a_in.Wp) >= 16 ? 16 : 0));
-    const bool wide_out = a_out.C % 64 == 0, wide_in = a_in.C % 64 == 0;
-    const bool narrow_ok_out = a_out.C == 16 || a_out.C == 32, narrow_ok_in = a_in.C == 16 || a_in.C == 32;
-    if (kp > 0 && ((wide_out && (wide_in || narrow_ok_in)) || (wide_in && narrow_ok_out)) && !a_out.parity && a_out.split == a_in.split &&
-        c.kh * c.kw <= V2V_MAX_TAPS) {
-      WgradParams& w = u.wg;
-      w.N = vin.N; w.gh = u.mode == 2 ? vin.H : oh; w.gw = u.mode == 2 ? vin.W : ow;
-      w.KP = kp; w.kmma = kp / 16; w.xsegs = (w.gw + kp - 1) / kp;
-      w.out_padt = a_out.pad_t; w.out_padl = a_out.pad_l;
-      w.swap = wide_out ? 0 : 1;                          // the narrow tensor (16 / 32 channels) always sits on the N side
-      const ActDesc& aA = w.swap ? a_in : a_out;
-      const ActDesc& aB = w.swap ? a_out : a_in;
-      w.a_C = aA.C; w.b_C = aB.C;
-      w.Mblocks = aA.C >= 128 ? 2 : 1;
-      w.b_row = aB.C >= 64 ? 128 : aB.C * 2;
-      w.Nblocks = aB.C >= 128 ? 2 : 1;
-      w.BN = aB.C >= 128 ? 128 : aB.C;
-      w.m_tiles = (aA.C + w.Mblocks * 64 - 1) / (w.Mblocks * 64); w.n_tiles = (aB.C + w.BN - 1) / w.BN;
-      w.ntaps = c.kh * c.kw; w.split = a_out.split; w.Mp = aA.C; w.Np = aB.C;
-      // taps: IN buffer coordinate of grid pixel (y, x).  Stride 1: (y + ky, x + kx); stride 2 (IN in parity planes):
-      // plane (ky & 1, kx & 1), (y + ky / 2, x + kx / 2) -- as conv_geometry lays the forward taps out
-      const bool s2 = (u.mode != 1);
-      for (int ky = 0; ky < c.kh; ++ky)
-        for (int kx = 0; kx < c.kw; ++kx)
-          w.taps[ky * c.kw + kx] = s2 ? WgradTap{(int8_t)(((ky & 1) << 1) | (kx & 1)), (int8_t)(ky >> 1), (int8_t)(kx >> 1), 0}
-                                      : WgradTap{0, (int8_t)ky, (int8_t)kx, 0};
-      V2V_REQUIRE(!s2 || a_in.parity, V2V_ERR_STATE, "internal: stride-2 weight gradient needs a parity-plane operand");
-      const int stage_bytes = (int)wgrad_stage_smem_bytes(w);
-      w.stages = std::max(2, std::min(6, kSmemBudget / stage_bytes));
-      w.chunks_total = w.N * w.gh * w.xsegs;
-      const int base_units = w.ntaps * w.m_tiles * w.n_tiles;
-      const int want = std::max(1, (2 * device_sm_count() + base_units - 1) / base_units);
-      w.chunks_per_unit = std::max(std::min(8, w.chunks_total), (w.chunks_total + want - 1) / want);
-      w.ksplit = (w.chunks_total + w.chunks_per_unit - 1) / w.chunks_per_unit;
-      // parameter gradient [R][Cc][taps]: rows = channels of OUT, columns = channels of IN
-      u.M = u.mode == 2 ? c.Cin : c.Cout; u.M1 = u.mode == 2 ? c.Cin : c.Cout - c.Cout2; u.Nv = u.mode == 2 ? c.Cout : c.Cin;
-      rc = make_tmap_act(&u.tmOut, a_out, kp, 1, std::min(a_out.C, 64)); if (rc) { P->bwd.push_back(u); return rc; }
-      rc = make_tmap_act(&u.tmIn, a_in, kp, 1, std::min(a_in.C, 64)); if (rc) { P->bwd.push_back(u); return rc; }
-      u.wgrad = true;
-      stage_max = std::max(stage_max, wgrad_stage_bytes(w));
+    if (u.wgrad) {
+      const ActDesc *a_out, *a_in;
+      wgrad_operands(P, u, &a_out, &a_in);
+      rc = make_tmap_act(&u.tmOut, *a_out, u.wg.KP, 1, std::min(a_out->C, 64)); if (rc) return rc;
+      rc = make_tmap_act(&u.tmIn, *a_in, u.wg.KP, 1, std::min(a_in->C, 64)); if (rc) return rc;
+      stage_max = std::max(stage_max, wgrad_stage_bytes(u.wg));
     }
-    P->bwd_of[i] = (int)P->bwd.size();
-    P->bwd.push_back(u);
+    P->bwd_of[i] = (int)P->bwd.size() - 1;
   }
   if (stage_max) {
     V2V_CUDA(cudaMalloc(reinterpret_cast<void**>(&P->wg_stage), stage_max));
@@ -1719,6 +1766,68 @@ int64_t v2v_plan_workspace_bytes(const v2v_plan* P_) {
   return (int64_t)P->arena_bytes;
 }
 
+}  // extern "C"
+
+// One conv record of v2v_plan_describe: the conv, its geometry and the kernel configuration fill_conv_params chooses (host-only
+// logic; no device state needed).
+static void describe_conv(v2v_plan* P, const GOp& op, std::string& s) {
+  char t[512];
+  const ConvGeom& g = op.geom;
+  GOp tmp = op;                                  // kernel configuration (host-only logic; no device state needed)
+  fill_conv_params(const_cast<v2v_plan*>(P), tmp);
+  const ConvKernelParams& kp = tmp.kp;
+  // EG: epilogue groups per tile, always 1 (one 256-thread epilogue stores every tile; async_epi: which threads run it)
+  snprintf(t, sizeof(t),
+           "{\"kind\":%d,\"Cin\":%d,\"Cout\":%d,\"k\":[%d,%d],\"stride\":%d,\"transposed\":%d,\"in\":%d,\"TH\":%d,\"TW\":%d,"
+           "\"R\":%d,\"groups\":%d,\"phases\":%d,\"grid\":[%d,%d],\"out\":[%d,%d],"
+           "\"BN\":%d,\"kc\":%d,\"MG\":%d,\"CG\":%d,\"SG\":%d,\"resident\":%d,\"EG\":1,\"units\":%d,\"split\":%d,\"ring2\":%d,\"TB\":%d,\"SBr\":%d,"
+           "\"p2d\":%d,\"a_exact\":%d,\"headkx\":%d,\"grad\":%d,",
+           (int)op.kind, op.conv.Cin, op.conv.Cout, op.conv.kh, op.conv.kw, op.conv.stride, op.conv.transposed,
+           op.value_in, g.TH, g.TW, g.R, g.n_groups, g.n_phases, g.grid_h, g.grid_w, g.out_h, g.out_w,
+           kp.BN, kp.kc, kp.MG, kp.CG, kp.SG, kp.b_resident, kp.total_units, kp.split, kp.ring2, kp.TB, kp.SBr,
+           g.patch2d_kc > 0 ? 1 : 0, kp.a_exact, kp.headkx, (int)P->op_live[&op - P->gops.data()]);
+  s += t;
+  // the derived launch parameters the kernel reads (ctas: persistent CTAs launched; smem: dynamic shared memory)
+  snprintf(t, sizeof(t),
+           "\"tiles_x\":%d,\"tiles_y\":%d,\"tile_dx\":%d,\"Cp\":%d,\"cblocks\":%d,\"row_bytes\":%d,\"kmma\":%d,\"kmma_last\":%d,\"BNt\":%d,\"layout_type\":%d,"
+           "\"sbo_bytes\":%d,\"sbo_a_bytes\":%d,\"RW\":%d,\"PW\":%d,\"PH\":%d,\"a_half_bytes\":%d,\"a_slot_bytes\":%d,"
+           "\"b_half_bytes\":%d,\"b_slot_bytes\":%d,\"SB\":%d,\"n_tiles\":%d,\"m_total\":%d,\"ctas\":%d,\"Khalf\":%d,\"smem\":%zu,\"async_epi\":%d}",
+           kp.tiles_x, kp.tiles_y, kp.tile_dx, kp.Cp, kp.cblocks, kp.row_bytes, kp.kmma, kp.kmma_last, kp.BNt, kp.layout_type, kp.sbo_bytes,
+           kp.sbo_a_bytes, kp.RW, kp.PW, kp.PH, kp.a_half_bytes, kp.a_slot_bytes, kp.b_half_bytes, kp.b_slot_bytes, kp.SB,
+           kp.n_tiles, kp.m_total, kp.grid, kp.Khalf, conv_umma_smem_bytes(kp), conv_umma_async_epilogue(kp));
+  s += t;
+}
+
+// One backward record: the data-gradient mode (0: SIMT, "simt" says why), the sub-plan's conv as a conv record, and the
+// weight-gradient launch (null: SIMT, "wgrad_simt" says why).
+static void describe_backward_unit(const BwdUnit& u, std::string& s) {
+  char t[640];
+  snprintf(t, sizeof(t), "{\"gop\":%d,\"mode\":%d,\"simt\":\"%s\",\"wgrad_simt\":\"%s\",\"conv\":", u.gop, u.mode, u.simt.c_str(),
+           u.wg_simt.c_str());
+  s += t;
+  if (u.mode) {
+    PadScope scope(u.child->pad_min);
+    describe_conv(u.child, u.child->gops[1], s);
+  } else {
+    s += "null";
+  }
+  s += ",\"wgrad\":";
+  if (u.wgrad) {
+    const WgradParams& w = u.wg;
+    snprintf(t, sizeof(t),
+             "{\"swap\":%d,\"KP\":%d,\"BN\":%d,\"Mblocks\":%d,\"Nblocks\":%d,\"b_row\":%d,\"m_tiles\":%d,\"n_tiles\":%d,\"ntaps\":%d,"
+             "\"ksplit\":%d,\"chunks_per_unit\":%d,\"chunks_total\":%d,\"xsegs\":%d,\"gh\":%d,\"gw\":%d,\"stages\":%d,\"split\":%d,"
+             "\"Mp\":%d,\"Np\":%d}}",
+             w.swap, w.KP, w.BN, w.Mblocks, w.Nblocks, w.b_row, w.m_tiles, w.n_tiles, w.ntaps, w.ksplit, w.chunks_per_unit,
+             w.chunks_total, w.xsegs, w.gh, w.gw, w.stages, w.split, w.Mp, w.Np);
+    s += t;
+  } else {
+    s += "null}";
+  }
+}
+
+extern "C" {
+
 int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
   v2v_plan* P = const_cast<v2v_plan*>(P_);
   if (!P) return 0;
@@ -1741,31 +1850,27 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
   bool first = true;
   for (const GOp& op : P->gops) {
     if (!(op.kind == G_CONV || op.kind == G_CONV_ACT || op.kind == G_HEAD)) continue;
-    const ConvGeom& g = op.geom;
-    GOp tmp = op;                                  // kernel configuration (host-only logic; no device state needed)
-    fill_conv_params(const_cast<v2v_plan*>(P), tmp);
-    const ConvKernelParams& kp = tmp.kp;
-    // EG: epilogue groups per tile, always 1 (one 256-thread epilogue stores every tile; async_epi: which threads run it)
-    snprintf(t, sizeof(t),
-             "%s{\"kind\":%d,\"Cin\":%d,\"Cout\":%d,\"k\":[%d,%d],\"stride\":%d,\"transposed\":%d,\"in\":%d,\"TH\":%d,\"TW\":%d,"
-             "\"R\":%d,\"groups\":%d,\"phases\":%d,\"grid\":[%d,%d],\"out\":[%d,%d],"
-             "\"BN\":%d,\"kc\":%d,\"MG\":%d,\"CG\":%d,\"SG\":%d,\"resident\":%d,\"EG\":1,\"units\":%d,\"split\":%d,\"ring2\":%d,\"TB\":%d,\"SBr\":%d,"
-             "\"p2d\":%d,\"a_exact\":%d,\"headkx\":%d,\"grad\":%d,",
-             first ? "" : ",", (int)op.kind, op.conv.Cin, op.conv.Cout, op.conv.kh, op.conv.kw, op.conv.stride, op.conv.transposed,
-             op.value_in, g.TH, g.TW, g.R, g.n_groups, g.n_phases, g.grid_h, g.grid_w, g.out_h, g.out_w,
-             kp.BN, kp.kc, kp.MG, kp.CG, kp.SG, kp.b_resident, kp.total_units, kp.split, kp.ring2, kp.TB, kp.SBr,
-             g.patch2d_kc > 0 ? 1 : 0, kp.a_exact, kp.headkx, (int)P->op_live[&op - P->gops.data()]);
-    s += t;
-    // the derived launch parameters the kernel reads (ctas: persistent CTAs launched; smem: dynamic shared memory)
-    snprintf(t, sizeof(t),
-             "\"tiles_x\":%d,\"tiles_y\":%d,\"tile_dx\":%d,\"Cp\":%d,\"cblocks\":%d,\"row_bytes\":%d,\"kmma\":%d,\"kmma_last\":%d,\"BNt\":%d,\"layout_type\":%d,"
-             "\"sbo_bytes\":%d,\"sbo_a_bytes\":%d,\"RW\":%d,\"PW\":%d,\"PH\":%d,\"a_half_bytes\":%d,\"a_slot_bytes\":%d,"
-             "\"b_half_bytes\":%d,\"b_slot_bytes\":%d,\"SB\":%d,\"n_tiles\":%d,\"m_total\":%d,\"ctas\":%d,\"Khalf\":%d,\"smem\":%zu,\"async_epi\":%d}",
-             kp.tiles_x, kp.tiles_y, kp.tile_dx, kp.Cp, kp.cblocks, kp.row_bytes, kp.kmma, kp.kmma_last, kp.BNt, kp.layout_type, kp.sbo_bytes,
-             kp.sbo_a_bytes, kp.RW, kp.PW, kp.PH, kp.a_half_bytes, kp.a_slot_bytes, kp.b_half_bytes, kp.b_slot_bytes, kp.SB,
-             kp.n_tiles, kp.m_total, kp.grid, kp.Khalf, conv_umma_smem_bytes(kp), conv_umma_async_epilogue(kp));
-    s += t;
+    if (!first) s += ",";
+    describe_conv(P, op, s);
     first = false;
+  }
+  // training plans: the backward of every live conv, as finalize built it, or as it would build it (same host-only choice)
+  if (P->train) {
+    s += "],\"backward\":[";
+    first = true;
+    if (P->finalized) {
+      for (const BwdUnit& u : P->bwd) { if (!first) s += ","; describe_backward_unit(u, s); first = false; }
+    } else {
+      for (size_t i = 0; i < P->gops.size(); ++i) {
+        const GOp& op = P->gops[i];
+        if (!(op.kind == G_CONV || op.kind == G_CONV_ACT || op.kind == G_HEAD) || !P->op_live[i]) continue;
+        BwdUnit u;
+        const int rc = choose_backward_unit(P, (int)i, u);
+        if (!rc) { if (!first) s += ","; describe_backward_unit(u, s); first = false; }
+        if (u.child) v2v_plan_destroy(u.child);
+        if (rc) return -1;
+      }
+    }
   }
   // ops the backward visits (0 for the forward-only branch of a feature L1 target) and values without a gradient buffer
   int bwd_ops = 0, detached = 0;
