@@ -1,4 +1,4 @@
-"""CPU: the algebra the tensor-core backward rests on (csrc/plan.cu:build_backward_units), checked with PyTorch autograd in
+"""CPU: the algebra the tensor-core backward rests on (csrc/plan_backward.cu:build_backward_units), checked with PyTorch autograd in
 fp64.  The data gradient of every conv of a training plan is evaluated as a FORWARD conv of the output gradient:
 
   mode 1  stride-1 conv, pad p (reflect or zero)  -> stride-1 conv of dY with zero pad k - 1 and transposed + flipped weights; the

@@ -2,7 +2,7 @@
 step runs must also be run by a GPU parity case against fp64 (test_gpu_backward_variants / test_gpu_backward), and the convs
 whose backward stays on the fp32 SIMT kernels are pinned with the reason.
 
-choose_backward_unit (csrc/plan.cu) picks, for each live conv of a training plan, the data-gradient mode (1 stride-1 conv,
+choose_backward_unit (csrc/plan_backward.cu) picks, for each live conv of a training plan, the data-gradient mode (1 stride-1 conv,
 2 transposed conv, 3 stride-2 conv as a cropped transposed conv), the sub-plan's forward conv on conv_umma_kernel and the
 wgrad_umma_kernel launch; v2v_plan_describe reports that choice under "backward" without a GPU, assuming the H100 SXM's
 132 SMs as the forward lowering does."""

@@ -2,7 +2,7 @@
 lowered by a GPU parity case (test_gpu_conv / test_gpu_backward), where it is compared with an fp64 (or bf16-emulated)
 evaluation of the same layers at unit tolerance.
 
-The host picks one configuration per convolution (fill_conv_params in csrc/plan.cu): 2-D patch or row tiles and the taps per
+The host picks one configuration per convolution (fill_conv_params in csrc/conv_lower.cu): 2-D patch or row tiles and the taps per
 patch, single or multi-phase (transposed) tiling, N tile, K block, M blocking, resident or streamed weights, the coupled
 stages or the decoupled operand rings (with taps per weight chunk), precise or fast arithmetic, the exact-bf16 input
 shortcut and the kx-GEMM head.  v2v_plan_describe reports that choice without a GPU.  The choice depends on the SM count:

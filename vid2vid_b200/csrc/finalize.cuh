@@ -1,7 +1,7 @@
 // Batch / instance-norm affine of ONE channel from the fixed-point statistics rows (see FinalizeParams): the few
-// double-precision operations sit in the mean / variance subtraction only.  Shared by the normalise pass prologue
-// (csrc/norm.cu), the stand-alone stats_finalize_kernel and the tail of conv_umma_kernel, which must stay call-free: the
-// divisions are div_rn_normal (ptx.cuh), whose operands here are counts and fixed-point sums, never near underflow.
+// double-precision operations sit in the mean / variance subtraction only.  Shared by the stand-alone stats_finalize_kernel
+// (csrc/norm.cu) and the tail of conv_umma_kernel, which must stay call-free: the divisions are div_rn_normal (ptx.cuh),
+// whose operands here are counts and fixed-point sums, never near underflow.
 #pragma once
 #include "ptx.cuh"
 #include "v2v_internal.h"

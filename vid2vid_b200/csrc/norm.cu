@@ -14,8 +14,9 @@
 
 namespace v2v {
 
-// Stand-alone finalisation (one thread per channel): only the grid-stride fallback of the normalise pass needs the scale /
-// shift arrays ahead of time; the row-segment kernel computes them in its block prologue (see finalize.cuh).
+// Stand-alone finalisation (one thread per channel): writes scale / shift and the train-mode side effects of the norm slices
+// whose producing conv launch does not finalise them in its tail (the SIMT conv implementation, a third slice of one raw).
+// Both normalise kernels only read the scale / shift arrays.
 __global__ void __launch_bounds__(128) stats_finalize_kernel(FinalizeParams p) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= p.C) return;
@@ -268,7 +269,7 @@ cudaError_t launch_stats_finalize(const FinalizeParams& p, cudaStream_t stream) 
   return cudaGetLastError();
 }
 
-// true: the row-segment kernel (which derives scale / shift in its prologue) handles this launch; false: grid-stride fallback
+// true: the row-segment kernel handles this launch; false: grid-stride fallback
 bool norm_apply_uses_rows(const ApplyParams& p) {
   const int vecs = p.out.C / 8;
   const int Hpad = p.out.H + p.out.pad_t + p.out.pad_b;

@@ -1,0 +1,219 @@
+// Internal declarations of the plan runtime: the graph, its lowering and the plan object, shared by plan.cu (graph
+// builders, lowering, arena layout, finalize, run / profile / repack), conv_lower.cu (conv geometry, tiling, tensor maps
+// and weight packing) and plan_backward.cu (gradient buffers and the tensor-core backward).
+#pragma once
+#include <string>
+#include <unordered_map>
+#include <vector>
+
+#include "../../include/v2v_b200.h"
+#include "v2v_internal.h"
+#include "backward.h"
+
+namespace v2v {
+
+void set_error(const char* fmt, ...);
+
+#define V2V_CUDA(expr)                                                                          \
+  do {                                                                                          \
+    cudaError_t e__ = (expr);                                                                   \
+    if (e__ != cudaSuccess) {                                                                   \
+      set_error("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(e__), __FILE__, __LINE__);   \
+      return (int)e__;                                                                          \
+    }                                                                                           \
+  } while (0)
+#define V2V_REQUIRE(cond, code, ...) \
+  do {                               \
+    if (!(cond)) {                   \
+      set_error(__VA_ARGS__);        \
+      return code;                   \
+    }                                \
+  } while (0)
+
+static inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
+static inline size_t round_up_sz(size_t a, size_t b) { return (a + b - 1) / b * b; }
+// padded channel count of an activation buffer: one K block of min(C,64) channels per shared-memory row (a plan's buffers
+// may be padded further: Value::Cp)
+static inline int pad_channels(int c) { return c <= 16 ? 16 : (c <= 32 ? 32 : round_up(c, 64)); }
+
+// ------------------------------------------------------------------------------ conv geometry
+struct ConvGeom {
+  int pads[4];            // top, left, bottom, right of the input buffer
+  int parity;
+  int grid_h, grid_w;     // grid the kernel iterates over
+  int out_h, out_w;       // conv output extent
+  int mul;                // output coord = grid coord * mul + phase add
+  int TH, TW, R;
+  int RW;                 // taps per patch row: tap r of a group reads the patch shifted by (r / RW) rows, (r % RW) columns
+  int patch2d_kc;         // > 0: 16x8 pixel tiles, ONE activation patch of (16+kh-1) x (8+kw-1) pixels serves all kh*kw taps;
+  int patch2d_bn;         //      K block / N tile chosen together with the geometry (they decide the fit)
+  int headkx;             // > 0 (= kw): small-Cout head evaluated as a GEMM over (kx, channel) columns (taps over ky only)
+  int n_groups, n_phases;
+  ConvGroup groups[V2V_MAX_TAPS];
+  ConvPhase phases[V2V_MAX_PHASES];
+};
+
+// ------------------------------------------------------------------------------ graph description
+struct Req { int mode, pads[4], parity; };
+
+struct Value {
+  int N, H, W, C;
+  int Cp;                    // padded channels of every buffer of the value (ActDesc::C) and of a conv reading it (kp.Cp):
+                             // pad_channels(C), at least the plan's pad_min
+  std::vector<Req> reqs;
+  std::vector<int> bufs;     // index into Plan::acts, one per req
+  float* gval = nullptr;     // training plans: gradient of the value, dense NHWC fp32 [N][H][W][C]
+  int input_slot = -1;       // >= 0: the value is an import of that IO slot (data gradient only on request)
+  bool exact_bf16 = false;   // caller promise: every element is exactly representable in bf16 (one-hot labels, edge maps)
+  bool detached = false;     // every consumer is a detached operand (or skipped in the backward): no gradient buffer
+};
+struct Raw {
+  int N, H, W, C;
+  int conv_op = -1;          // index of producing graph op
+  RawDesc desc{};
+  stat_t* stats = nullptr;           // [N][2][C] fixed-point statistics rows (zeroed at the start of every run)
+  float* scale = nullptr; float* shift = nullptr;
+  std::vector<int> running_done;   // channel offsets whose running stats already have an updating launch
+  float* mean = nullptr; float* rstd = nullptr;   // training plans: saved statistics [N][C]
+  float* graw = nullptr;           // training plans: gradient of the raw tensor, dense NHWC fp32 (channel stride desc.C)
+  bool no_stats = false;           // backward sub-plans: the conv output feeds no norm layer
+};
+
+enum GKind { G_INPUT, G_CONV, G_NORM_ACT, G_CONV_ACT, G_HEAD, G_EXPORT, G_COMPOSITE, G_CONCAT, G_CORR, G_RAWIN, G_MAXPOOL, G_FEATL1 };
+struct GOp {
+  GKind kind;
+  // input
+  int slot = -1, C_src = 0, c_off = 0;
+  int value_in = -1, value_out = -1, raw = -1;
+  v2v_conv_desc conv{};
+  ConvGeom geom{};
+  int req_index = -1;        // which materialisation of value_in this conv reads
+  v2v_norm_desc norm{};
+  int act = 0; float slope = 0.f;
+  int add[2] = {-1, -1};
+  int n_off = 0, cC = 0;     // G_NORM_ACT: channel slice [n_off, n_off + cC) of the raw
+  v2v_head_channel head[V2V_MAX_HEAD];
+  CompositeParams comp{};
+  std::vector<int> cat_in;   // G_CONCAT: source values in channel order
+  int value_in2 = -1;        // G_CORR: second operand; G_FEATL1: the (detached) target operand
+  int l1_index = 0;          // G_FEATL1: element of the output slot
+  int corr[5] = {0, 0, 0, 0, 0};   // pad, kernel, max_disp, stride1, stride2
+  const float* ext_raw = nullptr; int ext_C = 0;   // G_RAWIN: dense NHWC fp32 tensor owned by the parent plan (a gradient buffer)
+  // backward sub-plans: pack the forward weights [Cout_f][Cin_f][kh][kw] (+ second set from output channel dg_Cout1 on) transposed
+  // and flipped, so that this forward conv computes the data gradient of that conv
+  int pack_dgrad = 0; const float* dg_w2 = nullptr; int dg_Cout1 = 0;
+  // lowered
+  bf16* wpacked = nullptr; int Ktotal = 0, Cp = 0;
+  float* gdz = nullptr;      // training plans: G_HEAD / G_CONV_ACT pre-activation gradient, dense NHWC fp32 [.][Cout]
+  double macs = 0.0;
+  CUtensorMap tmA{}, tmB{};
+  ConvKernelParams kp{};
+};
+
+enum XKind { X_IMPORT, X_CONV, X_RAWSTATS, X_FINALIZE, X_APPLY, X_EXPORT, X_COMPOSITE, X_MEMSET, X_COPY, X_CORR, X_MAXPOOL, X_FEATL1 };
+struct XOp {
+  XKind kind;
+  int gop = -1;
+  ImportParams imp{};
+  ExportParams exp{};
+  FinalizeParams fin{};
+  ApplyParams app{};
+  CompositeParams comp{};
+  CopyParams copy{};
+  CorrParams corr{};
+  PoolParams pool{};
+  FeatL1Params fl1{};
+  RawDesc rawd{}; stat_t* stats = nullptr; int stats_C = 0;
+  void* ms_ptr = nullptr; size_t ms_bytes = 0;
+};
+
+}  // namespace v2v
+
+using namespace v2v;     // the plan object is the C ABI's opaque v2v_plan, outside the namespace
+
+// Tensor-core backward of one conv op of a training plan (precise plans, tensor-core implementation):
+//   data gradient   = a FORWARD conv of the output gradient, run by a sub-plan on conv_umma_kernel:
+//                       mode 1  stride-1 conv          -> stride-1 conv, zero pad k-1, weights transposed + flipped; the result covers
+//                                                         the padded input extent and fold_add folds the (reflect) halo back
+//                       mode 2  transposed conv (s 2)  -> stride-2 conv of dY with the same weight tensor
+//                       mode 3  stride-2 conv          -> transposed conv of dY with the same weight tensor
+//   weight gradient = wgrad_umma_kernel over the two activation buffers the passes above left in place
+// Mode 0: the fp32 SIMT backward (backward.cu) does all of the conv, `simt` says why; wgrad false with mode > 0: it does the
+// weight gradient, `wg_simt` says why.
+struct BwdUnit {
+  int gop = -1, mode = 0;
+  v2v_plan* child = nullptr;
+  int child_raw = -1;
+  bool wgrad = false;
+  std::string simt, wg_simt;
+  CUtensorMap tmOut{}, tmIn{};
+  WgradParams wg{};
+  int M = 0, M1 = 0, Nv = 0;
+};
+
+struct v2v_plan {
+  std::vector<BwdUnit> bwd;     // one per live conv op of a training plan, in graph order
+  std::vector<int> bwd_of;      // per graph op: its unit in bwd when that runs on the tensor cores (mode > 0), else -1
+  float* wg_stage = nullptr;    // staging buffer of the weight-gradient kernel (largest unit)
+  int pad_min = 0;              // minimum padded channel count of every buffer (a backward sub-plan's dY: see choose_backward_unit);
+                                // set before the first value (new_value reads it into Value::Cp)
+
+  int device = 0;
+  int impl = V2V_IMPL_UMMA;
+  int precise = 0;            // V2V_PREC_BF16X3: split activations / weights, fp32 raw tensors, 3 MMAs per K block
+  int sp() const { return precise ? 2 : 1; }
+  bool lowered = false, finalized = false;
+  bool train = false;          // keep what the backward needs (batch statistics) and allocate gradient buffers
+  void* garena = nullptr; size_t garena_bytes = 0;
+  std::vector<float*> gslot;   // per IO slot: plan-internal gradient of a head output produced by the composite backward
+  float* gsums = nullptr;      // scratch of the norm backward [2][N][Cmax]
+  float* train_stats = nullptr;
+  std::vector<Value> values;
+  std::vector<Raw> raws;
+  std::vector<GOp> gops;
+  std::vector<ActDesc> acts;
+  std::vector<int> act_pad_mode;
+  std::vector<char> op_live;    // per graph op: visited by the backward (0: all its outputs only feed detached operands)
+  std::vector<XOp> xops;
+  int n_slots = 0;
+  double conv_macs = 0.0;
+  struct BiasAffine { float* scale; float* shift; const float* bias; int N, C, stride; };
+  std::vector<BiasAffine> bias_affines;   // norm-less biased convs routed through the normalise pass (scale 1, shift bias)
+  // arena layout (size_arena) and device memory
+  struct RawOff { size_t raw = 0, stats = 0, scale = 0, shift = 0; };
+  bool sized = false, arena_owned = true;
+  std::vector<size_t> act_off, w_off, corr_off, l1_off;
+  std::vector<RawOff> raw_off;
+  size_t stats_begin = 0, stats_end = 0;
+  void* arena = nullptr; size_t arena_bytes = 0;
+  void** io_dev = nullptr;
+  cudaGraphExec_t graph_exec = nullptr;
+  cudaStream_t graph_stream = nullptr;
+};
+
+namespace v2v {
+
+// conv_lower.cu
+extern const int kSmemBudget;      // dynamic shared memory of a kernel's operand slots + resident weights
+int conv_geometry(const v2v_conv_desc& c, int Cp, int head, int N, int H, int W, bool allow_reuse, int sp, ConvGeom* g);
+void fill_conv_params(v2v_plan* P, GOp& op);
+int make_tmap_act(CUtensorMap* tm, const ActDesc& a, int box_w, int box_h, int kc);
+int make_tmap_w(CUtensorMap* tm, bf16* w, int Ktotal, int Cout, int BN, int kc);
+int pack_one(const GOp& op, cudaStream_t stream);
+void describe_conv(v2v_plan* P, const GOp& op, std::string& s);
+
+// plan.cu
+int new_value(v2v_plan* p, int N, int H, int W, int C);
+int size_arena(v2v_plan* P);
+int run_xop(v2v_plan* P, const XOp& x, cudaStream_t s);
+FeatL1Params featl1_params(const v2v_plan* P, const GOp& op);
+
+// plan_backward.cu
+int alloc_training(v2v_plan* P, cudaStream_t stream);
+int choose_backward_unit(v2v_plan* P, int i, BwdUnit& u);
+int build_backward_units(v2v_plan* P, cudaStream_t stream);
+int run_backward(v2v_plan* P, void* const* io, void* const* gio, const std::unordered_map<const void*, void*>& pg,
+                 cudaStream_t s);
+void describe_backward_unit(const BwdUnit& u, std::string& s);
+
+}  // namespace v2v

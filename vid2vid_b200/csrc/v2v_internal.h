@@ -85,7 +85,7 @@ typedef unsigned long long stat_t;
 struct FinalizeParams {
   const stat_t* stats;     // [N][2][Cs]
   int Cs, C;               // stats channel stride, channels
-  int N, tiles_per_img, num_phases;
+  int N;
   double count;            // elements per channel per image
   int instance;            // 0 = batch statistics over N, 1 = per-image statistics
   const float* gamma;      // may be null (-> 1)
@@ -190,7 +190,6 @@ struct ApplyParams {
   ActDesc add[2];          // interior is read (any padding / parity)
   ActDesc out;
   int pad_mode;            // PadMode of out's halo
-  FinalizeParams fin;
 };
 
 // fp32 NCHW (caller tensor, read through the IO table) -> halo-padded NHWC bf16

@@ -4,7 +4,7 @@
 //
 // where OUT is the gradient of the conv output and IN the conv input (train.py:83-90 back-propagates through every
 // nn.Conv2d / nn.ConvTranspose2d of models/networks.py; for a transposed conv the roles of "input" and "output gradient"
-// swap, see plan.cu).  Both operands are read where the forward pass left them: halo-padded NHWC activation buffers, a
+// swap, see plan_backward.cu).  Both operands are read where the forward pass left them: halo-padded NHWC activation buffers, a
 // pixel being [hi C | lo C] bf16.  A TMA box of KP pixels x 64 channels lands in shared memory as KP rows of 128 bytes with
 // the 128-byte swizzle -- the canonical *MN-major* SWIZZLE_128B operand layout (64 contiguous M / N elements per K index,
 // 8-K groups 1024 bytes apart, 64-element blocks one box apart), so no transposed copy of any tensor is made: the same
