@@ -92,12 +92,13 @@ int v2v_fg_mask(const float* real_A, float* mask, int B, int T, int C, int H, in
                 int n_labels, v2v_stream_t stream);
 
 /* Streaming clip input (test.py:31-41 feeds a tG-frame window of label ids per generated frame, of which only the newest
- * frame is new): window (T,H,W) float ids, oldest first, is shifted by one frame in place and `frame` (H,W; dtype 0 uint8,
- * 1 int32, 2 float) appended.  Keeps the window resident so a step uploads one uint8 frame instead of T float ones. */
-int v2v_ids_window_push(float* window, const void* frame, int dtype, int T, int H, int W, v2v_stream_t stream);
-/* util.tensor2im (util/util.py:48-71) on the device: image (C,H,W) float in [-1,1] -> out (H,W,C) uint8
+ * frame is new): each of the B windows (B,T,H,W) float ids, oldest first, is shifted by one frame in place and its clip's
+ * `frame` (B,H,W; dtype 0 uint8, 1 int32, 2 float) appended.  Keeps the windows resident so a step uploads one uint8 frame
+ * per clip instead of T float ones. */
+int v2v_ids_window_push(float* window, const void* frame, int dtype, int B, int T, int H, int W, v2v_stream_t stream);
+/* util.tensor2im (util/util.py:48-71) on the device: image (B,C,H,W) float in [-1,1] -> out (B,H,W,C) uint8
  * = uint8(clip((image + 1) / 2 * 255, 0, 255)). */
-int v2v_tensor2im_u8(const float* image, uint8_t* out, int C, int H, int W, v2v_stream_t stream);
+int v2v_tensor2im_u8(const float* image, uint8_t* out, int B, int C, int H, int W, v2v_stream_t stream);
 
 /* Losses of the training step (models/vid2vid_model_D.py:117-140,199-213; criteria models/networks.py:731-812) and the
  * backward of the helpers they differentiate through.  `out` / `grad_out` are 1-element device tensors (no host sync);
@@ -271,6 +272,12 @@ int v2v_g_composite_ex(v2v_plan* plan, int s_raw, int s_flow, int s_weight, int 
 
 /* Training plans (before finalize): keep the batch statistics and allocate dense fp32 gradient buffers. */
 int v2v_plan_set_training(v2v_plan* plan, int on);
+/* Per-sample statistics (before the plan is lowered; inference plans only, V2V_ERR_STATE together with training): every
+ * norm layer normalises image n of the batch with the statistics of image n alone (gamma / beta unchanged), and the running
+ * statistics take one momentum update per image, in image order.  Each conv keeps the kernel configuration of the
+ * one-image plan, so a batch of N independent clips gives each clip's outputs and leaves the running statistics bit for
+ * bit as N one-image runs in image order would. */
+int v2v_plan_set_sample_stats(v2v_plan* plan, int on);
 /* Backward of the LAST v2v_plan_run of this plan (whose intermediate buffers the plan still holds): autograd of
  * netG.forward / netD.forward as train.py:50-93 drives it.  io_ptrs: the forward tensors, as passed to v2v_plan_run.
  * grad_io_ptrs[slot]: for output slots the incoming gradient (fp32 NCHW, NULL = none); for input slots the destination of

@@ -18,8 +18,8 @@ cudaError_t launch_flownet_prep(const float*, const float*, long long, long long
 cudaError_t launch_resize(const float*, float*, float*, int, int, int, int, int, float, float, float, float, float, int, cudaStream_t);
 cudaError_t launch_sub_channels(const float*, const float*, float*, int, int, int, int, int, int, cudaStream_t);
 cudaError_t launch_flow_conf(const float*, const float*, float*, int, int, int, int, float, cudaStream_t);
-cudaError_t launch_ids_window_push(float*, const void*, int, int, int, int, cudaStream_t);
-cudaError_t launch_tensor2im_u8(const float*, uint8_t*, int, int, int, cudaStream_t);
+cudaError_t launch_ids_window_push(float*, const void*, int, int, int, int, int, cudaStream_t);
+cudaError_t launch_tensor2im_u8(const float*, uint8_t*, int, int, int, int, cudaStream_t);
 cudaError_t launch_l1_fwd(const float*, const float*, const float*, int, int, int, int, double*, float*, cudaStream_t);
 cudaError_t launch_l1_bwd(const float*, const float*, const float*, int, int, int, int, const float*, float*, float*, cudaStream_t);
 cudaError_t launch_mse_const_fwd(const float*, long long, float, double*, float*, cudaStream_t);
@@ -126,15 +126,15 @@ int v2v_fg_mask(const float* real_A, float* mask, int B, int T, int C, int H, in
   return 0;
 }
 
-int v2v_ids_window_push(float* window, const void* frame, int dtype, int T, int H, int W, v2v_stream_t stream) {
-  API_REQUIRE(window && frame && dtype >= 0 && dtype <= 2 && T >= 1 && H > 0 && W > 0, "ids_window_push: bad arguments");
-  API_CUDA(launch_ids_window_push(window, frame, dtype, T, H, W, reinterpret_cast<cudaStream_t>(stream)));
+int v2v_ids_window_push(float* window, const void* frame, int dtype, int B, int T, int H, int W, v2v_stream_t stream) {
+  API_REQUIRE(window && frame && dtype >= 0 && dtype <= 2 && B >= 1 && T >= 1 && H > 0 && W > 0, "ids_window_push: bad arguments");
+  API_CUDA(launch_ids_window_push(window, frame, dtype, B, T, H, W, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
 
-int v2v_tensor2im_u8(const float* image, uint8_t* out, int C, int H, int W, v2v_stream_t stream) {
-  API_REQUIRE(image && out && C > 0 && H > 0 && W > 0, "tensor2im_u8: bad arguments");
-  API_CUDA(launch_tensor2im_u8(image, out, C, H, W, reinterpret_cast<cudaStream_t>(stream)));
+int v2v_tensor2im_u8(const float* image, uint8_t* out, int B, int C, int H, int W, v2v_stream_t stream) {
+  API_REQUIRE(image && out && B >= 1 && C > 0 && H > 0 && W > 0, "tensor2im_u8: bad arguments");
+  API_CUDA(launch_tensor2im_u8(image, out, B, C, H, W, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
 

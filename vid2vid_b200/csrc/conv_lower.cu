@@ -224,7 +224,7 @@ static ConvTiling choose_tiling(const v2v_plan* P, const GOp& op, const ConvKern
   const bool head = op.kind == G_HEAD, p2d = g.patch2d_kc > 0;
   const int sp = P->sp(), sms = device_sm_count(), budget = kSmemBudget;
   const int Cp = kp.Cp, kc_nat = std::min(Cp, 64), bn_nat = std::min(128, round_up(c.Cout, 32));
-  const int m_tiles = kp.N * kp.tiles_x * kp.tiles_y;
+  const int m_tiles = P->tiling_n(kp.N) * kp.tiles_x * kp.tiles_y;
   auto a_slot = [&](int kc) { return a_slot_bytes(sp, kp.PW * kp.PH, kc); };
   ConvTiling t{};
   t.kc = kc_nat; t.BN = head ? (g.headkx ? 32 : 16) : bn_nat; t.MG = 1;

@@ -33,7 +33,16 @@ __device__ __forceinline__ ChannelAffine channel_affine(const FinalizeParams& p,
   return a;
 }
 
-// side effects of a train-mode norm layer for channel c: running statistics, and the per-image arrays the backward reads
+// nn.BatchNorm2d's train-mode running-statistics update from the statistics of n images (mean sum rm, unbiased variance sum rv)
+__device__ __forceinline__ void running_update(const FinalizeParams& p, int c, double rm, double rv, int n) {
+  const float bias = p.conv_bias ? p.conv_bias[c] : 0.f;
+  p.running_mean[c] = (1.f - p.momentum) * p.running_mean[c] + p.momentum * ((float)div_rn_normal(rm, n) + bias);
+  p.running_var[c] = (1.f - p.momentum) * p.running_var[c] + p.momentum * (float)div_rn_normal(rv, n);
+}
+
+// side effects of a train-mode norm layer for channel c: running statistics, and the per-image arrays the backward reads.
+// Per-sample plans (p.sample_running) update the running statistics once per image, in image order, with the expression a
+// one-image plan evaluates: N images leave them exactly as N one-image forwards in that order would.
 __device__ __forceinline__ void channel_side_effects(const FinalizeParams& p, int c) {
   double rm = 0.0, rv = 0.0;
   for (int n = 0; n < p.N; ++n) {
@@ -46,14 +55,16 @@ __device__ __forceinline__ void channel_side_effects(const FinalizeParams& p, in
       p.mean_out[(size_t)n * p.scale_stride + p.c_off + c] = a.mean;
       p.rstd_out[(size_t)n * p.scale_stride + p.c_off + c] = a.rstd;
     }
+    if (p.sample_running) {
+      if (p.running_mean) running_update(p, c, 0.0 + (double)a.mean, 0.0 + a.var_unbiased, 1);
+      continue;
+    }
     rm += a.mean; rv += a.var_unbiased;
     if (!p.instance && !p.scale && !p.mean_out) { rm *= p.N; rv *= p.N; break; }       // batch statistics: identical for all n
   }
   if (p.running_mean) {
-    const float bias = p.conv_bias ? p.conv_bias[c] : 0.f;
-    p.running_mean[c] = (1.f - p.momentum) * p.running_mean[c] + p.momentum * ((float)div_rn_normal(rm, p.N) + bias);
-    p.running_var[c] = (1.f - p.momentum) * p.running_var[c] + p.momentum * (float)div_rn_normal(rv, p.N);
-    if (c == 0 && p.num_batches_tracked) *p.num_batches_tracked += 1;
+    if (!p.sample_running) running_update(p, c, rm, rv, p.N);
+    if (c == 0 && p.num_batches_tracked) *p.num_batches_tracked += p.sample_running ? p.N : 1;
   }
 }
 

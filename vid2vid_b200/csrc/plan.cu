@@ -110,8 +110,8 @@ static int lower(v2v_plan* P) {
   for (auto& op : P->gops) {
     if (op.kind == G_CONV || op.kind == G_CONV_ACT || op.kind == G_HEAD) {
       Value& vin = P->values[op.value_in];
-      int rc = conv_geometry(op.conv, vin.Cp, op.kind == G_HEAD ? (P->impl == V2V_IMPL_UMMA ? 2 : 1) : 0, vin.N, vin.H, vin.W,
-                             true, P->sp(), &op.geom);
+      int rc = conv_geometry(op.conv, vin.Cp, op.kind == G_HEAD ? (P->impl == V2V_IMPL_UMMA ? 2 : 1) : 0, P->tiling_n(vin.N), vin.H,
+                             vin.W, true, P->sp(), &op.geom);
       if (rc) return rc;
       op.req_index = add_req(vin, conv_req(op.conv, op.geom));
       const v2v_conv_desc& c = op.conv;
@@ -248,7 +248,17 @@ int v2v_plan_set_precision(v2v_plan* p, int precision) {
 
 int v2v_plan_set_training(v2v_plan* p, int on) {
   V2V_REQUIRE(p && !p->finalized, V2V_ERR_STATE, "set the training flag before finalize");
+  V2V_REQUIRE(!(on && p->sample_stats), V2V_ERR_STATE,
+              "a per-sample-statistics plan cannot train: training normalises with the statistics of the whole batch");
   p->train = on != 0;
+  return 0;
+}
+
+int v2v_plan_set_sample_stats(v2v_plan* p, int on) {
+  V2V_REQUIRE(p && !p->lowered, V2V_ERR_STATE, "set per-sample statistics before the plan is lowered");
+  V2V_REQUIRE(!(on && p->train), V2V_ERR_STATE,
+              "per-sample statistics are for inference plans: a training plan normalises with the statistics of the whole batch");
+  p->sample_stats = on != 0;
   return 0;
 }
 
@@ -572,7 +582,8 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
         if (has_norm) {
           fp.stats = r.stats; fp.Cs = r.C; fp.C = op.cC; fp.c_off = op.n_off; fp.scale_stride = r.C;
           fp.N = r.N;
-          fp.count = (double)r.H * r.W; fp.instance = (op.norm.kind == V2V_NORM_INSTANCE);
+          fp.count = (double)r.H * r.W; fp.instance = (op.norm.kind == V2V_NORM_INSTANCE) || P->sample_stats;
+          fp.sample_running = P->sample_stats;
           const int cout1 = cop.conv.Cout - cop.conv.Cout2;
           V2V_REQUIRE(op.n_off == 0 || (cop.conv.Cout2 > 0 && op.n_off == cout1), V2V_ERR_UNSUPPORTED,
                       "a raw slice must start at channel 0 or at the second weight set");
@@ -867,8 +878,8 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
   int bwd_ops = 0, detached = 0;
   for (char l : P->op_live) bwd_ops += l;
   for (const Value& v : P->values) detached += v.detached;
-  snprintf(t, sizeof(t), "],\"conv_macs\":%.0f,\"n_slots\":%d,\"ops\":%zu,\"backward_ops\":%d,\"detached_values\":%d}", P->conv_macs,
-           P->n_slots, P->gops.size(), bwd_ops, detached);
+  snprintf(t, sizeof(t), "],\"conv_macs\":%.0f,\"n_slots\":%d,\"ops\":%zu,\"backward_ops\":%d,\"detached_values\":%d,\"sample_stats\":%d}",
+           P->conv_macs, P->n_slots, P->gops.size(), bwd_ops, detached, P->sample_stats ? 1 : 0);
   s += t;
   if (buf && cap > 0) {
     size_t n = std::min((size_t)cap - 1, s.size());

@@ -164,6 +164,12 @@ struct v2v_plan {
   int sp() const { return precise ? 2 : 1; }
   bool lowered = false, finalized = false;
   bool train = false;          // keep what the backward needs (batch statistics) and allocate gradient buffers
+  // Per-sample statistics (v2v_plan_set_sample_stats): every norm layer normalises image n with the statistics of image n.
+  // Such a plan also configures each conv as the plan of ONE image would (tiling_n): the configuration fixes the order in
+  // which a pixel's products are accumulated, so each image's outputs equal its one-image plan's bit for bit, and the N
+  // images only add work units.
+  bool sample_stats = false;
+  int tiling_n(int N) const { return sample_stats ? 1 : N; }
   void* garena = nullptr; size_t garena_bytes = 0;
   std::vector<float*> gslot;   // per IO slot: plan-internal gradient of a head output produced by the composite backward
   float* gsums = nullptr;      // scratch of the norm backward [2][N][Cmax]

@@ -104,24 +104,30 @@ __global__ void fg_mask_kernel(const float* __restrict__ real_A, float* __restri
   }
 }
 
-// Streaming input: window (T, HW) float ids, oldest frame first; drop the oldest, append the new frame converted from
-// uint8 / int32 / float (dtype 0 / 1 / 2).  One thread per pixel walks the frames, so the in-place shift has no hazard.
-__global__ void ids_window_push_kernel(float* __restrict__ window, const void* __restrict__ frame, int dtype, int T, size_t HW) {
-  for (size_t pix = blockIdx.x * (size_t)blockDim.x + threadIdx.x; pix < HW; pix += (size_t)gridDim.x * blockDim.x) {
-    for (int t = 0; t + 1 < T; ++t) window[(size_t)t * HW + pix] = window[(size_t)(t + 1) * HW + pix];
+// Streaming input: B windows (B, T, HW) float ids, oldest frame first; drop each window's oldest frame, append its clip's
+// new frame (B, HW) converted from uint8 / int32 / float (dtype 0 / 1 / 2).  One thread per (clip, pixel) walks the frames,
+// so the in-place shift has no hazard.
+__global__ void ids_window_push_kernel(float* __restrict__ window, const void* __restrict__ frame, int dtype, int T, size_t HW,
+                                       size_t total) {
+  for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
+    const size_t b = idx / HW, pix = idx - b * HW;
+    float* win = window + b * T * HW;
+    for (int t = 0; t + 1 < T; ++t) win[(size_t)t * HW + pix] = win[(size_t)(t + 1) * HW + pix];
     float v;
-    if (dtype == 0) v = (float)reinterpret_cast<const uint8_t*>(frame)[pix];
-    else if (dtype == 1) v = (float)reinterpret_cast<const int*>(frame)[pix];
-    else v = reinterpret_cast<const float*>(frame)[pix];
-    window[(size_t)(T - 1) * HW + pix] = v;
+    if (dtype == 0) v = (float)reinterpret_cast<const uint8_t*>(frame)[idx];
+    else if (dtype == 1) v = (float)reinterpret_cast<const int*>(frame)[idx];
+    else v = reinterpret_cast<const float*>(frame)[idx];
+    win[(size_t)(T - 1) * HW + pix] = v;
   }
 }
 
-// util.tensor2im (util/util.py:48-71): (C,H,W) float in [-1,1] -> (H,W,C) uint8 = clip((x + 1) / 2 * 255, 0, 255) truncated
-__global__ void tensor2im_u8_kernel(const float* __restrict__ img, uint8_t* __restrict__ out, int C, size_t HW) {
-  for (size_t pix = blockIdx.x * (size_t)blockDim.x + threadIdx.x; pix < HW; pix += (size_t)gridDim.x * blockDim.x) {
+// util.tensor2im (util/util.py:48-71) per image: (B,C,H,W) float in [-1,1] -> (B,H,W,C) uint8 = clip((x + 1) / 2 * 255, 0, 255)
+// truncated
+__global__ void tensor2im_u8_kernel(const float* __restrict__ img, uint8_t* __restrict__ out, int C, size_t HW, size_t total) {
+  for (size_t pix = blockIdx.x * (size_t)blockDim.x + threadIdx.x; pix < total; pix += (size_t)gridDim.x * blockDim.x) {
+    const size_t b = pix / HW, p = pix - b * HW;
     for (int c = 0; c < C; ++c) {
-      float v = __fmul_rn(__fdiv_rn(__fadd_rn(img[(size_t)c * HW + pix], 1.f), 2.0f), 255.0f);
+      float v = __fmul_rn(__fdiv_rn(__fadd_rn(img[(b * C + c) * HW + p], 1.f), 2.0f), 255.0f);
       v = fminf(fmaxf(v, 0.f), 255.f);
       out[pix * C + c] = (uint8_t)v;
     }
@@ -151,12 +157,12 @@ cudaError_t launch_avgpool3s2(const float* in, float* out, int P, int H, int W, 
   avgpool3s2_kernel<<<grid, 256, 0, s>>>(in, out, P, H, W, Ho, Wo);
   return cudaGetLastError();
 }
-cudaError_t launch_ids_window_push(float* window, const void* frame, int dtype, int T, int H, int W, cudaStream_t s) {
-  ids_window_push_kernel<<<grid1d((size_t)H * W), 256, 0, s>>>(window, frame, dtype, T, (size_t)H * W);
+cudaError_t launch_ids_window_push(float* window, const void* frame, int dtype, int B, int T, int H, int W, cudaStream_t s) {
+  ids_window_push_kernel<<<grid1d((size_t)B * H * W), 256, 0, s>>>(window, frame, dtype, T, (size_t)H * W, (size_t)B * H * W);
   return cudaGetLastError();
 }
-cudaError_t launch_tensor2im_u8(const float* img, uint8_t* out, int C, int H, int W, cudaStream_t s) {
-  tensor2im_u8_kernel<<<grid1d((size_t)H * W), 256, 0, s>>>(img, out, C, (size_t)H * W);
+cudaError_t launch_tensor2im_u8(const float* img, uint8_t* out, int B, int C, int H, int W, cudaStream_t s) {
+  tensor2im_u8_kernel<<<grid1d((size_t)B * H * W), 256, 0, s>>>(img, out, C, (size_t)H * W, (size_t)B * H * W);
   return cudaGetLastError();
 }
 cudaError_t launch_fg_mask(const float* real_A, float* mask, int B, int T, int C, int H, int W, int t,

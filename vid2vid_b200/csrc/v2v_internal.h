@@ -88,6 +88,7 @@ struct FinalizeParams {
   int N;
   double count;            // elements per channel per image
   int instance;            // 0 = batch statistics over N, 1 = per-image statistics
+  int sample_running;      // 1: running statistics take one update per image, in image order (per-sample plans)
   const float* gamma;      // may be null (-> 1)
   const float* beta;       // may be null (-> 0)
   const float* conv_bias;  // folded into running_mean only (cancels in the normalised output)

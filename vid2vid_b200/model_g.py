@@ -170,17 +170,56 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
 
     # ------------------------------------------------------------------ inference
     def inference(self, input_A, input_B, inst_A):
-        """vid2vid_model_G.py:198-209."""
+        """vid2vid_model_G.py:198-209.  input_A (b, T, C, H, W) holds b independent clips (the reference runs b = 1): the
+        generators then run per-sample-statistics plans (_Planned.sample_stats), so every clip's frames equal its own b = 1
+        run bit for bit.  The clips of one sequence start and advance together; b == 1 keeps the reference's batch-less
+        fake_B_prev."""
         with torch.no_grad():
             real_A, real_B, pool_map = self.encode_input(input_A, input_B, inst_A)
-            self.is_first_frame = self.fake_B_prev is None
-            if self.is_first_frame:
-                self.fake_B_prev = self.generate_first_frame(real_A, real_B, pool_map)
-            real_A = self.build_pyr(real_A)
-            self.fake_B_feat = self.flow_feat = self.fake_B_fg_feat = None
-            for s in range(self.n_scales):
-                fake_B = self.generate_frame_infer(real_A[self.n_scales - 1 - s], s)
-        return fake_B, real_A[0][0, -1]
+            with self._per_clip_statistics(self.bs > 1):
+                return self._inference(real_A, real_B, pool_map)
+
+    @contextlib.contextmanager
+    def _per_clip_statistics(self, on):
+        """The generators' per-sample-statistics plans (b independent clips, each normalised with its own statistics) for the
+        duration of one inference call: afterwards the modules build batch-statistics (and training) plans as before."""
+        nets = [getattr(self, 'netG' + str(s)) for s in range(self.n_scales)] + ([self.netG_i] if self.netG_i is not None else [])
+        prev = [getattr(net, 'sample_stats', False) for net in nets]
+        for net in nets:
+            net.sample_stats = on
+        try:
+            yield
+        finally:
+            for net, p in zip(nets, prev):
+                net.sample_stats = p
+
+    def _inference(self, real_A, real_B, pool_map):
+        self.is_first_frame = self.fake_B_prev is None
+        if self.is_first_frame:
+            self.fake_B_prev = self.generate_first_frame(real_A, real_B, pool_map)
+        elif self.bs != self._clips():
+            raise ValueError('this sequence was started with %d clip(s) and is fed %d: clips of one sequence start and advance '
+                             'together (reset_stream() starts a new one)' % (self._clips(), self.bs))
+        real_A = self.build_pyr(real_A)
+        self.fake_B_feat = self.flow_feat = self.fake_B_fg_feat = None
+        for s in range(self.n_scales):
+            fake_B = self.generate_frame_infer(real_A[self.n_scales - 1 - s], s)
+        return fake_B, (real_A[0][0, -1] if self.bs == 1 else real_A[0][:, -1])
+
+    def _clips(self):
+        """Clips of the running sequence: fake_B_prev keeps a batch axis only for b > 1 (the reference's b = 1 state has none)."""
+        return self.fake_B_prev[0].shape[0] if self.fake_B_prev[0].dim() == 5 else 1
+
+    def reset_stream(self, clips=None):
+        """Start a new sequence: the next inference() / inference_stream() call generates first frames again.  `clips` (a
+        list of clip indices) asks to restart only some clips of a running batch, which is not supported: the clips of a
+        batch start and advance together."""
+        n = self._clips() if self.fake_B_prev is not None else 0
+        if clips is not None and n > 1 and sorted(set(clips)) != list(range(n)):
+            raise NotImplementedError('restarting clip(s) %s of a running batch of %d clips is not supported: the clips of a batch '
+                                      'start and advance together; call reset_stream() to restart the whole batch' % (list(clips), n))
+        self.fake_B_prev = None
+        self._win_A = self._win_I = None
 
     # ------------------------------------------------------------------ streaming inference (one new frame per call)
     _DT = {torch.uint8: 0, torch.int32: 1, torch.float32: 2}
@@ -191,7 +230,9 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         test.py:31-41 re-sends every step stays resident on the device, so a step uploads one frame.  The first tG - 1
         calls only fill the window and return None.  Returns the generated frame (1, 3, H, W) float, or, when `out_u8`
         (a (H, W, 3) uint8 tensor, host or device) is given, util.tensor2im's uint8 image written into it
-        (computed on the device; util/util.py:48-71 does it on the CPU after copying the float frame back)."""
+        (computed on the device; util/util.py:48-71 does it on the CPU after copying the float frame back).
+        B clips at once: (B, H, W) id maps, frames (B, 3, H, W), out_u8 (B, H, W, 3); every step is one launch per helper
+        for all clips, and every call of one stream must feed the same B."""
         import ctypes as C
         from . import _lib as L
         if self.opt.dataset_mode == 'face' and self.use_single_G:
@@ -199,10 +240,16 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
                              '(use_single_G with dataset_mode face): use inference()')
         tG = self.opt.n_frames_G
         H, W = label_frame.shape[-2:]
+        B = label_frame.shape[0] if label_frame.dim() == 3 else 1
+        if inst_frame is not None and tuple(inst_frame.shape) != tuple(label_frame.shape):
+            raise ValueError('inst_frame %s does not match label_frame %s' % (tuple(inst_frame.shape), tuple(label_frame.shape)))
         dev = self.device_
+        if getattr(self, '_win_A', None) is not None and self._win_A.shape[0] != B:
+            raise ValueError('this stream was started with %d clip(s) and is fed %d: clips of one stream start and advance '
+                             'together (reset_stream() starts a new one)' % (self._win_A.shape[0], B))
         if getattr(self, '_win_A', None) is None or self._win_A.shape[-2:] != (H, W):
-            self._win_A = torch.zeros(1, tG, 1, H, W, device=dev)
-            self._win_I = torch.zeros(1, tG, 1, H, W, device=dev) if self.opt.use_instance else None
+            self._win_A = torch.zeros(B, tG, 1, H, W, device=dev)
+            self._win_I = torch.zeros(B, tG, 1, H, W, device=dev) if self.opt.use_instance else None
             self._win_n = 0
         for win, fr in ((self._win_A, label_frame), (self._win_I, inst_frame if inst_frame is not None else label_frame)):
             if win is None:
@@ -210,8 +257,8 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
             fr = fr.to(dev, non_blocking=True).contiguous()
             if fr.dtype not in self._DT:
                 raise TypeError('id maps must be uint8, int32 or float32')
-            L.check(L.lib().v2v_ids_window_push(C.c_void_p(win.data_ptr()), C.c_void_p(fr.data_ptr()), self._DT[fr.dtype], tG, H, W,
-                                                L.current_stream_ptr()))
+            L.check(L.lib().v2v_ids_window_push(C.c_void_p(win.data_ptr()), C.c_void_p(fr.data_ptr()), self._DT[fr.dtype], B, tG, H,
+                                                W, L.current_stream_ptr()))
             L.LAUNCHES[0] += 1
         self._win_n += 1
         if self._win_n < tG:
@@ -219,10 +266,11 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         fake_B, _ = self.inference(self._win_A, None, self._win_I)
         if out_u8 is None:
             return fake_B
-        if getattr(self, '_u8_dev', None) is None or self._u8_dev.shape[:2] != (H, W):
-            self._u8_dev = torch.empty(H, W, fake_B.shape[1], dtype=torch.uint8, device=dev)
-        L.check(L.lib().v2v_tensor2im_u8(C.c_void_p(fake_B.data_ptr()), C.c_void_p(self._u8_dev.data_ptr()), fake_B.shape[1], H, W,
-                                         L.current_stream_ptr()))
+        shape = (H, W, fake_B.shape[1]) if label_frame.dim() == 2 else (B, H, W, fake_B.shape[1])
+        if getattr(self, '_u8_dev', None) is None or tuple(self._u8_dev.shape) != shape:
+            self._u8_dev = torch.empty(shape, dtype=torch.uint8, device=dev)
+        L.check(L.lib().v2v_tensor2im_u8(C.c_void_p(fake_B.data_ptr()), C.c_void_p(self._u8_dev.data_ptr()), B, fake_B.shape[1], H,
+                                         W, L.current_stream_ptr()))
         L.LAUNCHES[0] += 1
         if out_u8.is_cuda:
             out_u8.copy_(self._u8_dev)
@@ -233,17 +281,23 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
     def generate_frame_infer(self, real_A, s):
         """vid2vid_model_G.py:211-229."""
         tG = self.opt.n_frames_G
-        _, _, _, h, w = real_A.size()
+        b, _, _, h, w = real_A.size()
         si = self.n_scales - 1 - s
         netG_s = getattr(self, 'netG' + str(s))
-        real_As_reshaped = real_A[0, :tG].reshape(1, -1, h, w)
-        fake_B_prevs_reshaped = self.fake_B_prev[si].reshape(1, -1, h, w)
-        mask_F = self.compute_mask(real_A, tG - 1)[0] if self.opt.fg else None
+        real_As_reshaped = real_A[:, :tG].reshape(b, -1, h, w)
+        fake_B_prevs_reshaped = self.fake_B_prev[si].reshape(b, -1, h, w)
+        mask_F = None
+        if self.opt.fg:
+            mask_F = self.compute_mask(real_A, tG - 1)
+            mask_F = mask_F[0] if b == 1 else mask_F
         use_raw_only = self.opt.no_first_img and self.is_first_frame
         fake_B, flow, weight, fake_B_raw, self.fake_B_feat, self.flow_feat, self.fake_B_fg_feat = netG_s.forward(
             real_As_reshaped, fake_B_prevs_reshaped, mask_F, self.fake_B_feat, self.flow_feat, self.fake_B_fg_feat,
             use_raw_only)
-        self.fake_B_prev[si] = torch.cat([self.fake_B_prev[si][1:, ...], fake_B])
+        if b == 1:
+            self.fake_B_prev[si] = torch.cat([self.fake_B_prev[si][1:, ...], fake_B])
+        else:
+            self.fake_B_prev[si] = torch.cat([self.fake_B_prev[si][:, 1:], fake_B.unsqueeze(1)], dim=1)
         return fake_B
 
     def generate_first_frame(self, real_A, real_B, pool_map=None):
@@ -257,14 +311,20 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
             if self.opt.use_instance:
                 real_A = real_A[:, :, :self.opt.label_nc, :, :]
             frames = []
-            for i in range(tG - 1):
-                feat_map = self.get_face_features(real_B[:, i], pool_map[:, i]) if self.opt.dataset_mode == 'face' else None
-                frames.append(self.netG_i.forward(real_A[:, i].contiguous(), feat_map).unsqueeze(1))
+            if self.opt.dataset_mode == 'face':
+                # get_face_features picks ONE table row over its whole batch (as the reference does): clip by clip
+                self.netG_i.sample_stats = False
+                for i in range(tG - 1):
+                    frames.append(torch.cat([self.netG_i.forward(real_A[c:c + 1, i].contiguous(), self.get_face_features(
+                        real_B[c:c + 1, i], pool_map[c:c + 1, i])) for c in range(self.bs)]).unsqueeze(1))
+            else:
+                for i in range(tG - 1):
+                    frames.append(self.netG_i.forward(real_A[:, i].contiguous(), None).unsqueeze(1))
             fake_B_prev = torch.cat(frames, dim=1)
         else:
             raise ValueError('Please specify the method for generating the first frame')
         fake_B_prev = self.build_pyr(fake_B_prev)
-        if not self.opt.isTrain:
+        if not self.opt.isTrain and self.bs == 1:
             fake_B_prev = [B[0] for B in fake_B_prev]
         return fake_B_prev
 

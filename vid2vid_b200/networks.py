@@ -329,6 +329,10 @@ class _Planned(nn.Module):
     align_corners = False   # installed-PyTorch grid_sample default; True = PyTorch-0.4 semantics (App. B #2)
     use_cuda_graph = True
     precision = None        # None: DEFAULT_PRECISION at plan-build time; or 'fast' / 'precise' per module
+    # True: inference plans normalise each image of the batch with its own statistics and update the running statistics
+    # once per image, in batch order (v2v_plan_set_sample_stats), so a batch of independent clips gives each clip exactly its
+    # batch-1 result.  Training plans keep the batch statistics: asking for a gradient of such a module is an error.
+    sample_stats = False
 
     def _precision(self):
         return self.precision or DEFAULT_PRECISION
@@ -359,7 +363,7 @@ class _Planned(nn.Module):
 
     def _get_plan(self, key, device, build, train=False):
         ptrs, ver = self._signature()
-        key = key + (('train',) if train else ()) + (self._precision(),)
+        key = key + (('train',) if train else ()) + (('sample_stats',) if self.sample_stats else ()) + (self._precision(),)
         ent = self._plans().get(key)
         if ent is not None and ent['ptrs'] != ptrs:
             ent = None
@@ -367,7 +371,7 @@ class _Planned(nn.Module):
             if os.environ.get('V2V_LOG_PLANS'):
                 print('v2v: building plan %s for %s (cached: %d)' % (key, type(self).__name__, len(self._plans())), file=sys.stderr, flush=True)
             plan = Plan(device.index if device.index is not None else torch.cuda.current_device(),
-                        precision=self._precision(), train=train)
+                        precision=self._precision(), train=train, sample_stats=self.sample_stats)
             build(plan)
             plan.finalize()
             ent = {'plan': plan, 'ptrs': ptrs, 'ver': ver}

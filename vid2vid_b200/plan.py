@@ -57,7 +57,7 @@ def norm_desc(m):
 
 
 class Plan:
-    def __init__(self, device=0, impl=None, precision='fast', train=False):
+    def __init__(self, device=0, impl=None, precision='fast', train=False, sample_stats=False):
         if impl is None:
             impl = L.IMPL_SIMT if os.environ.get('V2V_CONV_IMPL') == 'simt' else L.IMPL_UMMA
         self._h = C.c_void_p()
@@ -68,6 +68,10 @@ class Plan:
         self.train = bool(train)
         if train:
             L.check(L.lib().v2v_plan_set_training(self._h, 1))
+        # per-sample statistics: image n of the batch is normalised with its own statistics (independent clips)
+        self.sample_stats = bool(sample_stats)
+        if sample_stats:
+            L.check(L.lib().v2v_plan_set_sample_stats(self._h, 1))
         self.run_id = 0
         self._keep = []
         self.finalized = False
