@@ -96,6 +96,15 @@ int v2v_fg_mask(const float* real_A, float* mask, int B, int T, int C, int H, in
  * `frame` (B,H,W; dtype 0 uint8, 1 int32, 2 float) appended.  Keeps the windows resident so a step uploads one uint8 frame
  * per clip instead of T float ones. */
 int v2v_ids_window_push(float* window, const void* frame, int dtype, int B, int T, int H, int W, v2v_stream_t stream);
+/* Slot streams (B fixed slots whose clips start and stop independently): window (B,T,C,H,W) float, oldest frame first,
+ * frames (B,C,H,W; dtype 0 uint8, 1 int32, 2 float).  ops[b] (host array of B entries, passed to the kernel by value) is
+ * what slot b's window does this step: V2V_SLOT_KEEP leaves it, V2V_SLOT_PUSH drops the oldest frame and appends frame b,
+ * V2V_SLOT_RESTART zeroes it and appends frame b (a new clip), V2V_SLOT_CLEAR zeroes it.  B <= V2V_MAX_SLOTS.  C = 1 holds
+ * id maps, C = input_nc dense frames. */
+#define V2V_MAX_SLOTS 64
+enum { V2V_SLOT_KEEP = 0, V2V_SLOT_PUSH = 1, V2V_SLOT_RESTART = 2, V2V_SLOT_CLEAR = 3 };
+int v2v_slots_window_push(float* window, const void* frames, int dtype, int B, int T, int C, int H, int W, const int* ops,
+                          v2v_stream_t stream);
 /* util.tensor2im (util/util.py:48-71) on the device: image (B,C,H,W) float in [-1,1] -> out (B,H,W,C) uint8
  * = uint8(clip((image + 1) / 2 * 255, 0, 255)). */
 int v2v_tensor2im_u8(const float* image, uint8_t* out, int B, int C, int H, int W, v2v_stream_t stream);
@@ -278,6 +287,14 @@ int v2v_plan_set_training(v2v_plan* plan, int on);
  * one-image plan, so a batch of N independent clips gives each clip's outputs and leaves the running statistics bit for
  * bit as N one-image runs in image order would. */
 int v2v_plan_set_sample_stats(v2v_plan* plan, int on);
+/* Per-image flags (before finalize; per-sample-statistics inference plans only, V2V_ERR_STATE otherwise): IO slot `slot`
+ * holds a caller-owned int32 (N,) device tensor read at run time, so a captured graph stays valid while the flags change
+ * between runs.  V2V_IMAGE_ACTIVE: image n updates the running statistics (inactive images are computed but leave the
+ * running statistics and num_batches_tracked alone; num_batches_tracked advances by the number of active images).
+ * V2V_IMAGE_RAW_ONLY: the composite of image n takes the raw image (no warp), exactly as a plan built with use_warp 0. */
+#define V2V_IMAGE_ACTIVE 1
+#define V2V_IMAGE_RAW_ONLY 2
+int v2v_plan_set_image_flags(v2v_plan* plan, int slot);
 /* Backward of the LAST v2v_plan_run of this plan (whose intermediate buffers the plan still holds): autograd of
  * netG.forward / netD.forward as train.py:50-93 drives it.  io_ptrs: the forward tensors, as passed to v2v_plan_run.
  * grad_io_ptrs[slot]: for output slots the incoming gradient (fp32 NCHW, NULL = none); for input slots the destination of
@@ -309,7 +326,8 @@ int v2v_plan_profile(v2v_plan* plan, void* const* io_ptrs, int n_io, v2v_stream_
 int v2v_plan_num_kernels(const v2v_plan* plan);             /* kernels launched per run */
 double v2v_plan_conv_macs(const v2v_plan* plan);            /* algorithmic conv MACs per run (dense, unpadded) */
 int64_t v2v_plan_workspace_bytes(const v2v_plan* plan);       /* arena bytes; may be called before finalize (host only) */
-/* Writes a JSON description of the lowered plan (buffers, tiles, tap groups) into buf; returns needed size. */
+/* Writes a JSON description of the lowered plan (buffers, tiles, tap groups; "sample_stats" and "image_flags" say whether
+ * the plan keeps per-sample statistics and reads per-image flags) into buf; returns needed size. */
 int64_t v2v_plan_describe(const v2v_plan* plan, char* buf, int64_t cap);
 
 /* Host-only: the tap-group table the kernel would use for a convolution (pure function; no GPU).

@@ -19,6 +19,7 @@ cudaError_t launch_resize(const float*, float*, float*, int, int, int, int, int,
 cudaError_t launch_sub_channels(const float*, const float*, float*, int, int, int, int, int, int, cudaStream_t);
 cudaError_t launch_flow_conf(const float*, const float*, float*, int, int, int, int, float, cudaStream_t);
 cudaError_t launch_ids_window_push(float*, const void*, int, int, int, int, int, cudaStream_t);
+cudaError_t launch_slots_window_push(float*, const void*, int, int, int, int, int, int, const int*, cudaStream_t);
 cudaError_t launch_tensor2im_u8(const float*, uint8_t*, int, int, int, int, cudaStream_t);
 cudaError_t launch_l1_fwd(const float*, const float*, const float*, int, int, int, int, double*, float*, cudaStream_t);
 cudaError_t launch_l1_bwd(const float*, const float*, const float*, int, int, int, int, const float*, float*, float*, cudaStream_t);
@@ -129,6 +130,17 @@ int v2v_fg_mask(const float* real_A, float* mask, int B, int T, int C, int H, in
 int v2v_ids_window_push(float* window, const void* frame, int dtype, int B, int T, int H, int W, v2v_stream_t stream) {
   API_REQUIRE(window && frame && dtype >= 0 && dtype <= 2 && B >= 1 && T >= 1 && H > 0 && W > 0, "ids_window_push: bad arguments");
   API_CUDA(launch_ids_window_push(window, frame, dtype, B, T, H, W, reinterpret_cast<cudaStream_t>(stream)));
+  return 0;
+}
+
+int v2v_slots_window_push(float* window, const void* frames, int dtype, int B, int T, int C, int H, int W, const int* ops,
+                          v2v_stream_t stream) {
+  API_REQUIRE(window && frames && ops && dtype >= 0 && dtype <= 2 && B >= 1 && T >= 1 && C > 0 && H > 0 && W > 0,
+              "slots_window_push: bad arguments");
+  API_REQUIRE(B <= V2V_MAX_SLOTS, "slots_window_push: %d slots, at most %d", B, V2V_MAX_SLOTS);
+  for (int b = 0; b < B; ++b)
+    API_REQUIRE(ops[b] >= V2V_SLOT_KEEP && ops[b] <= V2V_SLOT_CLEAR, "slots_window_push: slot %d has unknown op %d", b, ops[b]);
+  API_CUDA(launch_slots_window_push(window, frames, dtype, B, T, C, H, W, ops, reinterpret_cast<cudaStream_t>(stream)));
   return 0;
 }
 

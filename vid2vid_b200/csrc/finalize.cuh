@@ -3,6 +3,7 @@
 // (csrc/norm.cu) and the tail of conv_umma_kernel, which must stay call-free: the divisions are div_rn_normal (ptx.cuh),
 // whose operands here are counts and fixed-point sums, never near underflow.
 #pragma once
+#include "../../include/v2v_b200.h"
 #include "ptx.cuh"
 #include "v2v_internal.h"
 
@@ -42,9 +43,13 @@ __device__ __forceinline__ void running_update(const FinalizeParams& p, int c, d
 
 // side effects of a train-mode norm layer for channel c: running statistics, and the per-image arrays the backward reads.
 // Per-sample plans (p.sample_running) update the running statistics once per image, in image order, with the expression a
-// one-image plan evaluates: N images leave them exactly as N one-image forwards in that order would.
+// one-image plan evaluates: N images leave them exactly as N one-image forwards in that order would.  With per-image flags
+// (p.flags_slot >= 0, per-sample plans only) an image without V2V_IMAGE_ACTIVE is skipped, so the running statistics end as
+// the one-image forwards of the active images in image order would leave them.
 __device__ __forceinline__ void channel_side_effects(const FinalizeParams& p, int c) {
+  const int* flags = p.flags_slot >= 0 ? reinterpret_cast<const int*>(p.io[p.flags_slot]) : nullptr;
   double rm = 0.0, rv = 0.0;
+  int active = 0;
   for (int n = 0; n < p.N; ++n) {
     const ChannelAffine a = channel_affine(p, n, c);
     if (p.scale) {
@@ -56,6 +61,8 @@ __device__ __forceinline__ void channel_side_effects(const FinalizeParams& p, in
       p.rstd_out[(size_t)n * p.scale_stride + p.c_off + c] = a.rstd;
     }
     if (p.sample_running) {
+      if (flags && !(__ldcg(flags + n) & V2V_IMAGE_ACTIVE)) continue;
+      ++active;
       if (p.running_mean) running_update(p, c, 0.0 + (double)a.mean, 0.0 + a.var_unbiased, 1);
       continue;
     }
@@ -64,7 +71,7 @@ __device__ __forceinline__ void channel_side_effects(const FinalizeParams& p, in
   }
   if (p.running_mean) {
     if (!p.sample_running) running_update(p, c, rm, rv, p.N);
-    if (c == 0 && p.num_batches_tracked) *p.num_batches_tracked += p.sample_running ? p.N : 1;
+    if (c == 0 && p.num_batches_tracked) *p.num_batches_tracked += p.sample_running ? active : 1;
   }
 }
 

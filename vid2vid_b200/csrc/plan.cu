@@ -256,9 +256,21 @@ int v2v_plan_set_training(v2v_plan* p, int on) {
 
 int v2v_plan_set_sample_stats(v2v_plan* p, int on) {
   V2V_REQUIRE(p && !p->lowered, V2V_ERR_STATE, "set per-sample statistics before the plan is lowered");
+  V2V_REQUIRE(on || p->flags_slot < 0, V2V_ERR_STATE, "a plan with per-image flags keeps per-sample statistics");
   V2V_REQUIRE(!(on && p->train), V2V_ERR_STATE,
               "per-sample statistics are for inference plans: a training plan normalises with the statistics of the whole batch");
   p->sample_stats = on != 0;
+  return 0;
+}
+
+int v2v_plan_set_image_flags(v2v_plan* p, int slot) {
+  V2V_REQUIRE(p && !p->finalized, V2V_ERR_STATE, "set the image flags before finalize");
+  V2V_REQUIRE(!p->train, V2V_ERR_STATE, "per-image flags are for inference plans: a training plan cannot skip images");
+  V2V_REQUIRE(p->sample_stats, V2V_ERR_STATE,
+              "per-image flags need a per-sample-statistics plan: batch statistics mix the images, so none can be skipped");
+  V2V_REQUIRE(slot >= 0, V2V_ERR_INVALID, "bad flags slot %d", slot);
+  p->flags_slot = slot;
+  p->n_slots = std::max(p->n_slots, slot + 1);
   return 0;
 }
 
@@ -584,6 +596,7 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
           fp.N = r.N;
           fp.count = (double)r.H * r.W; fp.instance = (op.norm.kind == V2V_NORM_INSTANCE) || P->sample_stats;
           fp.sample_running = P->sample_stats;
+          fp.io = P->io_dev; fp.flags_slot = P->flags_slot;
           const int cout1 = cop.conv.Cout - cop.conv.Cout2;
           V2V_REQUIRE(op.n_off == 0 || (cop.conv.Cout2 > 0 && op.n_off == cout1), V2V_ERR_UNSUPPORTED,
                       "a raw slice must start at channel 0 or at the second weight set");
@@ -656,7 +669,7 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
         break;
       }
       case G_COMPOSITE: {
-        XOp x; x.kind = X_COMPOSITE; x.comp = op.comp; x.comp.io = P->io_dev;
+        XOp x; x.kind = X_COMPOSITE; x.comp = op.comp; x.comp.io = P->io_dev; x.comp.s_flags = P->flags_slot;
         P->xops.push_back(x);
         break;
       }
@@ -878,8 +891,9 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
   int bwd_ops = 0, detached = 0;
   for (char l : P->op_live) bwd_ops += l;
   for (const Value& v : P->values) detached += v.detached;
-  snprintf(t, sizeof(t), "],\"conv_macs\":%.0f,\"n_slots\":%d,\"ops\":%zu,\"backward_ops\":%d,\"detached_values\":%d,\"sample_stats\":%d}",
-           P->conv_macs, P->n_slots, P->gops.size(), bwd_ops, detached, P->sample_stats ? 1 : 0);
+  snprintf(t, sizeof(t), "],\"conv_macs\":%.0f,\"n_slots\":%d,\"ops\":%zu,\"backward_ops\":%d,\"detached_values\":%d,\"sample_stats\":%d,"
+           "\"image_flags\":%d}", P->conv_macs, P->n_slots, P->gops.size(), bwd_ops, detached, P->sample_stats ? 1 : 0,
+           P->flags_slot >= 0 ? 1 : 0);
   s += t;
   if (buf && cap > 0) {
     size_t n = std::min((size_t)cap - 1, s.size());

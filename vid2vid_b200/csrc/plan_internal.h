@@ -170,6 +170,7 @@ struct v2v_plan {
   // images only add work units.
   bool sample_stats = false;
   int tiling_n(int N) const { return sample_stats ? 1 : N; }
+  int flags_slot = -1;         // v2v_plan_set_image_flags: IO slot of the per-image flags read by the finalisations and composites
   void* garena = nullptr; size_t garena_bytes = 0;
   std::vector<float*> gslot;   // per IO slot: plan-internal gradient of a head output produced by the composite backward
   float* gsums = nullptr;      // scratch of the norm backward [2][N][Cmax]

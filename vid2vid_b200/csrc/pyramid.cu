@@ -5,6 +5,7 @@
 //   avgpool3s2   : AvgPool2d(3, stride 2, pad 1, count_include_pad=False) pyramid level
 //                  (BaseModel.build_pyr, models/base_model.py:122-134; networks.py:400,652)
 //   fg_mask      : clamp(sum of fg label channels, 0, 1)  (compute_mask, vid2vid_model_G.py:322-330)
+#include "../../include/v2v_b200.h"
 #include "ptx.cuh"
 #include "v2v_internal.h"
 
@@ -121,6 +122,30 @@ __global__ void ids_window_push_kernel(float* __restrict__ window, const void* _
   }
 }
 
+// Slot streams: window (B, T, C*HW) float, frames (B, C*HW) uint8 / int32 / float (dtype 0 / 1 / 2).  Each slot's op
+// (V2V_SLOT_*) travels by value; one thread per (slot, element) walks the frames, so the in-place shift has no hazard.
+struct SlotOps { int v[V2V_MAX_SLOTS]; };
+__global__ void slots_window_push_kernel(float* __restrict__ window, const void* __restrict__ frames, int dtype, int T, size_t E,
+                                         size_t total, SlotOps ops) {
+  for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
+    const size_t b = idx / E, e = idx - b * E;
+    const int op = ops.v[b];
+    if (op == V2V_SLOT_KEEP) continue;
+    float* win = window + b * T * E;
+    if (op == V2V_SLOT_PUSH)
+      for (int t = 0; t + 1 < T; ++t) win[(size_t)t * E + e] = win[(size_t)(t + 1) * E + e];
+    else
+      for (int t = 0; t + 1 < T; ++t) win[(size_t)t * E + e] = 0.f;
+    float v = 0.f;
+    if (op != V2V_SLOT_CLEAR) {
+      if (dtype == 0) v = (float)reinterpret_cast<const uint8_t*>(frames)[idx];
+      else if (dtype == 1) v = (float)reinterpret_cast<const int*>(frames)[idx];
+      else v = reinterpret_cast<const float*>(frames)[idx];
+    }
+    win[(size_t)(T - 1) * E + e] = v;
+  }
+}
+
 // util.tensor2im (util/util.py:48-71) per image: (B,C,H,W) float in [-1,1] -> (B,H,W,C) uint8 = clip((x + 1) / 2 * 255, 0, 255)
 // truncated
 __global__ void tensor2im_u8_kernel(const float* __restrict__ img, uint8_t* __restrict__ out, int C, size_t HW, size_t total) {
@@ -159,6 +184,14 @@ cudaError_t launch_avgpool3s2(const float* in, float* out, int P, int H, int W, 
 }
 cudaError_t launch_ids_window_push(float* window, const void* frame, int dtype, int B, int T, int H, int W, cudaStream_t s) {
   ids_window_push_kernel<<<grid1d((size_t)B * H * W), 256, 0, s>>>(window, frame, dtype, T, (size_t)H * W, (size_t)B * H * W);
+  return cudaGetLastError();
+}
+cudaError_t launch_slots_window_push(float* window, const void* frames, int dtype, int B, int T, int C, int H, int W, const int* ops,
+                                    cudaStream_t s) {
+  SlotOps o{};
+  for (int b = 0; b < B; ++b) o.v[b] = ops[b];
+  const size_t E = (size_t)C * H * W;
+  slots_window_push_kernel<<<grid1d((size_t)B * E), 256, 0, s>>>(window, frames, dtype, T, E, (size_t)B * E, o);
   return cudaGetLastError();
 }
 cudaError_t launch_tensor2im_u8(const float* img, uint8_t* out, int B, int C, int H, int W, cudaStream_t s) {

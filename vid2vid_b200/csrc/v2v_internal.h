@@ -101,6 +101,9 @@ struct FinalizeParams {
   float* mean_out;         // training plans: batch / instance mean and 1/sqrt(var + eps), same indexing; may be null
   float* rstd_out;
   int c_off, scale_stride; // channel slice of the raw tensor this norm layer covers
+  // per-image flags (v2v_plan_set_image_flags): int32 (N,) tensor at io[flags_slot], read at run time; -1: every image active
+  void* const* io;
+  int flags_slot = -1;
 };
 
 struct ConvKernelParams {
@@ -249,6 +252,7 @@ struct CompositeParams {
   int N, H, W;
   int align_corners;
   int use_warp;            // 0: img_final = img_raw (use_raw_only / no_flow)
+  int s_flags = -1;        // >= 0: int32 (N,) per-image flags; an image with V2V_IMAGE_RAW_ONLY takes img_raw as if use_warp were 0
 };
 
 // 2x2 / stride-2 max-pool (floor) between two activation buffers: out interior = max over each window of in's interior

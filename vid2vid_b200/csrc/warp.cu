@@ -8,6 +8,7 @@
 // the flag is explicit.  Coordinate arithmetic mirrors get_grid (networks.py:79-93: torch.linspace)
 // and ATen's grid_sampler unnormalise / clip so results agree with the oracle to ~1e-6.
 #include <cstdlib>
+#include "../../include/v2v_b200.h"
 #include "ptx.cuh"
 #include "v2v_internal.h"
 
@@ -47,6 +48,11 @@ __device__ __forceinline__ float bilerp(const float* pl, const Bilerp& b, int W)
          v11 * (b.wx * b.wy);
 }
 
+// warp image n: the plan warps (use_warp) and the image's run-time flags do not ask for the raw image only
+__device__ __forceinline__ bool image_warps(const CompositeParams& p, int n) {
+  return p.use_warp && !(p.s_flags >= 0 && (reinterpret_cast<const int*>(p.io[p.s_flags])[n] & V2V_IMAGE_RAW_ONLY));
+}
+
 __global__ void composite_kernel(CompositeParams p) {
   const size_t HW = (size_t)p.H * p.W;
   const size_t total = (size_t)p.N * HW;
@@ -66,7 +72,7 @@ __global__ void composite_kernel(CompositeParams p) {
     float r[3], f[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) r[c] = raw[((size_t)n * 3 + c) * HW + pix];
-    if (p.use_warp) {
+    if (image_warps(p, n)) {
       const float fx = flow[((size_t)n * 2 + 0) * HW + pix], fy = flow[((size_t)n * 2 + 1) * HW + pix];
       const float w = wgt[(size_t)n * HW + pix];
       const Bilerp b = warp_coords(x, y, fx, fy, p.W, p.H, p.align_corners);
@@ -111,7 +117,7 @@ __global__ void __launch_bounds__(128) composite_vec4_kernel(CompositeParams p) 
   float4 r[3], f[3];
 #pragma unroll
   for (int c = 0; c < 3; ++c) r[c] = ld4(raw, c, 3);
-  if (p.use_warp) {
+  if (image_warps(p, n)) {
     const float* flow = reinterpret_cast<const float*>(p.io[p.s_flow]);
     const float* prev = reinterpret_cast<const float*>(p.io[p.s_prev]);
     const float4 fx = ld4(flow, 0, 2), fy = ld4(flow, 1, 2);

@@ -5,6 +5,7 @@ generate_first_frame / compute_mask / build_pyr), with every tensor op routed to
 Inference only in this round (the reference's own `inference` runs under torch.no_grad,
 vid2vid_model_G.py:199); the training forward needs the backward kernels (DESIGN.md, next rows).
 """
+import collections
 import contextlib
 import os
 
@@ -217,7 +218,8 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         n = self._clips() if self.fake_B_prev is not None else 0
         if clips is not None and n > 1 and sorted(set(clips)) != list(range(n)):
             raise NotImplementedError('restarting clip(s) %s of a running batch of %d clips is not supported: the clips of a batch '
-                                      'start and advance together; call reset_stream() to restart the whole batch' % (list(clips), n))
+                                      'start and advance together; call reset_stream() to restart the whole batch, or use '
+                                      'stream_slots(B), whose slots start and stop independently' % (list(clips), n))
         self.fake_B_prev = None
         self._win_A = self._win_I = None
 
@@ -277,6 +279,12 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         else:
             out_u8.copy_(self._u8_dev, non_blocking=True)
         return out_u8
+
+    def stream_slots(self, B):
+        """A slot stream (SlotStream) of B slots over this model's generators: every slot starts, restarts and stops its own
+        clips, and each clip's frames equal its own batch-1 inference_stream / inference run bit for bit.  Its state is its
+        own: this model's inference / inference_stream state is left as it is."""
+        return SlotStream(self, B)
 
     def generate_frame_infer(self, real_A, s):
         """vid2vid_model_G.py:211-229."""
@@ -414,3 +422,173 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         if fake_B.size()[1] > 1:
             fake_B_prev = torch.cat([fake_B_prev, fake_B[:, :-1].detach()], dim=1)
         return fake_B_prev
+
+
+class SlotStep(collections.namedtuple('SlotStep', 'ops ready join raw_only')):
+    """What one SlotStream step does per slot: the window op (v2v_slots_window_push, _lib.SLOT_*), whether the slot produces
+    a frame (ready), whether this is its clip's first produced frame (join: its previous frames are seeded first) and
+    whether that frame takes the raw composite (raw_only: a join under --no_first_img)."""
+
+    def flags(self):
+        """The per-image flags of the generators' slot plans (_lib.IMAGE_ACTIVE | IMAGE_RAW_ONLY)."""
+        from . import _lib as L
+        return [(L.IMAGE_ACTIVE if r else 0) | (L.IMAGE_RAW_ONLY if o else 0) for r, o in zip(self.ready, self.raw_only)]
+
+
+class SlotSchedule:
+    """Host bookkeeping of a slot stream: B slots, each feeding its clip through a tG-frame window.  start(k) (a new clip,
+    restarting a busy slot) and stop(k) (the slot goes idle) take effect at the next step().  A slot produces a frame once its
+    window holds tG frames of its clip, so a clip's first tG - 1 steps produce nothing, as with inference_stream."""
+
+    def __init__(self, B, tG, no_first_img=False):
+        from . import _lib as L
+        if not 1 <= B <= L.MAX_SLOTS:
+            raise ValueError('a slot stream has 1 to %d slots, not %d' % (L.MAX_SLOTS, B))
+        self.B, self.tG, self.no_first_img = B, tG, bool(no_first_img)
+        self.frames = [0] * B          # frames of the slot's running clip so far (0: idle)
+        self._next = [None] * B        # 'start' / 'stop' at the next step
+
+    def _slot(self, k):
+        if isinstance(k, bool) or not isinstance(k, int) or not 0 <= k < self.B:
+            raise IndexError('slot %r is out of range for a stream of %d slots' % (k, self.B))
+        return k
+
+    def start(self, k):
+        self._next[self._slot(k)] = 'start'
+
+    def stop(self, k):
+        self._next[self._slot(k)] = 'stop'
+
+    def step(self):
+        from . import _lib as L
+        ops = []
+        for k in range(self.B):
+            nxt, self._next[k] = self._next[k], None
+            if nxt == 'start':
+                self.frames[k] = 1
+                ops.append(L.SLOT_RESTART)
+            elif nxt == 'stop':
+                self.frames[k] = 0
+                ops.append(L.SLOT_CLEAR)
+            elif self.frames[k]:
+                self.frames[k] += 1
+                ops.append(L.SLOT_PUSH)
+            else:
+                ops.append(L.SLOT_KEEP)
+        ready = [n >= self.tG for n in self.frames]
+        join = [n == self.tG for n in self.frames]
+        return SlotStep(ops, ready, join, [j and self.no_first_img for j in join])
+
+
+class SlotStream:
+    """B slots over one set of per-sample generator plans (Vid2VidModelG.stream_slots).  Every slot starts a clip, restarts
+    with a new one or goes idle between steps; the batch shape never changes, so each scale keeps one slot plan and one CUDA
+    graph.  Slots that are idle or still filling their window are computed but produce nothing and leave the running
+    statistics alone: every clip's frames, and the running statistics, are those of its own batch-1 run."""
+
+    def __init__(self, model, B):
+        opt = model.opt
+        if opt.dataset_mode == 'face' and model.use_single_G:
+            raise ValueError('a slot stream does not take the real frames that the face first-frame generator needs '
+                             '(use_single_G with dataset_mode face): use inference()')
+        if not (opt.no_first_img or (model.use_single_G and not opt.use_real_img)):
+            raise ValueError('a slot stream seeds the first frames of a joining clip with --no_first_img or --use_single_G '
+                             '(it takes no real frames)')
+        self.model, self.B, self.tG = model, B, opt.n_frames_G
+        self.schedule = SlotSchedule(B, self.tG, opt.no_first_img)
+        self.C = 1 if opt.label_nc != 0 else opt.input_nc
+        self._win_A = self._win_I = self.fake_B_prev = self._flags = self._u8_dev = None
+
+    def start(self, k):
+        """Slot k begins a new clip at its next frame (restarting it if busy)."""
+        self.schedule.start(k)
+
+    def stop(self, k):
+        """Slot k goes idle from its next step on."""
+        self.schedule.stop(k)
+
+    def _check(self, frames, inst):
+        B, opt = self.B, self.model.opt
+        if opt.label_nc != 0:
+            if frames.dim() != 3 or frames.shape[0] != B:
+                raise ValueError('frames must be (%d, H, W) id maps, got %s' % (B, tuple(frames.shape)))
+            if frames.dtype not in Vid2VidModelG._DT:
+                raise TypeError('id maps must be uint8, int32 or float32')
+        elif frames.dim() != 4 or tuple(frames.shape[:2]) != (B, self.C) or frames.dtype != torch.float32:
+            raise ValueError('frames must be (%d, %d, H, W) float32, got %s %s' % (B, self.C, tuple(frames.shape), frames.dtype))
+        if inst is not None and (tuple(inst.shape) != tuple(frames.shape) or inst.dtype not in Vid2VidModelG._DT):
+            raise ValueError('inst %s does not match frames %s' % (tuple(inst.shape), tuple(frames.shape)))
+        H, W = frames.shape[-2:]
+        if self._win_A is not None and tuple(self._win_A.shape[-2:]) != (H, W):
+            raise ValueError('this slot stream runs %dx%d frames, got %dx%d' % (self._win_A.shape[-2], self._win_A.shape[-1], H, W))
+        return H, W
+
+    def step(self, frames, inst=None, out_u8=None):
+        """One frame for every slot: `frames` are the slots' newest frames, (B, H, W) id maps (uint8 / int32 / float32) when
+        label_nc != 0 or (B, input_nc, H, W) float32 frames, host or device; rows of idle slots are ignored.  Returns
+        (frames, ready): the generated (B, 3, H, W) float frames -- or `out_u8` ((B, H, W, 3) uint8, host or device) filled
+        with util.tensor2im's images -- and a host list of B bools, ready[k] = slot k produced a frame this step."""
+        import ctypes as C
+        from . import _lib as L
+        m, opt, B, tG = self.model, self.model.opt, self.B, self.tG
+        H, W = self._check(frames, inst)
+        dev = m.device_
+        if self._win_A is None:
+            self._win_A = torch.zeros(B, tG, self.C, H, W, device=dev)
+            self._win_I = torch.zeros(B, tG, 1, H, W, device=dev) if opt.use_instance else None
+            self.fake_B_prev, h, w = [], H, W
+            for _ in range(m.n_scales):            # build_pyr's level extents
+                self.fake_B_prev.append(torch.zeros(B, tG - 1, opt.output_nc, h, w, device=dev))
+                h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+            self._flags = torch.zeros(B, dtype=torch.int32, device=dev)
+        st = self.schedule.step()
+        ops = (C.c_int * B)(*st.ops)
+        for win, fr in ((self._win_A, frames), (self._win_I, inst if inst is not None else frames)):
+            if win is None:
+                continue
+            fr = fr.to(dev, non_blocking=True).contiguous()
+            L.check(L.lib().v2v_slots_window_push(C.c_void_p(win.data_ptr()), C.c_void_p(fr.data_ptr()), Vid2VidModelG._DT[fr.dtype],
+                                                  B, tG, win.shape[2], H, W, ops, L.current_stream_ptr()))
+            L.LAUNCHES[0] += 1
+        # one asynchronous pinned copy: the slot plans read the flags through their IO tables, so their graphs stay valid
+        self._flags.copy_(torch.tensor(st.flags(), dtype=torch.int32).pin_memory(), non_blocking=True)
+        with torch.no_grad():
+            real_A, _, _ = m.encode_input(self._win_A, None, self._win_I)
+            for k in range(B):
+                if st.join[k]:
+                    self._seed_first_frames(real_A, k)
+            real_A = m.build_pyr(real_A)
+            feats = (None, None, None)
+            with m._per_clip_statistics(True):
+                for s in range(m.n_scales):
+                    si = m.n_scales - 1 - s
+                    ra = real_A[si]
+                    h, w = ra.shape[-2:]
+                    mask = m.compute_mask(ra, tG - 1) if opt.fg else None
+                    fake_B, _, _, _, *feats = getattr(m, 'netG' + str(s)).forward(
+                        ra[:, :tG].reshape(B, -1, h, w), self.fake_B_prev[si].reshape(B, -1, h, w), mask, *feats, False,
+                        image_flags=self._flags)
+                    self.fake_B_prev[si] = torch.cat([self.fake_B_prev[si][:, 1:], fake_B.unsqueeze(1)], dim=1)
+        if out_u8 is None:
+            return fake_B, st.ready
+        if self._u8_dev is None or tuple(self._u8_dev.shape) != (B, H, W, fake_B.shape[1]):
+            self._u8_dev = torch.empty(B, H, W, fake_B.shape[1], dtype=torch.uint8, device=dev)
+        L.check(L.lib().v2v_tensor2im_u8(C.c_void_p(fake_B.data_ptr()), C.c_void_p(self._u8_dev.data_ptr()), B, fake_B.shape[1], H,
+                                         W, L.current_stream_ptr()))
+        L.LAUNCHES[0] += 1
+        out_u8.copy_(self._u8_dev, non_blocking=not out_u8.is_cuda)
+        return out_u8, st.ready
+
+    def _seed_first_frames(self, real_A, k):
+        """Slot k's previous frames when its window first fills: zeros (--no_first_img, with the raw composite this step) or
+        netG_i on the first tG - 1 frames of its window at batch 1 (--use_single_G), as generate_first_frame makes them for
+        a batch-1 run, copied into the slot's rows of every scale."""
+        m, opt = self.model, self.model.opt
+        if opt.no_first_img:
+            for prev in self.fake_B_prev:
+                prev[k].zero_()
+            return
+        a = real_A[k:k + 1, :, :opt.label_nc] if opt.use_instance else real_A[k:k + 1]
+        first = torch.cat([m.netG_i.forward(a[:, i].contiguous(), None).unsqueeze(1) for i in range(self.tG - 1)], dim=1)
+        for prev, p in zip(self.fake_B_prev, m.build_pyr(first)):
+            prev[k] = p[0]

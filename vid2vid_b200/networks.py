@@ -395,7 +395,7 @@ class _Planned(nn.Module):
 
 
 # IO slots of the composite generators
-S_IN, S_PREV, S_MASK, S_FINAL, S_FLOW, S_W, S_RAW, S_IMGF, S_FLOWF, S_FGF, S_FG, S_CI, S_CF, S_CG, S_RAWC = range(15)
+S_IN, S_PREV, S_MASK, S_FINAL, S_FLOW, S_W, S_RAW, S_IMGF, S_FLOWF, S_FGF, S_FG, S_CI, S_CF, S_CG, S_RAWC, S_FLAGS = range(16)
 
 
 class CompositeGenerator(_Planned):
@@ -485,7 +485,7 @@ class CompositeGenerator(_Planned):
                        S_FG if self.use_fg_model else -1, S_MASK if self.use_fg_model else -1, S_FINAL, N, H, W, warp,
                        self.align_corners, s_raw_out=S_RAWC if (plan.train and self.use_fg_model) else -1)   # :216-230
 
-    def _run(self, key, coarse, input, img_prev, mask, use_raw_only):
+    def _run(self, key, coarse, input, img_prev, mask, use_raw_only, image_flags=None):
         self._require_cuda(input, img_prev, mask, *coarse)
         input, img_prev = input.contiguous(), img_prev.contiguous()
         N, _, H, W = input.shape
@@ -497,10 +497,22 @@ class CompositeGenerator(_Planned):
         if self.output_nc != 3:
             raise NotImplementedError('the fused composite kernel handles 3 output channels')
         train = self._wants_grad(input, img_prev, *coarse)
+        build = lambda p: self._describe(p, N, H, W, use_raw_only)
+        if image_flags is not None:
+            # slot plans: a per-sample plan that reads per-image flags (Plan.set_image_flags), cached under its own key
+            if train:
+                raise RuntimeError('per-image flags are for inference plans: a slot plan has no gradient')
+            if not self.sample_stats:
+                raise ValueError('per-image flags need per-sample statistics (sample_stats = True)')
+            if not image_flags.is_cuda or image_flags.dtype != torch.int32 or image_flags.numel() != N:
+                raise ValueError('image_flags must be an int32 CUDA tensor of %d elements' % N)
+            key = key + ('image_flags',)
+            build = lambda p: (p.set_image_flags(S_FLAGS), self._describe(p, N, H, W, use_raw_only))
         plan = self._get_plan(key + (N, H, W, bool(use_raw_only), bool(self.align_corners), bool(self.input_exact_bf16)), input.device,
-                              lambda p: self._describe(p, N, H, W, use_raw_only), train=train)
+                              build, train=train)
         new = lambda c: torch.empty((N, c, H, W), device=input.device, dtype=torch.float32)
-        io = [None] * 15
+        io = [None] * 16
+        io[S_FLAGS] = image_flags
         io[S_IN], io[S_PREV] = input, img_prev
         io[S_FINAL], io[S_RAW], io[S_IMGF] = new(self.output_nc), new(self.output_nc), new(self._feat_c())
         if not self.no_flow:
@@ -533,8 +545,11 @@ class CompositeGenerator(_Planned):
     def _fg_feat_c(self):
         return self.indv_final[1].in_channels
 
-    def forward(self, input, img_prev, mask, img_feat_coarse, flow_feat_coarse, img_fg_feat_coarse, use_raw_only):
-        return self._run(('G',), (), input, img_prev, mask, use_raw_only)
+    def forward(self, input, img_prev, mask, img_feat_coarse, flow_feat_coarse, img_fg_feat_coarse, use_raw_only, image_flags=None):
+        """image_flags: None, or an int32 (N,) CUDA tensor of per-image flags (plan.L.IMAGE_ACTIVE | IMAGE_RAW_ONLY) read at run
+        time by a slot plan (per-sample statistics; inactive images leave the running statistics alone, raw-only images take
+        the raw composite)."""
+        return self._run(('G',), (), input, img_prev, mask, use_raw_only, image_flags)
 
 
 class CompositeLocalGenerator(CompositeGenerator):
@@ -597,9 +612,9 @@ class CompositeLocalGenerator(CompositeGenerator):
             emit_head(plan, self.indv_final, fg_feat, (S_FG, self.output_nc, 1.0))
         self._emit_composite(plan, N, H, W, use_raw_only)
 
-    def forward(self, input, img_prev, mask, img_feat_coarse, flow_feat_coarse, img_fg_feat_coarse, use_raw_only):
+    def forward(self, input, img_prev, mask, img_feat_coarse, flow_feat_coarse, img_fg_feat_coarse, use_raw_only, image_flags=None):
         return self._run(('GL',), (img_feat_coarse, flow_feat_coarse, img_fg_feat_coarse), input, img_prev, mask,
-                         use_raw_only)
+                         use_raw_only, image_flags)
 
 
 class GlobalGenerator(_Planned):

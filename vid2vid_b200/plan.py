@@ -86,6 +86,13 @@ class Plan:
         except Exception:
             pass
 
+    def set_image_flags(self, slot):
+        """Per-image flags (v2v_plan_set_image_flags; per-sample inference plans): IO slot `slot` holds an int32 (N,) device
+        tensor read at run time -- IMAGE_ACTIVE (the image updates the running statistics) | IMAGE_RAW_ONLY (its composite
+        takes the raw image) -- so a captured graph serves every combination."""
+        L.check(L.lib().v2v_plan_set_image_flags(self._h, slot))
+        self.n_slots = max(self.n_slots, slot + 1)
+
     # ---- description
     def input(self, slot, N, C_src, c_off, Cn, H, W, exact_bf16=False):
         v = C.c_int()
