@@ -23,6 +23,8 @@ sys.path.insert(0, ROOT)
 from vid2vid_b200 import networks as NW, ops               # noqa: E402
 from vid2vid_b200.utils import make_opt                    # noqa: E402
 
+SIZE = 512          # the demo's square frames (tests/product_plans.py lowers the first-frame networks at this size)
+
 
 def _ms(fn, reps, warm=3):
     for _ in range(warm):
@@ -50,7 +52,7 @@ def card():
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--reps', type=int, default=20)
-    ap.add_argument('--size', type=int, default=512)
+    ap.add_argument('--size', type=int, default=SIZE)
     a = ap.parse_args()
     assert torch.cuda.is_available(), 'time_face.py needs a CUDA device'
     NW.set_default_precision('precise')

@@ -23,6 +23,11 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), '..'
 from vid2vid_b200 import ops                                  # noqa: E402
 from oracle import face_disc_oracle as FD                      # noqa: E402
 
+# The measured step's options (tests/product_plans.py lowers the same networks at the same size for the conv census).
+SIZE = 512
+OPT = dict(label_nc=0, input_nc=6, use_instance=False, fg=False, n_scales_spatial=2, ngf=128, ndf=64, num_D=3, n_scales_temporal=2,
+           isTrain=True, no_vgg=True, n_frames_total=12, no_first_img=True, dataroot='datasets/pose', dataset_mode='pose')
+
 
 def _trainer(add_face_disc, H, W):
     from vid2vid_b200 import flownet as FN
@@ -30,9 +35,7 @@ def _trainer(add_face_disc, H, W):
     from vid2vid_b200.model_g import Vid2VidModelG
     from vid2vid_b200.trainer import Trainer
     from vid2vid_b200.utils import make_opt
-    opt = make_opt(label_nc=0, input_nc=6, use_instance=False, fg=False, n_scales_spatial=2, ngf=128, ndf=64, num_D=3,
-                   n_scales_temporal=2, isTrain=True, no_vgg=True, gpu_ids=[0], n_frames_total=12, no_first_img=True,
-                   add_face_disc=add_face_disc, fineSize=H, loadSize=H, dataroot='datasets/pose', dataset_mode='pose')
+    opt = make_opt(gpu_ids=[0], add_face_disc=add_face_disc, fineSize=H, loadSize=H, **OPT)
     torch.manual_seed(1234)
     G, D, F = Vid2VidModelG().initialize(opt), Vid2VidModelD().initialize(opt), FN.FlowNet().initialize(opt)
     return Trainer(opt, G, D, F, world=1), opt
@@ -95,7 +98,7 @@ def main():
                            text=True).stdout.strip()
     out = {'gpu': torch.cuda.get_device_name(0), 'power_limit': limit,
            'face_region_us': {'1x6x512x512': region_us(1, 512, 512), '8x6x1024x1024': region_us(8, 1024, 1024)},
-           'train_step_ms': train_steps(512, 512, args.steps, args.rounds)}
+           'train_step_ms': train_steps(SIZE, SIZE, args.steps, args.rounds)}
     print(json.dumps(out))
 
 

@@ -19,6 +19,8 @@ import torch
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), '..'))
 from vid2vid_b200 import networks as NW                     # noqa: E402
 
+LOSS_SIZES = ((512, 1024), (1024, 2048))      # (H, W) of the timed loss calls; tests/product_plans.py lowers their plans
+
 
 def _ms(fn, reps, warm=2):
     for _ in range(warm):
@@ -111,7 +113,7 @@ def main():
     crit = NW.VGGLoss(0, synthetic=True)
     crit.vgg.precision = 'precise'
     out = {'gpu': torch.cuda.get_device_name(0), 'precision': 'precise',
-           'loss_ms': {'1024x512': loss_times(crit, 512, 1024, args.reps), '2048x1024': loss_times(crit, 1024, 2048, args.reps)},
+           'loss_ms': {'%dx%d' % (W, H): loss_times(crit, H, W, args.reps) for H, W in LOSS_SIZES},
            'conv_rate_1024x512': conv_rate(crit, 512, 1024)}
     if not args.no_train:
         del crit
