@@ -756,9 +756,20 @@ int v2v_plan_repack(v2v_plan* P, v2v_stream_t stream_) {
   return 0;
 }
 
+// The vectorised composite moves its streamed slots as float4: refuse caller tensors that are not 16-byte aligned (a view
+// at an odd float offset) on the host, before anything is launched.
+static int check_composite_alignment(const v2v_plan* P, void* const* io_ptrs) {
+  for (const XOp& x : P->xops)
+    if (x.kind == X_COMPOSITE && composite_vec4(x.comp))
+      V2V_REQUIRE(composite_slots_aligned(x.comp, io_ptrs), V2V_ERR_INVALID,
+                  "composite (W %% 4 == 0) needs 16-byte aligned raw / final / flow / weight / fg / mask tensors");
+  return 0;
+}
+
 int v2v_plan_run(v2v_plan* P, void* const* io_ptrs, int n_io, int use_graph, v2v_stream_t stream_) {
   V2V_REQUIRE(P && P->finalized, V2V_ERR_STATE, "plan not finalized");
   V2V_REQUIRE(n_io >= P->n_slots && io_ptrs, V2V_ERR_INVALID, "need %d io pointers, got %d", P->n_slots, n_io);
+  if (int rc = check_composite_alignment(P, io_ptrs)) return rc;
   DeviceGuard guard(P->device);
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   V2V_CUDA(cudaMemcpyAsync(P->io_dev, io_ptrs, sizeof(void*) * P->n_slots, cudaMemcpyHostToDevice, stream));
@@ -802,6 +813,7 @@ int v2v_plan_profile(v2v_plan* P, void* const* io_ptrs, int n_io, v2v_stream_t s
                      float* ms, double* macs, int* n_ops) {
   V2V_REQUIRE(P && P->finalized, V2V_ERR_STATE, "plan not finalized");
   V2V_REQUIRE(n_io >= P->n_slots && io_ptrs && kinds && ms && macs && n_ops, V2V_ERR_INVALID, "bad profile arguments");
+  if (int rc = check_composite_alignment(P, io_ptrs)) return rc;
   DeviceGuard guard(P->device);
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   V2V_CUDA(cudaMemcpyAsync(P->io_dev, io_ptrs, sizeof(void*) * P->n_slots, cudaMemcpyHostToDevice, stream));

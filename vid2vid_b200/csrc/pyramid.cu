@@ -173,7 +173,9 @@ cudaError_t launch_onehot_edges(const float* labels, const float* inst, float* o
 }
 cudaError_t launch_avgpool3s2(const float* in, float* out, int P, int H, int W, cudaStream_t s) {
   const int Ho = (H - 1) / 2 + 1, Wo = (W - 1) / 2 + 1;
-  if (W % 4 == 0 && W >= 4) {
+  // the vector kernel loads float4 rows and stores float2 pairs: a caller's view at an odd float offset takes the scalar one
+  const bool aligned = (reinterpret_cast<uintptr_t>(in) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0;
+  if (W % 4 == 0 && W >= 4 && aligned) {
     dim3 grid((W / 4 + 127) / 128, Ho, P < 64 ? P : 64);
     avgpool3s2_vec_kernel<<<grid, 128, 0, s>>>(in, out, P, H, W, Ho, Wo);
     return cudaGetLastError();

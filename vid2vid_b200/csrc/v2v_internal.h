@@ -287,6 +287,8 @@ cudaError_t launch_act_copy(const CopyParams& p, cudaStream_t stream);
 cudaError_t launch_bias_affine(float* scale, float* shift, const float* bias, int N, int C, int stride, cudaStream_t stream);
 cudaError_t launch_correlation(const float*, const float*, float*, int, int, int, int, int, int, int, int, int, cudaStream_t);
 cudaError_t launch_composite(const CompositeParams& p, cudaStream_t stream);
+bool composite_vec4(const CompositeParams& p);                                  // launch_composite takes the float4 kernel
+bool composite_slots_aligned(const CompositeParams& p, void* const* io);       // host io table: its float4 slots 16-byte aligned
 cudaError_t launch_maxpool2(const PoolParams& p, cudaStream_t stream);
 // gin (dense NHWC fp32, in's logical extent and Cvalid channels) += gout routed to the first maximum of each window
 cudaError_t launch_maxpool2_bwd(const PoolParams& p, const float* gout, float* gin, cudaStream_t stream);

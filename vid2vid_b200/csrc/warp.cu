@@ -179,8 +179,18 @@ static inline int grid1d(size_t total) {
   return (int)(b < cap ? (b ? b : 1) : cap);
 }
 
+bool composite_vec4(const CompositeParams& p) { return p.W % 4 == 0 && p.H <= 65535 && p.N <= 65535; }
+
+// the slots composite_vec4_kernel moves as float4: raw, final, raw_out, and flow / weight / fg / mask when present
+bool composite_slots_aligned(const CompositeParams& p, void* const* io) {
+  const int slots[] = {p.s_raw, p.s_final, p.s_raw_out, p.use_warp ? p.s_flow : -1, p.use_warp ? p.s_weight : -1, p.s_fg, p.s_mask};
+  for (int s : slots)
+    if (s >= 0 && (reinterpret_cast<uintptr_t>(io[s]) & 15) != 0) return false;
+  return true;
+}
+
 cudaError_t launch_composite(const CompositeParams& p, cudaStream_t stream) {
-  if (p.W % 4 == 0 && p.H <= 65535 && p.N <= 65535)
+  if (composite_vec4(p))
     composite_vec4_kernel<<<dim3((p.W / 4 + 127) / 128, p.H, p.N), 128, 0, stream>>>(p);
   else
     composite_kernel<<<grid1d((size_t)p.N * p.H * p.W), 256, 0, stream>>>(p);
