@@ -532,36 +532,50 @@ cudaError_t launch_conv_bwd(const BwdConv& p, cudaStream_t s) {
   }
   if (p.dbias || p.dbias2) {
     const long long npix = (long long)p.N * p.oh * p.ow;
-    dim3 grid(p.Cout, (unsigned)std::max(1LL, std::min(64LL, npix / 4096)));
+    dim3 grid(p.Cout, (unsigned)bias_grad_blocks(npix));
     bias_grad_kernel<<<grid, 256, 0, s>>>(p.dy, p.dy_C, npix, p.Cout, p.dbias, p.dbias2, p.w2 ? p.Cout1 : p.Cout);
   }
   return cudaGetLastError();
 }
 
+int bias_grad_blocks(long long npix) { return (int)std::max(1LL, std::min(64LL, npix / 4096)); }
+
 cudaError_t launch_bias_grad(const float* dy, int dy_C, long long npix, int C, float* dbias, float* dbias2, int C1, cudaStream_t s) {
-  dim3 grid(C, (unsigned)std::max(1LL, std::min(64LL, npix / 4096)));
+  dim3 grid(C, (unsigned)bias_grad_blocks(npix));
   bias_grad_kernel<<<grid, 256, 0, s>>>(dy, dy_C, npix, C, dbias, dbias2, C1);
   return cudaGetLastError();
+}
+
+// The vectorised reduce aims at 4 blocks per SM of the H100 SXM (132 SMs) over the batch, each block summing at least 8
+// pixel rows per thread; the scalar kernel takes one block per channel and image, split over up to 32 slices of 8192 pixels.
+NormBwdLaunch norm_bwd_launch(int N, int H, int W, int C, int raw_C, int c_off, int has_norm, int param) {
+  NormBwdLaunch l{};
+  const long long HW = (long long)H * W;
+  l.param = param;
+  l.grid[0] = l.grid[1] = l.grid[2] = 1;
+  if (!has_norm && !param) return l;               // norm-less unit without a bias gradient: draw = dz needs no sums
+  if (C % 4 == 0 && C <= 1024 && raw_C % 4 == 0 && c_off % 4 == 0) {
+    l.reduce = 1;
+    l.ppb = 256 / (C / 4);
+    const long long want_blocks = std::max(1LL, (4LL * 132) / N);
+    l.chunk = std::max<long long>((long long)l.ppb * 8, (HW + want_blocks - 1) / want_blocks);
+    l.grid[0] = (int)((HW + l.chunk - 1) / l.chunk); l.grid[1] = N;
+  } else {
+    l.reduce = 2;
+    l.grid[0] = C; l.grid[1] = N; l.grid[2] = (int)std::max(1LL, std::min(32LL, HW / 8192));
+  }
+  return l;
 }
 
 cudaError_t launch_norm_bwd(const NormBwd& p, cudaStream_t s) {
   cudaError_t e = cudaMemsetAsync(p.sums, 0, sizeof(float) * 2 * p.N * p.C, s);
   if (e != cudaSuccess) return e;
-  if (p.has_norm || p.dbeta) {
-    const long long HW = (long long)p.H * p.W;
-    if (p.C % 4 == 0 && p.C <= 1024 && p.raw.C % 4 == 0 && p.c_off % 4 == 0) {
-      const int ppb = 256 / (p.C / 4);
-      const long long want_blocks = std::max(1LL, (4LL * 132) / p.N);
-      long long chunk = std::max<long long>((long long)ppb * 8, (HW + want_blocks - 1) / want_blocks);
-      dim3 grid((unsigned)((HW + chunk - 1) / chunk), p.N);
-      norm_bwd_reduce_vec_kernel<<<grid, 256, 2 * p.C * sizeof(float), s>>>(p, (int)chunk);
-    } else {
-      dim3 grid(p.C, p.N, (unsigned)std::max(1LL, std::min(32LL, HW / 8192)));
-      norm_bwd_reduce_kernel<<<grid, 256, 0, s>>>(p);
-    }
-  }
+  const NormBwdLaunch l = norm_bwd_launch(p.N, p.H, p.W, p.C, p.raw.C, p.c_off, p.has_norm, (p.dgamma || p.dbeta) ? 1 : 0);
+  const dim3 grid(l.grid[0], l.grid[1], l.grid[2]);
+  if (l.reduce == 1) norm_bwd_reduce_vec_kernel<<<grid, 256, 2 * p.C * sizeof(float), s>>>(p, (int)l.chunk);
+  else if (l.reduce == 2) norm_bwd_reduce_kernel<<<grid, 256, 0, s>>>(p);
   norm_bwd_apply_kernel<<<grid1d((size_t)p.N * p.H * p.W * p.C), 256, 0, s>>>(p);
-  if (p.dgamma || p.dbeta) norm_param_grad_kernel<<<(p.C + 127) / 128, 128, 0, s>>>(p);
+  if (l.param) norm_param_grad_kernel<<<(p.C + 127) / 128, 128, 0, s>>>(p);
   return cudaGetLastError();
 }
 

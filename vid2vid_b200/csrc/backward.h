@@ -74,6 +74,18 @@ cudaError_t launch_fold_add(const float* src, int Cs, int PH, int PW, float* dx,
                             cudaStream_t s);
 cudaError_t launch_bias_grad(const float* dy, int dy_C, long long npix, int C, float* dbias, float* dbias2, int C1, cudaStream_t s);
 
+// Launch shape of launch_norm_bwd, chosen on the host from the unit's extent alone (v2v_plan_describe reports the same).
+// param: norm_param_grad_kernel runs, i.e. the unit has gamma / beta (or, norm-less, a bias) whose gradient is requested.
+struct NormBwdLaunch {
+  int reduce;                  // per-channel sums: 0 none (norm-less unit without a bias gradient), 1 vectorised, 2 scalar kernel
+  int ppb;                     // vectorised: pixel rows per block pass (256 threads / (C / 4))
+  long long chunk;             // vectorised: pixels per block and image
+  int grid[3];                 // reduce grid (vectorised: chunks x N x 1; scalar: C x N x pixel slices)
+  int param;                   // norm_param_grad_kernel runs (norm_bwd_apply_kernel always does)
+};
+NormBwdLaunch norm_bwd_launch(int N, int H, int W, int C, int raw_C, int c_off, int has_norm, int param);
+int bias_grad_blocks(long long npix);          // bias_grad_kernel: blocks per channel (grid.y)
+
 cudaError_t launch_conv_bwd(const BwdConv& p, cudaStream_t s);
 cudaError_t launch_norm_bwd(const NormBwd& p, cudaStream_t s);
 cudaError_t launch_head_bwd(const HeadBwd& p, cudaStream_t s);

@@ -898,6 +898,9 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
         if (rc) return -1;
       }
     }
+    s += "],\"epilogue_backward\":[";
+    if (!P->sized && size_arena(P)) return -1;        // the raw tensors' element type and channel stride (host-only)
+    describe_epilogue_backward(P, s);
   }
   // ops the backward visits (0 for the forward-only branch of a feature L1 target) and values without a gradient buffer
   int bwd_ops = 0, detached = 0;

@@ -382,4 +382,52 @@ void describe_backward_unit(const BwdUnit& u, std::string& s) {
   }
 }
 
+// One record per live G_NORM_ACT / G_CONV_ACT / G_HEAD: the launches of its epilogue backward as run_backward makes them,
+// assuming every parameter gradient (gamma, beta, bias) is requested.  Norm units: the norm_bwd_launch choice; conv_act and
+// head units: the dense dz buffer's channel stride, the stacked second bias (channels from C1 on go to dbias2) and the
+// bias_grad grid.
+void describe_epilogue_backward(const v2v_plan* P, std::string& s) {
+  char t[640];
+  bool first = true;
+  for (size_t i = 0; i < P->gops.size(); ++i) {
+    const GOp& op = P->gops[i];
+    if (!P->op_live[i] || !(op.kind == G_NORM_ACT || op.kind == G_CONV_ACT || op.kind == G_HEAD)) continue;
+    if (!first) s += ",";
+    first = false;
+    if (op.kind == G_NORM_ACT) {
+      const Raw& r = P->raws[op.raw];
+      const GOp& cop = P->gops[r.conv_op];
+      const Value& vo = P->values[op.value_out];
+      const int has_norm = op.norm.kind != V2V_NORM_NONE;
+      const int param = has_norm ? (op.norm.gamma || op.norm.beta) : ((op.n_off == 0 ? cop.conv.bias : cop.conv.bias2) != nullptr);
+      const NormBwdLaunch l = norm_bwd_launch(vo.N, vo.H, vo.W, op.cC, r.desc.C, op.n_off, has_norm, param);
+      snprintf(t, sizeof(t),
+               "{\"kind\":\"norm_act\",\"gop\":%zu,\"raw\":%d,\"C\":%d,\"N\":%d,\"H\":%d,\"W\":%d,\"c_off\":%d,\"raw_C\":%d,\"raw_f32\":%d,"
+               "\"has_norm\":%d,\"batch_stats\":%d,\"act\":%d,\"adds\":%d,\"reduce\":\"%s\",\"ppb\":%d,\"chunk\":%lld,\"grid\":[%d,%d,%d],"
+               "\"param\":%d}",
+               i, op.raw, op.cC, vo.N, vo.H, vo.W, op.n_off, r.desc.C, r.desc.f32, has_norm, op.norm.kind == V2V_NORM_BATCH ? 1 : 0,
+               op.act, (op.add[0] >= 0) + (op.add[1] >= 0), l.reduce == 1 ? "vec" : (l.reduce == 2 ? "scalar" : "none"), l.ppb,
+               l.chunk, l.grid[0], l.grid[1], l.grid[2], l.param);
+      s += t;
+      continue;
+    }
+    const v2v_conv_desc& c = op.conv;
+    const Value& vin = P->values[op.value_in];
+    const long long npix = (long long)vin.N * op.geom.out_h * op.geom.out_w;
+    const int has_bias = c.bias != nullptr || (c.Cout2 > 0 && c.bias2 != nullptr);
+    snprintf(t, sizeof(t),
+             "{\"kind\":\"%s\",\"gop\":%zu,\"C\":%d,\"N\":%d,\"H\":%d,\"W\":%d,\"dz_C\":%d,\"bias\":%d,\"C1\":%d,\"bias_grid\":[%d,%d],"
+             "\"acts\":[",
+             op.kind == G_HEAD ? "head" : "conv_act", i, c.Cout, vin.N, op.geom.out_h, op.geom.out_w, round_up(c.Cout, 8), has_bias,
+             c.Cout2 > 0 ? c.Cout - c.Cout2 : c.Cout, has_bias ? c.Cout : 0, has_bias ? bias_grad_blocks(npix) : 0);
+    s += t;
+    const int nch = op.kind == G_HEAD ? c.Cout : 1;
+    for (int j = 0; j < nch; ++j) {
+      snprintf(t, sizeof(t), "%s%d", j ? "," : "", op.kind == G_HEAD ? op.head[j].act : op.act);
+      s += t;
+    }
+    s += "]}";
+  }
+}
+
 }  // namespace v2v

@@ -222,5 +222,6 @@ int build_backward_units(v2v_plan* P, cudaStream_t stream);
 int run_backward(v2v_plan* P, void* const* io, void* const* gio, const std::unordered_map<const void*, void*>& pg,
                  cudaStream_t s);
 void describe_backward_unit(const BwdUnit& u, std::string& s);
+void describe_epilogue_backward(const v2v_plan* P, std::string& s);
 
 }  // namespace v2v
