@@ -269,11 +269,23 @@ cudaError_t launch_stats_finalize(const FinalizeParams& p, cudaStream_t stream) 
   return cudaGetLastError();
 }
 
-// true: the row-segment kernel handles this launch; false: grid-stride fallback
-bool norm_apply_uses_rows(const ApplyParams& p) {
-  const int vecs = p.out.C / 8;
-  const int Hpad = p.out.H + p.out.pad_t + p.out.pad_b;
-  return vecs <= 256 && (long long)p.out.N * Hpad <= 65535;
+// Row-segment kernel while a block can hold one vector per thread of a padded row (vecs <= 256) and the rows fit grid.y;
+// the grid-stride kernel otherwise.  v2v_plan_describe reports the same choice.
+NormApplyLaunch norm_apply_launch(const ApplyParams& p) {
+  NormApplyLaunch l{};
+  const long long total = (long long)p.out.N * (p.out.H + p.out.pad_t + p.out.pad_b) *
+                          (p.out.W + p.out.pad_l + p.out.pad_r) * (p.out.C / 8);
+  const int Wpad = p.out.W + p.out.pad_l + p.out.pad_r, Hpad = p.out.H + p.out.pad_t + p.out.pad_b;
+  l.vecs = p.out.C / 8;
+  l.rows = l.vecs <= 256 && (long long)p.out.N * Hpad <= 65535;
+  if (l.rows) {
+    l.ppb = 256 / l.vecs;                           // pixels per block pass
+    l.xt = l.ppb * 8;                               // 8 items per thread
+    l.grid[0] = (Wpad + l.xt - 1) / l.xt; l.grid[1] = p.out.N * Hpad;
+  } else {
+    l.grid[0] = grid_for(total, 256); l.grid[1] = 1;
+  }
+  return l;
 }
 
 cudaError_t launch_norm_apply(const ApplyParams& p, cudaStream_t stream) {
@@ -282,12 +294,10 @@ cudaError_t launch_norm_apply(const ApplyParams& p, cudaStream_t stream) {
   if (total >= (1LL << 31)) return cudaErrorInvalidValue;
   const bool prec = p.raw.f32 != 0;
   if (prec != (p.out.split != 0)) return cudaErrorInvalidValue;      // precise plans: fp32 raw <-> split activations
-  const int vecs = p.out.C / 8;
-  const int Wpad = p.out.W + p.out.pad_l + p.out.pad_r, Hpad = p.out.H + p.out.pad_t + p.out.pad_b;
-  if (norm_apply_uses_rows(p)) {
-    const int ppb = 256 / vecs;                     // pixels per block pass
-    const int xt = ppb * 8;                         // 8 items per thread
-    dim3 grid((Wpad + xt - 1) / xt, p.out.N * Hpad);
+  const NormApplyLaunch l = norm_apply_launch(p);
+  if (l.rows) {
+    const dim3 grid(l.grid[0], l.grid[1]);
+    const int xt = l.xt, ppb = l.ppb;
     if (prec) {
       if (p.n_add == 0) norm_apply_rows_kernel<0, true><<<grid, 256, 0, stream>>>(p, xt, ppb);
       else if (p.n_add == 1) norm_apply_rows_kernel<1, true><<<grid, 256, 0, stream>>>(p, xt, ppb);
@@ -298,7 +308,7 @@ cudaError_t launch_norm_apply(const ApplyParams& p, cudaStream_t stream) {
       else norm_apply_rows_kernel<2, false><<<grid, 256, 0, stream>>>(p, xt, ppb);
     }
   } else {
-    norm_apply_kernel<<<grid_for(total, 256), 256, 0, stream>>>(p);
+    norm_apply_kernel<<<l.grid[0], 256, 0, stream>>>(p);
   }
   return cudaGetLastError();
 }

@@ -222,6 +222,159 @@ FeatL1Params featl1_params(const v2v_plan* P, const GOp& op) {
   return f;
 }
 
+// Where the statistics of each (raw, channel slice) are finalised, per graph op: 0 / 1 = the tail slot of the producing
+// tensor-core conv launch (the CTA that takes its last ticket, conv_umma.cu), 2 = a stand-alone stats_finalize launch (the
+// SIMT implementation, a third slice of one raw), -1 = nothing (not a normalising op, or a later pass over a slice an earlier
+// op finalises: a second output layout, defer_last).  The side effects happen once per slice, however many passes read it.
+std::vector<int> finalize_sites(const v2v_plan* P) {
+  std::vector<int> site(P->gops.size(), -1);
+  std::vector<std::vector<int>> done(P->raws.size());          // per raw: the slice offsets finalised so far
+  for (size_t i = 0; i < P->gops.size(); ++i) {
+    const GOp& op = P->gops[i];
+    if (op.kind != G_NORM_ACT || op.norm.kind == V2V_NORM_NONE) continue;
+    std::vector<int>& d = done[op.raw];
+    if (std::find(d.begin(), d.end(), op.n_off) != d.end()) continue;
+    site[i] = (P->impl == V2V_IMPL_UMMA && d.size() < 2) ? (int)d.size() : 2;
+    d.push_back(op.n_off);
+  }
+  return site;
+}
+
+// The finalisation of the slice a normalising G_NORM_ACT reads, with its train-mode side effects (running statistics; the
+// scale / shift / mean / rstd arrays the normalise passes and the backward read).  Arena pointers are valid after size_arena.
+static int finalize_params(const v2v_plan* P, const GOp& op, FinalizeParams& fp) {
+  const Raw& r = P->raws[op.raw];
+  const GOp& cop = P->gops[r.conv_op];
+  fp.stats = r.stats; fp.Cs = r.C; fp.C = op.cC; fp.c_off = op.n_off; fp.scale_stride = r.C;
+  fp.N = r.N;
+  fp.count = (double)r.H * r.W; fp.instance = (op.norm.kind == V2V_NORM_INSTANCE) || P->sample_stats;
+  fp.sample_running = P->sample_stats;
+  fp.io = P->io_dev; fp.flags_slot = P->flags_slot;
+  const int cout1 = cop.conv.Cout - cop.conv.Cout2;
+  V2V_REQUIRE(op.n_off == 0 || (cop.conv.Cout2 > 0 && op.n_off == cout1), V2V_ERR_UNSUPPORTED,
+              "a raw slice must start at channel 0 or at the second weight set");
+  fp.gamma = op.norm.gamma; fp.beta = op.norm.beta; fp.conv_bias = op.n_off == 0 ? cop.conv.bias : cop.conv.bias2;
+  fp.momentum = op.norm.momentum; fp.eps = op.norm.eps;
+  fp.running_mean = op.norm.running_mean; fp.running_var = op.norm.running_var;
+  fp.num_batches_tracked = reinterpret_cast<long long*>(op.norm.num_batches_tracked);
+  fp.scale = r.scale; fp.shift = r.shift; fp.mean_out = r.mean; fp.rstd_out = r.rstd;
+  return 0;
+}
+
+// The normalise pass of a G_NORM_ACT (or the plain conversion of a G_RAWIN) into output layout m of its value.  The raw is
+// read through the op's channel slice at the full row stride; scale / shift are the slice's (null: identity, G_RAWIN and
+// norm-less unbiased convs).  Arena pointers are valid after finalize; the launch shape depends on the layouts only.
+ApplyParams apply_params(const v2v_plan* P, const GOp& op, size_t m) {
+  const Value& vo = P->values[op.value_out];
+  ApplyParams ap{};
+  if (op.kind == G_RAWIN) {
+    ap.raw.base = const_cast<float*>(op.ext_raw); ap.raw.N = vo.N; ap.raw.H = vo.H; ap.raw.W = vo.W; ap.raw.C = op.ext_C;
+    ap.raw.Cvalid = vo.C; ap.raw.f32 = 1;
+    ap.scale = nullptr; ap.shift = nullptr; ap.scale_stride = 0; ap.act = ACT_NONE; ap.slope = 0.f; ap.n_add = 0;
+  } else {
+    const Raw& r = P->raws[op.raw];
+    const GOp& cop = P->gops[r.conv_op];
+    ap.raw = r.desc;
+    ap.raw.base = reinterpret_cast<uint8_t*>(r.desc.base) + (size_t)op.n_off * r.desc.elem_bytes();
+    ap.raw.Cvalid = op.cC;                                               // channel slice, full row stride
+    ap.scale = (op.norm.kind != V2V_NORM_NONE || cop.conv.bias != nullptr) ? r.scale + op.n_off : nullptr;
+    ap.shift = r.shift + op.n_off;
+    ap.scale_stride = r.C;
+    ap.act = op.act; ap.slope = op.slope;
+    ap.n_add = 0;
+    for (int k = 0; k < 2; ++k) if (op.add[k] >= 0) ap.add[ap.n_add++] = P->acts[P->values[op.add[k]].bufs[0]];
+  }
+  ap.out = P->acts[vo.bufs[m]]; ap.pad_mode = P->act_pad_mode[vo.bufs[m]];
+  return ap;
+}
+
+
+// The forward epilogue of the plan's norm layers, as finalize emits it (the same host functions choose it), three kinds of
+// record:
+//   stats     one per conv whose raw a norm layer reads: how conv_umma_kernel accumulates the statistics rows (async_epi, MG,
+//             BN, phases, units over ctas persistent CTAs) or raw_stats_kernel (SIMT), and where each slice is finalised;
+//   finalize  one per (raw, slice): batch / instance / per-sample statistics, image flags, running buffers, conv bias, the
+//             saved mean / rstd of training plans, the slice;
+//   apply     one per normalise pass and output layout: the norm_apply_launch choice and what the kernel reads and writes.
+void describe_epilogue_forward(v2v_plan* P, std::string& s) {
+  static const char* kSite[] = {"tail0", "tail1", "standalone"};
+  const std::vector<int> site = finalize_sites(P);
+  std::vector<std::vector<int>> slices(P->raws.size());      // per raw: finalising ops, in order
+  for (size_t i = 0; i < P->gops.size(); ++i) if (site[i] >= 0) slices[P->gops[i].raw].push_back((int)i);
+  char t[768];
+  bool first = true;
+  auto sep = [&]() { if (!first) s += ","; first = false; };
+  for (size_t i = 0; i < P->gops.size(); ++i) {
+    const GOp& op = P->gops[i];
+    if (op.kind != G_CONV || slices[op.raw].empty()) continue;
+    const Raw& r = P->raws[op.raw];
+    GOp tmp = op;
+    fill_conv_params(P, tmp);
+    const ConvKernelParams& kp = tmp.kp;
+    sep();
+    snprintf(t, sizeof(t),
+             "{\"kind\":\"stats\",\"gop\":%zu,\"raw\":%d,\"N\":%d,\"C\":%d,\"H\":%d,\"W\":%d,\"raw_f32\":%d,\"impl\":\"%s\","
+             "\"async_epi\":%d,\"MG\":%d,\"BN\":%d,\"phases\":%d,\"n_tiles\":%d,\"m_total\":%d,\"units\":%d,\"ctas\":%d,\"fin\":[",
+             i, op.raw, r.N, r.C, r.H, r.W, r.desc.f32, P->impl == V2V_IMPL_UMMA ? "umma" : "simt", conv_umma_async_epilogue(kp),
+             kp.MG, kp.BN, kp.num_phases, kp.n_tiles, kp.m_total, kp.total_units, kp.grid);
+    s += t;
+    for (size_t k = 0; k < slices[op.raw].size(); ++k) {
+      snprintf(t, sizeof(t), "%s\"%s\"", k ? "," : "", kSite[site[slices[op.raw][k]]]);
+      s += t;
+    }
+    s += "]}";
+  }
+  for (size_t i = 0; i < P->gops.size(); ++i) {
+    if (site[i] < 0) continue;
+    const GOp& op = P->gops[i];
+    FinalizeParams fp{};
+    finalize_params(P, op, fp);
+    sep();
+    snprintf(t, sizeof(t),
+             "{\"kind\":\"finalize\",\"gop\":%zu,\"raw\":%d,\"site\":\"%s\",\"stats\":\"%s\",\"N\":%d,\"flags\":%d,"
+             "\"running\":%d,\"bias\":%d,\"mean_rstd\":%d,\"c_off\":%d,\"C\":%d}",
+             i, op.raw, kSite[site[i]], fp.sample_running ? "sample" : (fp.instance ? "instance" : "batch"), fp.N,
+             fp.flags_slot >= 0, fp.running_mean != nullptr, fp.conv_bias != nullptr, P->train ? 1 : 0, fp.c_off, fp.C);
+    s += t;
+  }
+  std::vector<std::pair<int, int>> read;                     // (raw, slice) pairs an earlier normalise pass has read
+  for (size_t i = 0; i < P->gops.size(); ++i) {
+    const GOp& op = P->gops[i];
+    if (op.kind != G_NORM_ACT && op.kind != G_RAWIN) continue;
+    bool repeat = false;
+    if (op.kind == G_NORM_ACT) {
+      const std::pair<int, int> key(op.raw, op.n_off);
+      repeat = std::find(read.begin(), read.end(), key) != read.end();
+      if (!repeat) read.push_back(key);
+    }
+    const char* scale = op.kind == G_RAWIN ? "none" : (op.norm.kind != V2V_NORM_NONE ? "norm" :
+                        (P->gops[P->raws[op.raw].conv_op].conv.bias != nullptr ? "bias" : "none"));
+    const Value& vo = P->values[op.value_out];
+    for (size_t m = 0; m < vo.bufs.size(); ++m) {
+      const ApplyParams ap = apply_params(P, op, m);
+      const NormApplyLaunch l = norm_apply_launch(ap);
+      const ActDesc& o = ap.out;
+      const int Wpad = o.W + o.pad_l + o.pad_r;
+      sep();
+      snprintf(t, sizeof(t),
+               "{\"kind\":\"apply\",\"gop\":%zu,\"op\":\"%s\",\"raw\":%d,\"layout\":%zu,\"repeat\":%d,\"kernel\":\"%s\",\"prec\":%d,"
+               "\"nadd\":%d,\"vecs\":%d,\"ppb\":%d,\"xt\":%d,\"grid\":[%d,%d],\"idle\":%d,\"ragged\":%d,\"N\":%d,\"H\":%d,"
+               "\"W\":%d,\"C\":%d,\"Cvalid\":%d,\"raw_C\":%d,\"c_off\":%d,\"pad_mode\":%d,\"pads\":[%d,%d,%d,%d],\"parity\":%d,"
+               "\"split\":%d,\"scale\":\"%s\",\"act\":%d,\"adds\":[",
+               i, op.kind == G_RAWIN ? "rawin" : "norm_act", op.raw, m, repeat ? 1 : 0, l.rows ? "rows" : "grid_stride",
+               ap.raw.f32, ap.n_add, l.vecs, l.ppb, l.xt, l.grid[0], l.grid[1], l.rows && 256 % l.vecs != 0,
+               l.rows && Wpad % l.xt != 0, o.N, o.H, o.W, o.C, ap.raw.Cvalid, ap.raw.C, op.kind == G_RAWIN ? 0 : op.n_off,
+               ap.pad_mode, o.pad_t, o.pad_l, o.pad_b, o.pad_r, o.parity, o.split, scale, ap.act);
+      s += t;
+      for (int a = 0; a < ap.n_add; ++a) {
+        snprintf(t, sizeof(t), "%s{\"parity\":%d,\"split\":%d,\"C\":%d}", a ? "," : "", ap.add[a].parity, ap.add[a].split, ap.add[a].C);
+        s += t;
+      }
+      s += "]}";
+    }
+  }
+}
+
 }  // namespace v2v
 
 // =============================================================================================== C ABI
@@ -529,6 +682,7 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
     XOp m; m.kind = X_MEMSET; m.ms_ptr = base + stats_begin; m.ms_bytes = stats_end - stats_begin;
     P->xops.push_back(m);
   }
+  const std::vector<int> fin_site = finalize_sites(P);
   for (size_t i = 0; i < P->gops.size(); ++i) {
     GOp& op = P->gops[i];
     switch (op.kind) {
@@ -589,20 +743,8 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
       case G_NORM_ACT: {
         Raw& r = P->raws[op.raw];
         const GOp& cop = P->gops[r.conv_op];
-        FinalizeParams fp{};
         const bool has_norm = op.norm.kind != V2V_NORM_NONE;
-        if (has_norm) {
-          fp.stats = r.stats; fp.Cs = r.C; fp.C = op.cC; fp.c_off = op.n_off; fp.scale_stride = r.C;
-          fp.N = r.N;
-          fp.count = (double)r.H * r.W; fp.instance = (op.norm.kind == V2V_NORM_INSTANCE) || P->sample_stats;
-          fp.sample_running = P->sample_stats;
-          fp.io = P->io_dev; fp.flags_slot = P->flags_slot;
-          const int cout1 = cop.conv.Cout - cop.conv.Cout2;
-          V2V_REQUIRE(op.n_off == 0 || (cop.conv.Cout2 > 0 && op.n_off == cout1), V2V_ERR_UNSUPPORTED,
-                      "a raw slice must start at channel 0 or at the second weight set");
-          fp.gamma = op.norm.gamma; fp.beta = op.norm.beta; fp.conv_bias = op.n_off == 0 ? cop.conv.bias : cop.conv.bias2;
-          fp.momentum = op.norm.momentum; fp.eps = op.norm.eps;
-        } else if (cop.conv.bias != nullptr) {
+        if (!has_norm && cop.conv.bias != nullptr) {
           // norm-less biased conv (FlowNet2's conv / deconv / predict_flow units): the normalise pass runs with scale 1 and
           // shift = bias, written here and after every repack
           V2V_REQUIRE(op.n_off == 0 && cop.conv.Cout2 == 0, V2V_ERR_UNSUPPORTED, "biased norm-less conv cannot be sliced");
@@ -612,40 +754,19 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
         }
         const Value& vo = P->values[op.value_out];
         for (size_t m = 0; m < vo.bufs.size(); ++m) {
-          XOp a; a.kind = X_APPLY;
-          ApplyParams& ap = a.app;
-          ap.raw = r.desc;
-          ap.raw.base = reinterpret_cast<uint8_t*>(r.desc.base) + (size_t)op.n_off * r.desc.elem_bytes();
-          ap.raw.Cvalid = op.cC;                                               // channel slice, full row stride
-          ap.scale = (has_norm || cop.conv.bias != nullptr) ? r.scale + op.n_off : nullptr;
-          ap.shift = r.shift + op.n_off;
-          ap.scale_stride = r.C;
-          ap.act = op.act; ap.slope = op.slope;
-          ap.n_add = 0;
-          for (int k = 0; k < 2; ++k) if (op.add[k] >= 0) ap.add[ap.n_add++] = P->acts[P->values[op.add[k]].bufs[0]];
-          ap.out = P->acts[vo.bufs[m]]; ap.pad_mode = P->act_pad_mode[vo.bufs[m]];
-          if (has_norm) {
-            // Train-mode side effects (running statistics; the scale / shift / mean / rstd arrays the backward and the
-            // grid-stride fallback read) happen ONCE per (raw, slice), however many normalise passes read it (two output
-            // layouts; defer_last emits the same slice twice).
-            const bool first = std::find(r.running_done.begin(), r.running_done.end(), op.n_off) == r.running_done.end();
-            FinalizeParams side = fp;
-            side.running_mean = op.norm.running_mean; side.running_var = op.norm.running_var;
-            side.num_batches_tracked = reinterpret_cast<long long*>(op.norm.num_batches_tracked);
-            side.scale = r.scale; side.shift = r.shift; side.mean_out = r.mean; side.rstd_out = r.rstd;
-            if (first) {
-              // scale / shift come from the tail of the producing tensor-core launch (last-CTA finalisation, conv_umma.cu); the
-              // SIMT cross-check implementation and a third slice of one raw use a stats_finalize launch instead
+          if (m == 0 && fin_site[i] >= 0) {
+            FinalizeParams side{};
+            rc = finalize_params(P, op, side); if (rc) return rc;
+            if (fin_site[i] < 2) {
               GOp& prod = P->gops[r.conv_op];
-              if (P->impl == V2V_IMPL_UMMA && prod.kp.n_fin < 2) {
-                prod.kp.fin[prod.kp.n_fin++] = side;
-                prod.kp.fin_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<uint8_t*>(r.stats) + (size_t)r.N * 2 * r.C * sizeof(stat_t));
-              } else {
-                XOp f; f.kind = X_FINALIZE; f.fin = side; P->xops.push_back(f);
-              }
-              r.running_done.push_back(op.n_off);
+              prod.kp.fin[fin_site[i]] = side;
+              prod.kp.n_fin = fin_site[i] + 1;
+              prod.kp.fin_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<uint8_t*>(r.stats) + (size_t)r.N * 2 * r.C * sizeof(stat_t));
+            } else {
+              XOp f; f.kind = X_FINALIZE; f.fin = side; P->xops.push_back(f);
             }
           }
+          XOp a; a.kind = X_APPLY; a.app = apply_params(P, op, m);
           P->xops.push_back(a);
         }
         break;
@@ -653,12 +774,7 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
       case G_RAWIN: {
         const Value& vo = P->values[op.value_out];
         for (size_t m = 0; m < vo.bufs.size(); ++m) {
-          XOp a; a.kind = X_APPLY;
-          ApplyParams& ap = a.app;
-          ap.raw.base = const_cast<float*>(op.ext_raw); ap.raw.N = vo.N; ap.raw.H = vo.H; ap.raw.W = vo.W; ap.raw.C = op.ext_C;
-          ap.raw.Cvalid = vo.C; ap.raw.f32 = 1;
-          ap.scale = nullptr; ap.shift = nullptr; ap.scale_stride = 0; ap.act = ACT_NONE; ap.slope = 0.f; ap.n_add = 0;
-          ap.out = P->acts[vo.bufs[m]]; ap.pad_mode = P->act_pad_mode[vo.bufs[m]];
+          XOp a; a.kind = X_APPLY; a.app = apply_params(P, op, m);
           P->xops.push_back(a);
         }
         break;
@@ -902,6 +1018,9 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
     if (!P->sized && size_arena(P)) return -1;        // the raw tensors' element type and channel stride (host-only)
     describe_epilogue_backward(P, s);
   }
+  s += "],\"epilogue_forward\":[";
+  if (!P->sized && size_arena(P)) return -1;          // the raw tensors' element type and channel stride (host-only)
+  describe_epilogue_forward(P, s);
   // ops the backward visits (0 for the forward-only branch of a feature L1 target) and values without a gradient buffer
   int bwd_ops = 0, detached = 0;
   for (char l : P->op_live) bwd_ops += l;

@@ -73,7 +73,6 @@ struct Raw {
   RawDesc desc{};
   stat_t* stats = nullptr;           // [N][2][C] fixed-point statistics rows (zeroed at the start of every run)
   float* scale = nullptr; float* shift = nullptr;
-  std::vector<int> running_done;   // channel offsets whose running stats already have an updating launch
   float* mean = nullptr; float* rstd = nullptr;   // training plans: saved statistics [N][C]
   float* graw = nullptr;           // training plans: gradient of the raw tensor, dense NHWC fp32 (channel stride desc.C)
   bool no_stats = false;           // backward sub-plans: the conv output feeds no norm layer
@@ -214,6 +213,9 @@ int new_value(v2v_plan* p, int N, int H, int W, int C);
 int size_arena(v2v_plan* P);
 int run_xop(v2v_plan* P, const XOp& x, cudaStream_t s);
 FeatL1Params featl1_params(const v2v_plan* P, const GOp& op);
+std::vector<int> finalize_sites(const v2v_plan* P);
+ApplyParams apply_params(const v2v_plan* P, const GOp& op, size_t m);
+void describe_epilogue_forward(v2v_plan* P, std::string& s);
 
 // plan_backward.cu
 int alloc_training(v2v_plan* P, cudaStream_t stream);

@@ -279,7 +279,14 @@ __device__ __forceinline__ void split_bf16(float x, bf16& hi, bf16& lo) {
 }
 cudaError_t launch_stats_finalize(const FinalizeParams& p, cudaStream_t stream);
 cudaError_t launch_norm_apply(const ApplyParams& p, cudaStream_t stream);
-bool norm_apply_uses_rows(const ApplyParams& p);
+// Launch shape of launch_norm_apply, chosen on the host from the output layout alone.
+struct NormApplyLaunch {
+  int rows;                    // 1: norm_apply_rows_kernel, one block per (padded row, segment of xt pixels); 0: grid-stride kernel
+  int vecs;                    // 8-channel vectors per output pixel (rows kernel: thread t keeps vector t % vecs)
+  int ppb, xt;                 // rows kernel: pixels per block pass (256 / vecs), pixels per block (8 ppb)
+  int grid[2];                 // rows kernel: segments x (N * padded rows); grid-stride kernel: blocks x 1
+};
+NormApplyLaunch norm_apply_launch(const ApplyParams& p);
 cudaError_t launch_import_nchw(const ImportParams& p, cudaStream_t stream);
 cudaError_t launch_export_nchw(const ExportParams& p, cudaStream_t stream);
 cudaError_t launch_pack_weights(const PackParams& p, cudaStream_t stream);
