@@ -5,36 +5,14 @@ padded channels [Cin, Cp) are zero).  BNt: MMA width of the last N tile, its val
 the kernel has an instantiation of that width.  The 7x7 stems over the 108-channel label input (3 frames x 35 one-hot
 labels + 1 edge channel, padded to 128) are the layers these matter for."""
 import pytest
-import torch
 
-import bench
-from vid2vid_b200 import networks as NW
-from vid2vid_b200.plan import Plan
-
-H100_SXM_SMS = 132
-
-
-@pytest.fixture(autouse=True)
-def _h100_sxm():
-    if torch.cuda.is_available() and torch.cuda.get_device_properties(0).multi_processor_count != H100_SXM_SMS:
-        pytest.skip('the tilings below are those of a %d-SM H100 SXM' % H100_SXM_SMS)
+import product_plans as PP
+from product_plans import h100_sxm  # noqa: F401  (autouse: the tilings below are those of a 132-SM H100 SXM)
 
 
 def _cfg4_convs(mode):
-    """{scale: describe() convs} of the cfg4 generators; the finest scale reads the exact one-hot + edge input, as
-    Vid2VidModelG sets it."""
-    W = bench.WORKLOADS['cfg4']
-    opt = bench.make_opt_for('cfg4')
-    opt.gpu_ids = []
-    out = {}
-    for s in range(W['n_scales']):
-        sc = 2 ** (W['n_scales'] - 1 - s)
-        net = NW.build_netG(opt, s)
-        net.input_exact_bf16 = s == W['n_scales'] - 1
-        p = Plan(0, precision=mode)
-        net._describe(p, 1, W['H'] // sc, W['W'] // sc)
-        out[s] = p.describe()['convs']
-    return out
+    """[describe() convs of scale s] of the cfg4 generators, as bench.py lowers them."""
+    return [PP.describe(s)['convs'] for s in PP.group('bench') if s.tag.startswith('cfg4 ') and s.precision == mode]
 
 
 # mode, scale, Cout -> (BN, BNt, kc, kmma, kmma_last)
@@ -63,7 +41,7 @@ def test_cfg4_stems_issue_only_valid_columns_and_k_steps(mode):
 @pytest.mark.parametrize('mode', ['fast', 'precise'])
 def test_unpadded_convs_keep_full_widths(mode):
     n = 0
-    for convs in _cfg4_convs(mode).values():
+    for convs in _cfg4_convs(mode):
         for c in convs:
             if c['Cin'] % 16 == 0 and c['Cin'] == c['Cp'] and c['Cout'] % c['BN'] == 0:
                 assert c['kmma_last'] == c['kmma'] and c['BNt'] == c['BN'], c

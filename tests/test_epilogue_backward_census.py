@@ -8,12 +8,9 @@ assuming the H100 SXM's 132 SMs.  Each record is reduced to the fields that sele
 import collections
 import functools
 
-import pytest
-
+import census as C
 import product_plans as PP
-import test_backward_variant_census as BC
-from test_conv_variant_census import _h100_sxm  # noqa: F401  (autouse: the census describes a 132-SM device)
-from vid2vid_b200.plan import Plan
+from product_plans import h100_sxm  # noqa: F401  (autouse: the census describes a 132-SM device)
 
 NormKey = collections.namedtuple('NormKey', 'reduce ppb1 multi_block ragged c_off adds act twice raw_f32 batch_stats multi_image')
 BiasKey = collections.namedtuple('BiasKey', 'kind acts split multi_block')
@@ -37,32 +34,21 @@ def keys_of(d):
     return out
 
 
-def _describe(describe, precision='precise'):
-    p = Plan(0, precision=precision, train=True)
-    describe(p)
-    return p.describe()
-
-
 @functools.lru_cache(maxsize=None)
 def product_keys():
     """{key: where} over cfg3's training step (generator scales, D and D_T towers, as bench.py runs it) and the pose step with
-    the face discriminator (tests/product_plans.pose_step)."""
-    found = collections.OrderedDict()
-    for tag, describe in BC._benchmark_describes() + PP.pose_step():
-        for k, r in keys_of(_describe(describe)).items():
-            found.setdefault(k, '%s: %s %d ch @ %dx%d' % (tag, r['kind'], r['C'], r['H'], r['W']))
-    return found
+    the face discriminator: the training plans of the inventory's bench and pose_step groups."""
+    return C.first_where((k, '%s: %s %d ch @ %dx%d' % (s.tag, r['kind'], r['C'], r['H'], r['W']))
+                         for s in PP.group('bench', 'pose_step') if s.train for k, r in keys_of(PP.describe(s)).items())
 
 
 @functools.lru_cache(maxsize=None)
 def case_keys():
     """{case id: keys} over the GPU cases, described from the same builders the GPU test runs (modules on the CPU)."""
     import test_gpu_epilogue_backward as EB
-    out = collections.OrderedDict()
-    for name, spec in EB.CASES:
-        d = _describe(lambda p: EB.build(p, spec, 'cpu'), EB.precision(spec))
-        out[name] = set(keys_of(d))
-    return out
+    return {name: set(keys_of(PP.describe(PP.PlanSpec('case', name, functools.partial(EB.build, spec=spec, device='cpu'),
+                                                      EB.precision(spec), True))))
+            for name, spec in EB.CASES}
 
 
 # The launch paths GPU cases run although no product plan reaches them, each with the reason.  They are listed key by key, so
@@ -79,30 +65,18 @@ UNREACHED = {
 
 
 def test_every_product_epilogue_key_has_a_gpu_case():
-    reached = set().union(*case_keys().values())
-    missing = [(k, where) for k, where in product_keys().items() if k not in reached]
-    print('%d epilogue backward keys in the products, %d reached by a GPU case' % (len(product_keys()), len(product_keys()) - len(missing)))
-    assert not missing, '%d epilogue backward launch paths of the products are reached by no GPU case:\n%s' % (
-        len(missing), '\n'.join('  %s  e.g. %s' % (tuple(k), where) for k, where in missing))
+    C.assert_reached('epilogue backward launch paths of the products', product_keys(), case_keys())
 
 
 def test_unreached_keys_are_listed():
     """Every listed path is run by a GPU case and reached by no product; every case key is a product key or listed."""
-    prod = set(product_keys())
-    reached = set().union(*case_keys().values())
-    assert not set(UNREACHED) & prod, sorted(set(UNREACHED) & prod)
-    assert set(UNREACHED) <= reached, sorted(set(UNREACHED) - reached)
-    unlisted = sorted((name, tuple(k)) for name, ks in case_keys().items() for k in ks - prod - set(UNREACHED))
-    assert not unlisted, 'case keys no product reaches and UNREACHED does not list: %s' % unlisted
+    C.assert_unreached_listed(product_keys(), case_keys(), UNREACHED)
 
 
 def test_every_gpu_case_is_needed():
     """Each case reaches a key no other case reaches: a product key or a listed unreached one."""
-    wanted = set(product_keys()) | set(UNREACHED)
-    cases = case_keys()
-    for name, keys in cases.items():
-        others = set().union(*(k for n, k in cases.items() if n != name))
-        assert (keys & wanted) - others, '%s reaches no key of its own: %s' % (name, sorted(keys))
+    import test_gpu_epilogue_backward as EB
+    C.assert_needed([name for name, _ in EB.CASES], [({**product_keys(), **UNREACHED}, case_keys())])
 
 
 def test_census_is_not_vacuous():
@@ -112,17 +86,3 @@ def test_census_is_not_vacuous():
     assert any(k.ppb1 for k in norm) and any(k.ragged for k in norm) and any(k.c_off for k in norm) and any(k.twice for k in norm)
     assert {k.adds for k in norm} == {0, 1, 2} and {k.act for k in norm} == {0, 1, 2}
 
-
-def main():
-    cases = case_keys()
-    keys = product_keys()
-    print('product epilogue backward keys: %d' % len(keys))
-    for k, where in keys.items():
-        by = [n for n, ks in cases.items() if k in ks]
-        print('  %s\n      %s\n      reached by: %s' % (tuple(k), where, by[0] if by else 'NONE'))
-    for name, ks in cases.items():
-        print('%s: %s' % (name, [tuple(k) for k in ks - set(keys)]))
-
-
-if __name__ == '__main__':
-    main()

@@ -1,4 +1,4 @@
-"""GPU parity of the tensor-core backward at the configurations cfg3's training step runs (tests/test_backward_variant_census.py
+"""GPU parity of the tensor-core backward at the configurations cfg3's training step runs (tests/test_conv_census.py
 fails when one of them is reached by no case).  Each case mirrors benchmark layers -- channels, kernel, stride, padding and
 grid -- as smooth units (conv, conv + BatchNorm, transposed conv + BatchNorm, the tanh image head; no ReLU / LeakyReLU), so no
 activation gate can flip between our forward and the reference's, and the gradients are compared with PyTorch autograd in

@@ -166,7 +166,7 @@ def test_head(name, build, head, scale, shape, mode):
 
 # Kernel configurations that the benchmark's plans lower (cfg4 / cfg2 / cfg3 generators, the cfg3 image and temporal
 # discriminators, FlowNet2) and the cases above do not reach, each at the smallest shape that selects it on 132 SMs.
-# tests/test_conv_variant_census.py fails when one of them goes missing or stops being needed.
+# tests/test_conv_census.py fails when one of them goes missing or stops being needed.
 # name, layer list builder, input shape, modes, input = one-hot labels + 0/1 edges declared exact in bf16 (_label_x)
 # FlowNet2's units are conv + bias + LeakyReLU(0.1) lowered as a conv with the raw + statistics epilogue (bias-free) and a
 # normalise pass that adds the bias (plan.cu, G_NORM_ACT without a norm).  A batch norm in its place gives the conv kernel the

@@ -78,7 +78,7 @@ def test_per_sample_forward_equals_batch1_forwards(case, mode):
 # Kernel configurations that the plans of tools/time_multiclip.py lower and no other GPU parity case reaches, each at a small
 # shape that selects it on 132 SMs, run as a per-sample plan over N images and checked against the same layers evaluated
 # image by image in fp64 (precise) or bf16-emulated fp32 (fast) at tests/test_gpu_conv.py's tolerances.
-# tests/test_multiclip_census.py fails when a configuration goes uncovered or a case stops being needed.
+# tests/test_conv_census.py fails when a configuration goes uncovered or a case stops being needed.
 # name, layer list builder, input shape (N, C, H, W), modes
 BN = NW.get_norm_layer('batch')
 CONV_CASES = [

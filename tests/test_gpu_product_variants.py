@@ -1,5 +1,5 @@
 """GPU parity of the conv kernel configurations that product paths outside bench.py run and no other parity case reaches
-(tests/product_plans.py lists the plans; tests/test_product_census.py fails when one of their configurations goes uncovered or
+(tests/product_plans.py lists the plans; tests/test_conv_census.py fails when one of their configurations goes uncovered or
 a case here stops being needed): the face first frame's Encoder and Global_with_z, the pose training step with the face
 discriminator (generator scales, netD / netD_f / netD_T towers), and the VGG19 loss.
 

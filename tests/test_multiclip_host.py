@@ -1,22 +1,16 @@
 """Host-side checks of per-sample-statistics plans (v2v_plan_set_sample_stats), no GPU needed: the switch is refused on
 training plans, and a per-sample plan of B clips lowers every conv with the kernel configuration of the batch-1 plan (that
 configuration fixes each pixel's accumulation order, which is what keeps every clip bit-identical to its own run)."""
-import os
-import sys
-
 import pytest
 
 import bench
+import product_plans as PP
 from vid2vid_b200 import _lib as L
 from vid2vid_b200 import networks as NW
 from vid2vid_b200.plan import Plan
-from vid2vid_b200.utils import make_opt
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), '..', 'tools'))
-import time_multiclip as TM     # noqa: E402
 
 # the launch quantities that scale with the number of images, and the epilogue placement chosen from them (the epilogue
-# only stores results: it does not change any sum; tests/test_multiclip_census.py keys configurations by it)
+# only stores results: it does not change any sum; tests/test_conv_census.py keys configurations by it)
 PER_LAUNCH = ('units', 'm_total', 'ctas', 'async_epi')
 
 
@@ -42,25 +36,16 @@ def test_sample_stats_module_refuses_autograd():
 
 
 def _convs(net, N, H, W, mode, sample_stats):
-    p = Plan(0, precision=mode, sample_stats=sample_stats)
-    net._describe(p, N, H, W)
-    d = p.describe()
+    d = PP.describe(PP.PlanSpec('multiclip', 'B=%d' % N, lambda p: net._describe(p, N, H, W), mode, sample_stats=sample_stats))
     assert d['sample_stats'] == int(sample_stats)
     return d['convs']
 
 
 @pytest.mark.parametrize('mode', ['precise', 'fast'])
-@pytest.mark.parametrize('wl', list(TM.WORKLOADS))
+@pytest.mark.parametrize('wl', list(PP.TM.WORKLOADS))
 def test_per_sample_plan_keeps_the_batch1_configuration(wl, mode):
-    W = TM.WORKLOADS[wl]
-    o = dict(W['opt'])
-    opt = make_opt(gpu_ids=[], synthetic_weights=True, **o)
-    S = opt.n_scales_spatial
-    for s in range(S):
-        sc = 2 ** (S - 1 - s)
-        net = NW.build_netG(opt, s)
-        net.input_exact_bf16 = s == S - 1 and opt.label_nc != 0
-        h, w = W['H'] // sc, W['W'] // sc
+    W = PP.TM.WORKLOADS[wl]
+    for net, h, w in PP.scales(PP.clip_opt(W), W['H'], W['W']):
         one = _convs(net, 1, h, w, mode, False)
         four = _convs(net, 4, h, w, mode, True)
         assert len(one) == len(four)

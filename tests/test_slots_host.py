@@ -1,22 +1,18 @@
 """Host-side checks of slot streams (Vid2VidModelG.stream_slots), no GPU needed: the slot bookkeeping over a scripted
 schedule, the argument errors, the refusals of v2v_plan_set_image_flags, and that a slot plan (a per-sample plan reading
 per-image flags) lowers every conv exactly as the per-sample plan of the same shape does -- the configuration fixes each
-pixel's accumulation order, and tests/test_multiclip_census.py covers every per-sample configuration."""
+pixel's accumulation order, and tests/test_conv_census.py covers every per-sample configuration."""
 import ctypes as C
-import os
-import sys
 import types
 
 import pytest
 
+import product_plans as PP
 from vid2vid_b200 import _lib as L
 from vid2vid_b200 import networks as NW
 from vid2vid_b200.model_g import SlotSchedule, SlotStream
 from vid2vid_b200.plan import Plan
 from vid2vid_b200.utils import make_opt
-
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), '..', 'tools'))
-import time_slots as TS     # noqa: E402
 
 K, P, R, X = L.SLOT_KEEP, L.SLOT_PUSH, L.SLOT_RESTART, L.SLOT_CLEAR
 
@@ -126,25 +122,16 @@ def test_image_flags_are_refused_on_training_and_batch_statistics_plans():
 
 
 def _describe(net, B, h, w, mode, flags):
-    p = Plan(0, precision=mode, sample_stats=True)
-    if flags:
-        p.set_image_flags(NW.S_FLAGS)
-    net._describe(p, B, h, w)
-    d = p.describe()
+    d = PP.describe(PP.PlanSpec('slots', 'B=%d' % B, lambda p: net._describe(p, B, h, w), mode, sample_stats=True, flags=flags))
     assert d['image_flags'] == int(flags) and d['sample_stats'] == 1
     return d
 
 
 @pytest.mark.parametrize('mode', ['precise', 'fast'])
-@pytest.mark.parametrize('wl', list(TS.WORKLOADS))
+@pytest.mark.parametrize('wl', list(PP.TS.WORKLOADS))
 def test_slot_plans_lower_as_per_sample_plans(wl, mode):
-    w = TS.WORKLOADS[wl]
-    opt = make_opt(gpu_ids=[], synthetic_weights=True, **w['opt'])
-    S = opt.n_scales_spatial
-    for s in range(S):
-        net = NW.build_netG(opt, s)
-        net.input_exact_bf16 = s == S - 1 and opt.label_nc != 0      # as Vid2VidModelG.initialize sets it
-        h, w_ = w['H'] // 2 ** (S - 1 - s), w['W'] // 2 ** (S - 1 - s)
+    w = PP.TS.WORKLOADS[wl]
+    for s, (net, h, w_) in enumerate(PP.scales(PP.clip_opt(w), w['H'], w['W'])):
         for B in w['bs']:
             slot, ref = _describe(net, B, h, w_, mode, True), _describe(net, B, h, w_, mode, False)
             assert slot['convs'] == ref['convs'], (wl, mode, s, B)

@@ -16,9 +16,8 @@ opt.gpu_ids = []
 for mode in ('fast', 'precise'):
     print(mode)
     seen = set()
-    for s in range(W['n_scales']):
+    for s, net in enumerate(NW.build_netGs(opt)):
         sc = 2 ** (W['n_scales'] - 1 - s)
-        net = NW.build_netG(opt, s)
         plan = Plan(0, precision=mode)
         net._describe(plan, 1, W['H'] // sc, W['W'] // sc)
         for c in plan.describe()['convs']:

@@ -43,11 +43,8 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
             opt.no_flow = True
         dev = torch.device('cuda', self.gpu_ids[0] if len(self.gpu_ids) else torch.cuda.current_device())
         self.device_ = dev
-        for s in range(self.n_scales):
-            setattr(self, 'netG' + str(s), networks.build_netG(opt, s).to(dev))
-        # the finest scale reads encode_input's one-hot + edge map at full resolution: exact in bf16 (coarser pyramid levels
-        # are avg-pooled, pose inputs are real-valued: not exact)
-        getattr(self, 'netG' + str(self.n_scales - 1)).input_exact_bf16 = bool(opt.label_nc != 0)
+        for s, net in enumerate(networks.build_netGs(opt)):
+            setattr(self, 'netG' + str(s), net.to(dev))
         # vid2vid_model_G.py:46-51: checkpoints are loaded whenever not training (or continuing / pre-training); a missing G0
         # is an error there (base_model.py:63-72).  opt.synthetic_weights (benchmarks / tests, no checkpoints offline) skips it.
         if (not self.isTrain or getattr(opt, 'continue_train', False) or getattr(opt, 'load_pretrain', '')) and \

@@ -968,6 +968,15 @@ def build_netG(opt, s):
                     opt.n_downsample_G, opt.norm, s, [], opt)
 
 
+def build_netGs(opt):
+    """[netG0, ..., netG{n_scales_spatial - 1}] as Vid2VidModelG.initialize builds them.  The finest scale reads
+    encode_input's one-hot + edge map at full resolution, which is exact in bf16 (coarser pyramid levels are avg-pooled, pose
+    inputs are real-valued: not exact)."""
+    nets = [build_netG(opt, s) for s in range(opt.n_scales_spatial)]
+    nets[-1].input_exact_bf16 = opt.label_nc != 0
+    return nets
+
+
 class SequentialRunner(_Planned):
     """Runs a list of supported layer containers (conv / norm / activation units, ResnetBlocks, transposed
     convs; optionally a trailing small-Cout head) through the plan runtime: fp32 NCHW in -> fp32 NCHW out.
