@@ -149,7 +149,12 @@ int v2v_face_region(const float* real_A, int N, int C, int H, int W, int openpos
  *     For each label present, feat_ori = pooled at its first pixel in flat (n, y, x) order; dists[m] = sum over present
  *     labels and k of (feat_ori - table[label][m][k])^2 for m < num_images (absent labels contribute nothing); *chosen
  *     (device int32) = the first minimum; out[n,k,p] = table[inst][min(chosen, rows[inst] - 1)][k].  A present label with
- *     fewer than num_images rows is V2V_ERR_INVALID.  n_labels <= V2V_FACE_MAX_LABELS, feat_num <= V2V_FACE_MAX_FEAT. */
+ *     fewer than num_images rows is V2V_ERR_INVALID.  n_labels <= V2V_FACE_MAX_LABELS, feat_num <= V2V_FACE_MAX_FEAT.
+ *   face_features_per_image: the same lookup for N independent images (one clip each), in one launch sequence: image n's
+ *     search runs over the labels present in image n only, from their first pixels in image n, and chosen (device int32,
+ *     N entries) gets its own first minimum; out[n] is painted from chosen[n].  An invalid id in image n (or a present label
+ *     with too few rows) makes the call V2V_ERR_INVALID; under graph capture that image gets chosen[n] = -1 and a NaN map.
+ *     At N = 1 it equals face_features bit for bit. */
 #define V2V_MAX_INSTANCE_IDS 256
 #define V2V_FACE_MAX_LABELS 32
 #define V2V_FACE_MAX_FEAT 64
@@ -157,6 +162,9 @@ int v2v_instance_mean(const float* x, const float* inst, float* out, int N, int 
 int v2v_face_features(const float* pooled, const float* inst, const float* table, const int* rows, int n_labels, int max_rows,
                       int num_images, int feat_num, int table_stride, float* out, int* chosen, int N, int H, int W,
                       v2v_stream_t stream);
+int v2v_face_features_per_image(const float* pooled, const float* inst, const float* table, const int* rows, int n_labels,
+                                int max_rows, int num_images, int feat_num, int table_stride, float* out, int* chosen, int N, int H,
+                                int W, v2v_stream_t stream);
 
 /* FlowNet2 glue (models/flownet2_pytorch/models.py:97-160, models/flownet.py:43-58), fp32 NCHW.
  * flownet_prep: the image pair -> x (B,6,H,W) = (pair - mean over both frames and all pixels, per sample and colour) / rgb_max,

@@ -45,7 +45,7 @@ SYMBOLS = [
     'v2v_correlation_out_shape', 'v2v_correlation_forward', 'v2v_resample2d_forward', 'v2v_channelnorm_forward',
     'v2v_resample_forward', 'v2v_onehot_edges', 'v2v_avgpool3s2', 'v2v_fg_mask',
     'v2v_l1_loss_forward', 'v2v_l1_loss_backward', 'v2v_mse_const_forward', 'v2v_mse_const_backward', 'v2v_avgpool3s2_backward',
-    'v2v_resample_backward', 'v2v_avgpool2', 'v2v_avgpool2_backward', 'v2v_face_region', 'v2v_instance_mean', 'v2v_face_features', 'v2v_ids_window_push', 'v2v_slots_window_push', 'v2v_tensor2im_u8', 'v2v_flownet_prep', 'v2v_resize', 'v2v_sub_channels', 'v2v_flow_conf',
+    'v2v_resample_backward', 'v2v_avgpool2', 'v2v_avgpool2_backward', 'v2v_face_region', 'v2v_instance_mean', 'v2v_face_features', 'v2v_face_features_per_image', 'v2v_ids_window_push', 'v2v_slots_window_push', 'v2v_tensor2im_u8', 'v2v_flownet_prep', 'v2v_resize', 'v2v_sub_channels', 'v2v_flow_conf',
     'v2v_plan_create', 'v2v_plan_destroy', 'v2v_plan_set_precision', 'v2v_g_input', 'v2v_g_input_ex', 'v2v_g_conv', 'v2v_g_norm_act', 'v2v_g_norm_act_slice', 'v2v_g_conv_act',
     'v2v_g_head', 'v2v_g_concat', 'v2v_g_correlation', 'v2v_g_maxpool2', 'v2v_g_feature_l1', 'v2v_g_export', 'v2v_g_composite', 'v2v_g_composite_ex', 'v2v_plan_set_training', 'v2v_plan_set_sample_stats', 'v2v_plan_set_image_flags', 'v2v_plan_backward', 'v2v_plan_finalize', 'v2v_plan_finalize_ws', 'v2v_plan_repack', 'v2v_plan_run',
     'v2v_plan_profile', 'v2v_plan_num_kernels', 'v2v_plan_conv_macs', 'v2v_plan_workspace_bytes', 'v2v_plan_describe',
@@ -118,6 +118,7 @@ def lib():
     l.v2v_face_region.argtypes = [fp] + [C.c_int] * 5 + [vp, vp]
     l.v2v_instance_mean.argtypes = [fp, fp, fp] + [C.c_int] * 5 + [vp]
     l.v2v_face_features.argtypes = [fp, fp, fp, ip] + [C.c_int] * 5 + [fp, vp] + [C.c_int] * 3 + [vp]
+    l.v2v_face_features_per_image.argtypes = l.v2v_face_features.argtypes
     l.v2v_resample_backward.argtypes = [fp, fp, fp, fp, fp] + [C.c_int] * 5 + [vp]
     l.v2v_ids_window_push.argtypes = [fp, vp] + [C.c_int] * 5 + [vp]
     l.v2v_slots_window_push.argtypes = [fp, vp] + [C.c_int] * 6 + [ip, vp]

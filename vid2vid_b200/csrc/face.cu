@@ -7,7 +7,8 @@
 //   face_features   get_face_features (models/vid2vid_model_G.py:290-320) + dists_min (models/base_model.py:136-144): the
 //                   pooled feature at the first pixel of each label present (integer atomicMin of the flat (n, y, x)
 //                   index), squared distances to the rows of the packed features table in double, the first minimum, and
-//                   the chosen rows painted over the part map.
+//                   the chosen rows painted over the part map.  The search runs once per group of images: the whole batch
+//                   (the reference's get_face_features) or each image on its own (B independent clips, one block each).
 #include <climits>
 
 #include "../../include/v2v_b200.h"
@@ -95,33 +96,37 @@ struct FaceFeatParams {
   const float* inst;       // (N, 1, H, W) label ids
   const float* table;      // (n_labels, max_rows, stride)
   float* out;              // (N, feat_num, H, W)
-  int* chosen;             // device int32
-  int* first;              // scratch [FACE_MAX_LABELS]: first flat (n, y, x) index of each label, >= N * H * W = absent
+  int* chosen;             // device int32 [groups]
+  int* first;              // scratch [groups][FACE_MAX_LABELS]: first flat (n, y, x) index of each label, >= N * H * W = absent
+  int* bad;                // scratch [groups]: the group's part map holds an invalid id
   int* err;
   int rows[FACE_MAX_LABELS];
   int n_labels, max_rows, num_images, feat_num, stride, N, H, W;
+  int per_image;           // 0: one group (the whole batch); 1: one group per image
+  __device__ int group_of(int n) const { return per_image ? n : 0; }
 };
 
 __global__ void __launch_bounds__(256) face_first_index_kernel(FaceFeatParams p) {
   const int total = p.N * p.H * p.W;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const float id = __ldg(p.inst + i);
-    if (!valid_id(id, p.n_labels)) { atomicOr(p.err, FACE_ERR_ID); continue; }
-    atomicMin(p.first + (int)id, i);
+    const int g = p.group_of(i / (p.H * p.W));
+    if (!valid_id(id, p.n_labels)) { atomicOr(p.err, FACE_ERR_ID); atomicOr(p.bad + g, 1); continue; }
+    atomicMin(p.first + g * FACE_MAX_LABELS + (int)id, i);
   }
 }
 
-// One block.  dists[m] = sum_k sum_label (feat_ori[label][k] - table[label][m][k])^2 over the labels present, in double, in
+// One block per group.  dists[m] = sum_k sum_label (feat_ori[label][k] - table[label][m][k])^2 over the labels present, in double, in
 // the reference's order (labels first, then k); the first minimum over m < num_images wins.
 __global__ void __launch_bounds__(256) face_choose_kernel(FaceFeatParams p) {
   __shared__ float s_ori[FACE_MAX_LABELS][FACE_MAX_FEAT];
   __shared__ int s_present[FACE_MAX_LABELS];
   __shared__ double s_d[256];
   __shared__ int s_m[256];
-  const int HW = p.H * p.W;
+  const int HW = p.H * p.W, g = blockIdx.x;
   bool bad = false;
   for (int l = 0; l < p.n_labels; ++l) {
-    const int f = p.first[l];
+    const int f = p.first[g * FACE_MAX_LABELS + l];
     const bool present = f < p.N * HW;
     if (threadIdx.x == 0) s_present[l] = present;
     if (present && p.rows[l] < p.num_images) bad = true;
@@ -130,8 +135,8 @@ __global__ void __launch_bounds__(256) face_choose_kernel(FaceFeatParams p) {
       for (int k = threadIdx.x; k < p.feat_num; k += blockDim.x) s_ori[l][k] = p.pooled[((size_t)n * p.feat_num + k) * HW + px];
     }
   }
-  if (bad || (*p.err & FACE_ERR_ID)) {
-    if (threadIdx.x == 0) { if (bad) atomicOr(p.err, FACE_ERR_ROWS); *p.chosen = -1; }
+  if (bad || p.bad[g]) {
+    if (threadIdx.x == 0) { if (bad) atomicOr(p.err, FACE_ERR_ROWS); p.chosen[g] = -1; }
     return;
   }
   __syncthreads();
@@ -160,19 +165,20 @@ __global__ void __launch_bounds__(256) face_choose_kernel(FaceFeatParams p) {
     }
     __syncthreads();
   }
-  if (threadIdx.x == 0) *p.chosen = s_m[0] == INT_MAX ? 0 : s_m[0];
+  if (threadIdx.x == 0) p.chosen[g] = s_m[0] == INT_MAX ? 0 : s_m[0];
 }
 
-// out[n, k, y, x] = table[label][min(chosen, rows[label] - 1)][k]; NaN when no index was chosen (an error was flagged)
+// out[n, k, y, x] = table[label][min(chosen, rows[label] - 1)][k] with the chosen index of image n's group; NaN when no
+// index was chosen (an error was flagged)
 __global__ void __launch_bounds__(256) face_paint_kernel(FaceFeatParams p) {
   const int HW = p.H * p.W;
   const size_t total = (size_t)p.N * p.feat_num * HW;
-  const int chosen = *p.chosen;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int px = (int)(i % HW);
     const size_t t = i / HW;
     const int k = (int)(t % p.feat_num), n = (int)(t / p.feat_num);
     const float id = __ldg(p.inst + (size_t)n * HW + px);
+    const int chosen = p.chosen[p.group_of(n)];
     float v = __int_as_float(0x7fc00000);
     if (chosen >= 0 && valid_id(id, p.n_labels)) {
       const int l = (int)id;
@@ -223,6 +229,41 @@ static cudaError_t read_flag(const int* err, cudaStream_t s, int* flag) {
   return cudaStreamSynchronize(s);
 }
 
+static int face_features(const float* pooled, const float* inst, const float* table, const int* rows, int n_labels, int max_rows,
+                         int num_images, int feat_num, int table_stride, float* out, int* chosen, int N, int H, int W, int per_image,
+                         v2v_stream_t stream) {
+  FACE_REQUIRE(pooled && inst && table && rows && out && chosen && N > 0 && H > 0 && W > 0, "face_features: null tensor or empty shape");
+  FACE_REQUIRE(n_labels >= 1 && n_labels <= V2V_FACE_MAX_LABELS && feat_num >= 1 && feat_num <= V2V_FACE_MAX_FEAT &&
+               table_stride >= feat_num && num_images >= 1 && max_rows >= num_images,
+               "face_features: bad table geometry (n_labels %d, feat_num %d, stride %d, num_images %d, max_rows %d)", n_labels,
+               feat_num, table_stride, num_images, max_rows);
+  FaceFeatParams p{};
+  for (int l = 0; l < n_labels; ++l) {
+    FACE_REQUIRE(rows[l] >= 0 && rows[l] <= max_rows, "face_features: label %d has %d rows of %d", l, rows[l], max_rows);
+    p.rows[l] = rows[l];
+  }
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  p.pooled = pooled; p.inst = inst; p.table = table; p.out = out; p.chosen = chosen;
+  p.n_labels = n_labels; p.max_rows = max_rows; p.num_images = num_images; p.feat_num = feat_num; p.stride = table_stride;
+  p.N = N; p.H = H; p.W = W; p.per_image = per_image;
+  const int groups = per_image ? N : 1;
+  Scratch sc(s);
+  FACE_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&sc.p), sizeof(int) * ((size_t)groups * (FACE_MAX_LABELS + 1) + 1), s));
+  FACE_CUDA(cudaMemsetAsync(sc.p, 0x7f, sizeof(int) * (size_t)groups * FACE_MAX_LABELS, s));   // 0x7f7f7f7f: above any flat index
+  FACE_CUDA(cudaMemsetAsync(sc.p + (size_t)groups * FACE_MAX_LABELS, 0, sizeof(int) * (groups + 1), s));
+  p.first = sc.p; p.bad = sc.p + (size_t)groups * FACE_MAX_LABELS; p.err = p.bad + groups;
+  face_first_index_kernel<<<grid_of((size_t)N * H * W), 256, 0, s>>>(p);
+  face_choose_kernel<<<groups, 256, 0, s>>>(p);
+  face_paint_kernel<<<grid_of((size_t)N * feat_num * H * W), 256, 0, s>>>(p);
+  FACE_CUDA(cudaGetLastError());
+  int flag;
+  FACE_CUDA(read_flag(p.err, s, &flag));
+  FACE_REQUIRE(!(flag & FACE_ERR_ID), "face_features: the part map holds a value that is not an integer in [0, %d)", n_labels);
+  FACE_REQUIRE(!(flag & FACE_ERR_ROWS), "face_features: a label present in the part map has fewer than num_images = %d rows",
+               num_images);
+  return 0;
+}
+
 }  // namespace v2v
 
 using namespace v2v;
@@ -247,35 +288,15 @@ int v2v_instance_mean(const float* x, const float* inst, float* out, int N, int 
 int v2v_face_features(const float* pooled, const float* inst, const float* table, const int* rows, int n_labels, int max_rows,
                       int num_images, int feat_num, int table_stride, float* out, int* chosen, int N, int H, int W,
                       v2v_stream_t stream) {
-  FACE_REQUIRE(pooled && inst && table && rows && out && chosen && N > 0 && H > 0 && W > 0, "face_features: null tensor or empty shape");
-  FACE_REQUIRE(n_labels >= 1 && n_labels <= V2V_FACE_MAX_LABELS && feat_num >= 1 && feat_num <= V2V_FACE_MAX_FEAT &&
-               table_stride >= feat_num && num_images >= 1 && max_rows >= num_images,
-               "face_features: bad table geometry (n_labels %d, feat_num %d, stride %d, num_images %d, max_rows %d)", n_labels,
-               feat_num, table_stride, num_images, max_rows);
-  FaceFeatParams p{};
-  for (int l = 0; l < n_labels; ++l) {
-    FACE_REQUIRE(rows[l] >= 0 && rows[l] <= max_rows, "face_features: label %d has %d rows of %d", l, rows[l], max_rows);
-    p.rows[l] = rows[l];
-  }
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  p.pooled = pooled; p.inst = inst; p.table = table; p.out = out; p.chosen = chosen;
-  p.n_labels = n_labels; p.max_rows = max_rows; p.num_images = num_images; p.feat_num = feat_num; p.stride = table_stride;
-  p.N = N; p.H = H; p.W = W;
-  Scratch sc(s);
-  FACE_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&sc.p), sizeof(int) * (FACE_MAX_LABELS + 1), s));
-  FACE_CUDA(cudaMemsetAsync(sc.p, 0x7f, sizeof(int) * FACE_MAX_LABELS, s));      // 0x7f7f7f7f: above any flat index
-  FACE_CUDA(cudaMemsetAsync(sc.p + FACE_MAX_LABELS, 0, sizeof(int), s));
-  p.first = sc.p; p.err = sc.p + FACE_MAX_LABELS;
-  face_first_index_kernel<<<grid_of((size_t)N * H * W), 256, 0, s>>>(p);
-  face_choose_kernel<<<1, 256, 0, s>>>(p);
-  face_paint_kernel<<<grid_of((size_t)N * feat_num * H * W), 256, 0, s>>>(p);
-  FACE_CUDA(cudaGetLastError());
-  int flag;
-  FACE_CUDA(read_flag(p.err, s, &flag));
-  FACE_REQUIRE(!(flag & FACE_ERR_ID), "face_features: the part map holds a value that is not an integer in [0, %d)", n_labels);
-  FACE_REQUIRE(!(flag & FACE_ERR_ROWS), "face_features: a label present in the part map has fewer than num_images = %d rows",
-               num_images);
-  return 0;
+  return face_features(pooled, inst, table, rows, n_labels, max_rows, num_images, feat_num, table_stride, out, chosen, N, H, W, 0,
+                       stream);
+}
+
+int v2v_face_features_per_image(const float* pooled, const float* inst, const float* table, const int* rows, int n_labels,
+                                int max_rows, int num_images, int feat_num, int table_stride, float* out, int* chosen, int N, int H,
+                                int W, v2v_stream_t stream) {
+  return face_features(pooled, inst, table, rows, n_labels, max_rows, num_images, feat_num, table_stride, out, chosen, N, H, W, 1,
+                       stream);
 }
 
 }  // extern "C"

@@ -146,7 +146,7 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         elif self.opt.use_instance:
             raise NotImplementedError('use_instance without label_nc')
         pool_map = None
-        if self.opt.dataset_mode == 'face':
+        if self.opt.dataset_mode == 'face' and inst_map is not None:
             pool_map = inst_map.to(self.device_, torch.float32)
         if real_image is not None:
             real_image = real_image.to(self.device_, torch.float32)
@@ -181,7 +181,8 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
     def _per_clip_statistics(self, on):
         """The generators' per-sample-statistics plans (b independent clips, each normalised with its own statistics) for the
         duration of one inference call: afterwards the modules build batch-statistics (and training) plans as before."""
-        nets = [getattr(self, 'netG' + str(s)) for s in range(self.n_scales)] + ([self.netG_i] if self.netG_i is not None else [])
+        nets = [getattr(self, 'netG' + str(s)) for s in range(self.n_scales)] + [
+            net for net in (self.netG_i, getattr(self, 'netE', None)) if net is not None]
         prev = [getattr(net, 'sample_stats', False) for net in nets]
         for net in nets:
             net.sample_stats = on
@@ -218,12 +219,12 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
                                       'start and advance together; call reset_stream() to restart the whole batch, or use '
                                       'stream_slots(B), whose slots start and stop independently' % (list(clips), n))
         self.fake_B_prev = None
-        self._win_A = self._win_I = None
+        self._win_A = self._win_I = self._win_B = self._win_P = None
 
     # ------------------------------------------------------------------ streaming inference (one new frame per call)
     _DT = {torch.uint8: 0, torch.int32: 1, torch.float32: 2}
 
-    def inference_stream(self, label_frame, inst_frame=None, out_u8=None):
+    def inference_stream(self, label_frame, inst_frame=None, out_u8=None, real_frame=None):
         """Same computation as inference() for a clip fed frame by frame: `label_frame` / `inst_frame` are the NEWEST
         (H, W) id maps (uint8, int32 or float32; host -- ideally pinned -- or device).  The tG-frame id window that
         test.py:31-41 re-sends every step stays resident on the device, so a step uploads one frame.  The first tG - 1
@@ -231,41 +232,50 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         (a (H, W, 3) uint8 tensor, host or device) is given, util.tensor2im's uint8 image written into it
         (computed on the device; util/util.py:48-71 does it on the CPU after copying the float frame back).
         B clips at once: (B, H, W) id maps, frames (B, 3, H, W), out_u8 (B, H, W, 3); every step is one launch per helper
-        for all clips, and every call of one stream must feed the same B."""
+        for all clips, and every call of one stream must feed the same B.
+
+        With label_nc 0 (the pose and face demos) `label_frame` is the newest dense frame, (input_nc, H, W) or
+        (B, input_nc, H, W) float32, pushed into a resident (B, tG, input_nc, H, W) window.  Face streams (dataset_mode face
+        with use_single_G) also take, on each of the first tG - 1 calls, the real frame `real_frame` ((B,) 3, H, W) and the
+        part map `inst_frame` ((B,) H, W ids): the first frames are generated from them as inference() generates them from
+        real_B[:, :tG - 1] and the part maps; later calls ignore both."""
         import ctypes as C
         from . import _lib as L
-        if self.opt.dataset_mode == 'face' and self.use_single_G:
-            raise ValueError('inference_stream does not take the real frames that the face first-frame generator needs '
-                             '(use_single_G with dataset_mode face): use inference()')
-        tG = self.opt.n_frames_G
-        H, W = label_frame.shape[-2:]
-        B = label_frame.shape[0] if label_frame.dim() == 3 else 1
-        if inst_frame is not None and tuple(inst_frame.shape) != tuple(label_frame.shape):
-            raise ValueError('inst_frame %s does not match label_frame %s' % (tuple(inst_frame.shape), tuple(label_frame.shape)))
-        dev = self.device_
-        if getattr(self, '_win_A', None) is not None and self._win_A.shape[0] != B:
-            raise ValueError('this stream was started with %d clip(s) and is fed %d: clips of one stream start and advance '
-                             'together (reset_stream() starts a new one)' % (self._win_A.shape[0], B))
-        if getattr(self, '_win_A', None) is None or self._win_A.shape[-2:] != (H, W):
-            self._win_A = torch.zeros(B, tG, 1, H, W, device=dev)
-            self._win_I = torch.zeros(B, tG, 1, H, W, device=dev) if self.opt.use_instance else None
+        opt, tG, dev = self.opt, self.opt.n_frames_G, self.device_
+        B, H, W, batched, fresh = self._stream_frames(label_frame, inst_frame, real_frame)
+        face = opt.dataset_mode == 'face' and self.use_single_G
+        if fresh:
+            self._win_A = torch.zeros(B, tG, opt.input_nc if opt.label_nc == 0 else 1, H, W, device=dev)
+            self._win_I = torch.zeros(B, tG, 1, H, W, device=dev) if opt.use_instance else None
+            self._win_B = torch.zeros(B, tG - 1, 3, H, W, device=dev) if face else None
+            self._win_P = torch.zeros(B, tG - 1, 1, H, W, device=dev) if face else None
             self._win_n = 0
-        for win, fr in ((self._win_A, label_frame), (self._win_I, inst_frame if inst_frame is not None else label_frame)):
-            if win is None:
-                continue
-            fr = fr.to(dev, non_blocking=True).contiguous()
-            if fr.dtype not in self._DT:
-                raise TypeError('id maps must be uint8, int32 or float32')
-            L.check(L.lib().v2v_ids_window_push(C.c_void_p(win.data_ptr()), C.c_void_p(fr.data_ptr()), self._DT[fr.dtype], B, tG, H,
-                                                W, L.current_stream_ptr()))
+        if opt.label_nc == 0:
+            fr = label_frame.to(dev, non_blocking=True).contiguous()
+            push = (C.c_int * B)(*[L.SLOT_PUSH] * B)
+            L.check(L.lib().v2v_slots_window_push(C.c_void_p(self._win_A.data_ptr()), C.c_void_p(fr.data_ptr()), self._DT[fr.dtype], B,
+                                                  tG, opt.input_nc, H, W, push, L.current_stream_ptr()))
             L.LAUNCHES[0] += 1
+        else:
+            for win, fr in ((self._win_A, label_frame), (self._win_I, inst_frame if inst_frame is not None else label_frame)):
+                if win is None:
+                    continue
+                fr = fr.to(dev, non_blocking=True).contiguous()
+                if fr.dtype not in self._DT:
+                    raise TypeError('id maps must be uint8, int32 or float32')
+                L.check(L.lib().v2v_ids_window_push(C.c_void_p(win.data_ptr()), C.c_void_p(fr.data_ptr()), self._DT[fr.dtype], B, tG,
+                                                    H, W, L.current_stream_ptr()))
+                L.LAUNCHES[0] += 1
+        if face and self._win_n < tG - 1:            # the frames generate_first_frame reads
+            self._win_B[:, self._win_n].copy_(real_frame.reshape(B, 3, H, W), non_blocking=True)
+            self._win_P[:, self._win_n, 0].copy_(inst_frame.reshape(B, H, W), non_blocking=True)
         self._win_n += 1
         if self._win_n < tG:
             return None
-        fake_B, _ = self.inference(self._win_A, None, self._win_I)
+        fake_B, _ = self.inference(self._win_A, self._win_B, self._win_P if face else self._win_I)
         if out_u8 is None:
             return fake_B
-        shape = (H, W, fake_B.shape[1]) if label_frame.dim() == 2 else (B, H, W, fake_B.shape[1])
+        shape = (B, H, W, fake_B.shape[1]) if batched else (H, W, fake_B.shape[1])
         if getattr(self, '_u8_dev', None) is None or tuple(self._u8_dev.shape) != shape:
             self._u8_dev = torch.empty(shape, dtype=torch.uint8, device=dev)
         L.check(L.lib().v2v_tensor2im_u8(C.c_void_p(fake_B.data_ptr()), C.c_void_p(self._u8_dev.data_ptr()), B, fake_B.shape[1], H,
@@ -276,6 +286,50 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         else:
             out_u8.copy_(self._u8_dev, non_blocking=True)
         return out_u8
+
+    def _stream_frames(self, label_frame, inst_frame, real_frame):
+        """Checks one inference_stream call's frames against the options and the running stream before anything is
+        launched.  Returns (B, H, W, batched: the frames carry a clip axis, fresh: this call starts a new window)."""
+        opt, tG = self.opt, self.opt.n_frames_G
+        face = opt.dataset_mode == 'face' and self.use_single_G
+        win = getattr(self, '_win_A', None)
+
+        def need_face_frames():
+            missing = [n for n, t in (('real_frame', real_frame), ('inst_frame (the part map)', inst_frame)) if t is None]
+            if missing:
+                raise ValueError('a face stream (dataset_mode face with use_single_G) needs %s on each of its first %d calls: the '
+                                 'face first-frame generator reads them' % (' and '.join(missing), tG - 1))
+        if face and (win is None or self._win_n < tG - 1):
+            need_face_frames()
+        if opt.label_nc == 0:
+            C_ = opt.input_nc
+            if label_frame.dim() not in (3, 4) or label_frame.shape[-3] != C_ or label_frame.dtype != torch.float32:
+                raise ValueError('label_frame must be a dense (%d, H, W) or (B, %d, H, W) float32 frame (label_nc 0, input_nc %d), '
+                                 'got %s %s' % (C_, C_, C_, tuple(label_frame.shape), label_frame.dtype))
+            batched = label_frame.dim() == 4
+        else:
+            batched = label_frame.dim() == 3
+            if inst_frame is not None and tuple(inst_frame.shape) != tuple(label_frame.shape):
+                raise ValueError('inst_frame %s does not match label_frame %s' % (tuple(inst_frame.shape), tuple(label_frame.shape)))
+        B = label_frame.shape[0] if batched else 1
+        H, W = label_frame.shape[-2:]
+        if win is not None and win.shape[0] != B:
+            raise ValueError('this stream was started with %d clip(s) and is fed %d: clips of one stream start and advance '
+                             'together (reset_stream() starts a new one)' % (win.shape[0], B))
+        fresh = win is None or tuple(win.shape[-2:]) != (H, W)
+        if not face:
+            if real_frame is not None:
+                raise ValueError('real_frame is taken by face streams only (dataset_mode face with use_single_G)')
+        elif fresh or self._win_n < tG - 1:
+            need_face_frames()                      # a new frame size starts a new window
+            lead = (B,) if batched else ()
+            for name, t, want in (('real_frame', real_frame, lead + (3, H, W)), ('inst_frame', inst_frame, lead + (H, W))):
+                if tuple(t.shape) != want:
+                    raise ValueError('%s %s does not match label_frame %s: expected %s' % (
+                        name, tuple(t.shape), tuple(label_frame.shape), want))
+            if not real_frame.is_floating_point() or inst_frame.dtype not in self._DT:
+                raise TypeError('real_frame must be floating point and inst_frame uint8, int32 or float32')
+        return B, H, W, batched, fresh
 
     def stream_slots(self, B):
         """A slot stream (SlotStream) of B slots over this model's generators: every slot starts, restarts and stops its own
@@ -316,12 +370,17 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
             if self.opt.use_instance:
                 real_A = real_A[:, :, :self.opt.label_nc, :, :]
             frames = []
-            if self.opt.dataset_mode == 'face':
-                # get_face_features picks ONE table row over its whole batch (as the reference does): clip by clip
-                self.netG_i.sample_stats = False
+            if self.opt.dataset_mode == 'face' and self.bs == 1:
                 for i in range(tG - 1):
-                    frames.append(torch.cat([self.netG_i.forward(real_A[c:c + 1, i].contiguous(), self.get_face_features(
-                        real_B[c:c + 1, i], pool_map[c:c + 1, i])) for c in range(self.bs)]).unsqueeze(1))
+                    frames.append(self.netG_i.forward(real_A[:, i].contiguous(), self.get_face_features(
+                        real_B[:, i], pool_map[:, i])).unsqueeze(1))
+            elif self.opt.dataset_mode == 'face':
+                # b independent clips: batch-b per-sample plans (every conv configured as at batch 1) and one table row per
+                # clip, so each clip's first frames equal its own b = 1 run bit for bit
+                with self._per_clip_statistics(True):
+                    for i in range(tG - 1):
+                        frames.append(self.netG_i.forward(real_A[:, i].contiguous(), self.get_face_features_per_clip(
+                            real_B[:, i], pool_map[:, i])).unsqueeze(1))
             else:
                 for i in range(tG - 1):
                     frames.append(self.netG_i.forward(real_A[:, i].contiguous(), None).unsqueeze(1))
@@ -340,6 +399,15 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
         self.face_chosen keeps the (1,) int32 device tensor of the index."""
         feat = self.netE.forward(real_image.contiguous(), inst.contiguous())
         feat_map, self.face_chosen = ops.face_features(feat, inst.contiguous(), self.face_table, self.face_rows, self.face_num_images)
+        return feat_map
+
+    def get_face_features_per_clip(self, real_image, inst):
+        """get_face_features for b independent clips, one image each: the Encoder runs once on the batch and every image gets
+        the nearest table row of its own labels (ops.face_features per_image).  self.face_chosen keeps the (b,) int32 device
+        tensor of the indices."""
+        feat = self.netE.forward(real_image.contiguous(), inst.contiguous())
+        feat_map, self.face_chosen = ops.face_features(feat, inst.contiguous(), self.face_table, self.face_rows, self.face_num_images,
+                                                       per_image=True)
         return feat_map
 
     # ------------------------------------------------------------------ training forward

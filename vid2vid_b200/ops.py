@@ -251,10 +251,12 @@ def instance_mean(x, inst, n_ids, out=None):
     return out
 
 
-def face_features(pooled, inst, table, rows, num_images):
+def face_features(pooled, inst, table, rows, num_images, per_image=False):
     """get_face_features's nearest-neighbour lookup (models/vid2vid_model_G.py:290-320): pooled (N, feat_num, H, W) Encoder
     output, inst (N, 1, H, W) part labels, table (n_labels, max_rows, feat_num + 1) the packed features.npy, rows the
-    per-label row counts (host ints).  Returns (feat_map (N, feat_num, H, W), chosen (1,) int32 device tensor)."""
+    per-label row counts (host ints).  Returns (feat_map (N, feat_num, H, W), chosen int32 device tensor): one row for the
+    whole batch, chosen (1,), as the reference picks it; with per_image every image is an independent clip that gets its own
+    row from its own labels, chosen (N,)."""
     _chk(pooled, inst, table)
     N, F_, H, W = pooled.shape
     n_labels, max_rows, stride = table.shape
@@ -262,11 +264,12 @@ def face_features(pooled, inst, table, rows, num_images):
         raise ValueError('face_features: part map %s / rows %d do not match features %s / table %s' % (
             tuple(inst.shape), len(rows), tuple(pooled.shape), tuple(table.shape)))
     out = torch.empty_like(pooled)
-    chosen = torch.empty(1, dtype=torch.int32, device=pooled.device)
+    chosen = torch.empty(N if per_image else 1, dtype=torch.int32, device=pooled.device)
     arr = (C.c_int * n_labels)(*[int(r) for r in rows])
+    fn = L.lib().v2v_face_features_per_image if per_image else L.lib().v2v_face_features
     with _on(pooled):
-        _ck(L.lib().v2v_face_features(_p(pooled), _p(inst), _p(table), arr, n_labels, max_rows, int(num_images), F_, stride, _p(out),
-                                      C.c_void_p(chosen.data_ptr()), N, H, W, _st(pooled)))
+        _ck(fn(_p(pooled), _p(inst), _p(table), arr, n_labels, max_rows, int(num_images), F_, stride, _p(out),
+               C.c_void_p(chosen.data_ptr()), N, H, W, _st(pooled)))
     return out, chosen
 
 
