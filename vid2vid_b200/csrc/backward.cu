@@ -588,9 +588,13 @@ cudaError_t launch_composite_bwd(const CompositeBwd& p, cudaStream_t s) {
   else composite_bwd_kernel<false><<<grid1d((size_t)p.N * p.H * p.W), 256, 0, s>>>(p);
   return cudaGetLastError();
 }
+// The gradient import / export transposes through 32 x 32 shared-memory tiles (grad_layout_tiled_kernel) when a tile row of
+// channels is worth it and the grid fits; narrow tensors (C < 8: the 3-channel images) take the elementwise kernels.
+int grad_layout_tiled(int N, int C, long long HW) { return C >= 8 && (HW + 31) / 32 <= 0x7fffffffLL && N <= 65535; }
+
 cudaError_t launch_grad_import(const float* g, float* dst, int N, int C_src, int c_off, int C, int H, int W, cudaStream_t s) {
   const size_t HW = (size_t)H * W;
-  if (C >= 8 && (HW + 31) / 32 <= 0x7fffffffULL && N <= 65535) {
+  if (grad_layout_tiled(N, C, (long long)HW)) {
     dim3 grid((unsigned)((HW + 31) / 32), (C + 31) / 32, N);
     grad_layout_tiled_kernel<true><<<grid, 256, 0, s>>>(const_cast<float*>(g), dst, C_src, c_off, C, HW);
     return cudaGetLastError();
@@ -600,7 +604,7 @@ cudaError_t launch_grad_import(const float* g, float* dst, int N, int C_src, int
 }
 cudaError_t launch_grad_export(const float* src, float* g, int N, int C_src, int c_off, int C, int H, int W, cudaStream_t s) {
   const size_t HW = (size_t)H * W;
-  if (C >= 8 && N <= 65535) {
+  if (grad_layout_tiled(N, C, (long long)HW)) {
     dim3 grid((unsigned)((HW + 31) / 32), (C + 31) / 32, N);
     grad_layout_tiled_kernel<false><<<grid, 256, 0, s>>>(g, const_cast<float*>(src), C_src, c_off, C, HW);
     return cudaGetLastError();

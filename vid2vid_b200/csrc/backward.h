@@ -85,6 +85,7 @@ struct NormBwdLaunch {
 };
 NormBwdLaunch norm_bwd_launch(int N, int H, int W, int C, int raw_C, int c_off, int has_norm, int param);
 int bias_grad_blocks(long long npix);          // bias_grad_kernel: blocks per channel (grid.y)
+int grad_layout_tiled(int N, int C, long long HW);   // 1: launch_grad_import / launch_grad_export take the tiled kernel
 
 cudaError_t launch_conv_bwd(const BwdConv& p, cudaStream_t s);
 cudaError_t launch_norm_bwd(const NormBwd& p, cudaStream_t s);

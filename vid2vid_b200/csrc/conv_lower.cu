@@ -386,7 +386,8 @@ void fill_conv_params(v2v_plan* P, GOp& op) {
   kp.Khalf = op.Ktotal;
 }
 
-int pack_one(const GOp& op, cudaStream_t stream) {
+// The packing of a lowered conv op's weights (out: op.wpacked, null before finalize)
+PackParams pack_params(const GOp& op) {
   PackParams pp{};
   pp.w = op.conv.weight; pp.transposed = op.conv.transposed;
   pp.w2 = op.conv.Cout2 > 0 ? op.conv.weight2 : nullptr; pp.Cout1 = op.conv.Cout - op.conv.Cout2;
@@ -396,8 +397,26 @@ int pack_one(const GOp& op, cudaStream_t stream) {
     for (int kx = 0; kx < op.conv.kw; ++kx) { pp.tap_ky[ky * op.conv.kw + kx] = (int8_t)ky; pp.tap_kx[ky * op.conv.kw + kx] = (int8_t)kx; }
   pp.out = op.wpacked;
   if (op.pack_dgrad) { pp.dgrad = 1; pp.w2 = op.dg_w2; pp.Cout1 = op.dg_Cout1; }
-  V2V_CUDA(launch_pack_weights(pp, stream));
+  return pp;
+}
+
+int pack_one(const GOp& op, cudaStream_t stream) {
+  V2V_CUDA(launch_pack_weights(pack_params(op), stream));
   return 0;
+}
+
+// One "pack" layout record: the packed matrix [rows][split + 1][Ktotal] at arena offset w_off and the path that writes it
+// (TC of the tiled kernel, 0 for the elementwise one).  Needs the op lowered and the arena sized.
+void describe_pack(const v2v_plan* P, size_t i, std::string& s) {
+  const GOp& op = P->gops[i];
+  const PackParams pp = pack_params(op);
+  char t[512];
+  snprintf(t, sizeof(t),
+           "{\"kind\":\"pack\",\"gop\":%zu,\"w_off\":%zu,\"rows\":%d,\"Ktotal\":%d,\"Cout\":%d,\"Cin\":%d,\"k\":[%d,%d],\"ntaps\":%d,"
+           "\"Cp\":%d,\"split\":%d,\"transposed\":%d,\"headkx\":%d,\"dgrad\":%d,\"w2\":%d,\"Cout1\":%d,\"TC\":%d}",
+           i, P->w_off[i], pp.headkx ? pp.headkx * pp.Cout : pp.Cout, op.Ktotal, pp.Cout, pp.Cin, pp.kh, pp.kw, pp.ntaps, pp.Cp,
+           pp.split, pp.transposed, pp.headkx, pp.dgrad, pp.w2 != nullptr, pp.Cout1, pack_weights_tiling(pp));
+  s += t;
 }
 
 // One conv record of v2v_plan_describe: the conv, its geometry and the kernel configuration fill_conv_params chooses (host-only

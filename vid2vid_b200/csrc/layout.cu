@@ -215,11 +215,14 @@ cudaError_t launch_bias_affine(float* scale, float* shift, const float* bias, in
   return cudaGetLastError();
 }
 
+// channels per import block: 16 for narrow buffers (one block covers every channel), else 64
+int import_tile_channels(const ActDesc& o) { return o.C <= 16 ? 16 : 64; }
+
 cudaError_t launch_import_nchw(const ImportParams& p, cudaStream_t stream) {
   const ActDesc& o = p.out;
   const int Wpad = o.W + o.pad_l + o.pad_r, Hpad = o.H + o.pad_t + o.pad_b;
   dim3 block(32, 8);
-  if (o.C <= 16) {
+  if (import_tile_channels(o) == 16) {
     dim3 grid((Wpad + 127) / 128, Hpad * o.N, 1);
     import_nchw_kernel<16><<<grid, block, 0, stream>>>(p);
   } else {
@@ -287,22 +290,29 @@ __global__ void __launch_bounds__(256) pack_weights_tiled_kernel(PackParams p, i
   }
 }
 
-cudaError_t launch_pack_weights(const PackParams& p, cudaStream_t stream) {
+// TC of pack_weights_tiled_kernel (forward output channels per block: 32, 16 or 4, as many as fit 40 KB of staging), or 0
+// when the elementwise kernel packs: transposed convs, kx-GEMM heads, tap orders other than the filter's, tiles over 48 KB
+int pack_weights_tiling(const PackParams& p) {
   const int taps = p.kh * p.kw;
   bool natural = !p.transposed && !p.headkx && p.ntaps == taps;
   for (int t = 0; t < taps && natural; ++t) natural = (p.tap_ky[t] * p.kw + p.tap_kx[t] == t);
-  if (natural) {
-    const int tstride = taps | 1;
-    int TC = 32;
-    while (TC > 4 && (size_t)TC * (32 * tstride + 1) * sizeof(float) > 40 * 1024) TC >>= 1;
-    if ((size_t)TC * (32 * tstride + 1) * sizeof(float) <= 48 * 1024) {
-      // grid: x over the 32-wide tiles of the forward INPUT channel axis, y over TC-wide tiles of the forward OUTPUT channel axis;
-      // each axis covers the padded extent where it is the K axis of the packed matrix (zero fill)
-      const int f_out = p.dgrad ? std::max(p.Cin, p.Cp) : p.Cout, f_in = p.dgrad ? p.Cout : std::max(p.Cin, p.Cp);
-      dim3 grid((f_in + 31) / 32, (f_out + TC - 1) / TC);
-      pack_weights_tiled_kernel<<<grid, 256, (size_t)TC * (32 * tstride + 1) * sizeof(float), stream>>>(p, TC);
-      return cudaGetLastError();
-    }
+  if (!natural) return 0;
+  const int tstride = taps | 1;
+  int TC = 32;
+  while (TC > 4 && (size_t)TC * (32 * tstride + 1) * sizeof(float) > 40 * 1024) TC >>= 1;
+  return (size_t)TC * (32 * tstride + 1) * sizeof(float) <= 48 * 1024 ? TC : 0;
+}
+
+cudaError_t launch_pack_weights(const PackParams& p, cudaStream_t stream) {
+  const int TC = pack_weights_tiling(p);
+  if (TC) {
+    const int tstride = (p.kh * p.kw) | 1;
+    // grid: x over the 32-wide tiles of the forward INPUT channel axis, y over TC-wide tiles of the forward OUTPUT channel axis;
+    // each axis covers the padded extent where it is the K axis of the packed matrix (zero fill)
+    const int f_out = p.dgrad ? std::max(p.Cin, p.Cp) : p.Cout, f_in = p.dgrad ? p.Cout : std::max(p.Cin, p.Cp);
+    dim3 grid((f_in + 31) / 32, (f_out + TC - 1) / TC);
+    pack_weights_tiled_kernel<<<grid, 256, (size_t)TC * (32 * tstride + 1) * sizeof(float), stream>>>(p, TC);
+    return cudaGetLastError();
   }
   const long long total = (long long)(p.headkx ? p.headkx * p.Cout : p.Cout) * p.ntaps * p.Cp;
   long long b = (total + 255) / 256;

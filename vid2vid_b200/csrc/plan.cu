@@ -289,6 +289,117 @@ ApplyParams apply_params(const v2v_plan* P, const GOp& op, size_t m) {
 }
 
 
+// The arena layout of v2v_plan_describe (host-only: needs the arena sized): one "buffers" record per activation buffer (its byte
+// offset in the arena and the ActDesc fields that place element (n, c, y, x)), and one "scratch" record per correlation's fp32
+// scratch [in1 | in2 | out], each NCHW.  A caller that finalizes into its own workspace can decode every buffer from these.
+void describe_buffers(const v2v_plan* P, std::string& s) {
+  char t[512];
+  bool first = true;
+  for (size_t v = 0; v < P->values.size(); ++v)
+    for (size_t m = 0; m < P->values[v].bufs.size(); ++m) {
+      const int b = P->values[v].bufs[m];
+      const ActDesc& a = P->acts[b];
+      snprintf(t, sizeof(t),
+               "%s{\"value\":%zu,\"buf\":%d,\"off\":%zu,\"N\":%d,\"H\":%d,\"W\":%d,\"C\":%d,\"Cvalid\":%d,\"pads\":[%d,%d,%d,%d],"
+               "\"parity\":%d,\"P\":%d,\"Hp\":%d,\"Wp\":%d,\"split\":%d,\"mode\":%d}",
+               first ? "" : ",", v, b, P->act_off[b], a.N, a.H, a.W, a.C, a.Cvalid, a.pad_t, a.pad_l, a.pad_b, a.pad_r, a.parity, a.P,
+               a.Hp, a.Wp, a.split, P->act_pad_mode[b]);
+      s += t;
+      first = false;
+    }
+  s += "],\"scratch\":[";
+  first = true;
+  for (size_t i = 0; i < P->gops.size(); ++i) {
+    const GOp& op = P->gops[i];
+    if (op.kind != G_CORR) continue;
+    const Value& a = P->values[op.value_in], &o = P->values[op.value_out];
+    snprintf(t, sizeof(t), "%s{\"gop\":%zu,\"off\":%zu,\"N\":%d,\"C\":%d,\"H\":%d,\"W\":%d,\"C_out\":%d,\"H_out\":%d,\"W_out\":%d}",
+             first ? "" : ",", i, P->corr_off[i], a.N, a.C, a.H, a.W, o.C, o.H, o.W);
+    s += t;
+    first = false;
+  }
+}
+
+static void describe_import(const v2v_plan* P, size_t i, int buf, int slot, int C_src, int c_off, int direct, int act, int skip_lo,
+                            std::string& s) {
+  const ActDesc& o = P->acts[buf];
+  char t[512];
+  snprintf(t, sizeof(t),
+           "{\"kind\":\"import\",\"gop\":%zu,\"buf\":%d,\"slot\":%d,\"direct\":%d,\"C_src\":%d,\"c_off\":%d,\"act\":%d,\"pad_mode\":%d,"
+           "\"skip_lo\":%d,\"split\":%d,\"parity\":%d,\"N\":%d,\"H\":%d,\"W\":%d,\"C\":%d,\"Cvalid\":%d,\"Wpad\":%d,\"CT\":%d}",
+           i, buf, slot, direct, C_src, c_off, act, P->act_pad_mode[buf], skip_lo, o.split, o.parity, o.N, o.H, o.W, o.C, o.Cvalid,
+           o.W + o.pad_l + o.pad_r, import_tile_channels(o));
+  s += t;
+}
+
+static void describe_export(const v2v_plan* P, size_t i, int buf, int direct, std::string& s) {
+  const ActDesc& a = P->acts[buf];
+  char t[320];
+  snprintf(t, sizeof(t), "{\"kind\":\"export\",\"gop\":%zu,\"buf\":%d,\"direct\":%d,\"split\":%d,\"N\":%d,\"H\":%d,\"W\":%d,\"C\":%d,\"Cvalid\":%d}",
+           i, buf, direct, a.split, a.N, a.H, a.W, a.C, a.Cvalid);
+  s += t;
+}
+
+static void describe_grad_layout(const char* kind, size_t i, const Value& v, int C_src, int c_off, std::string& s) {
+  char t[320];
+  const long long HW = (long long)v.H * v.W;
+  snprintf(t, sizeof(t), "{\"kind\":\"%s\",\"gop\":%zu,\"N\":%d,\"C\":%d,\"H\":%d,\"W\":%d,\"C_src\":%d,\"c_off\":%d,\"tiled\":%d}", kind,
+           i, v.N, v.C, v.H, v.W, C_src, c_off, grad_layout_tiled(v.N, v.C, HW));
+  s += t;
+}
+
+// The "layout" records of v2v_plan_describe, in the order finalize emits the launches: every import (caller tensor or
+// correlation scratch), export, concat copy and weight pack, with the fields that select its code path.  Training plans add
+// the gradient import of every export and the gradient export of every input (assuming the caller passes both gradients),
+// and per tensor-core backward unit its fold, dgrad pack and unstage (describe_backward_layout).
+void describe_layout(const v2v_plan* P, std::string& s) {
+  char t[320];
+  bool first = true;
+  auto sep = [&]() { if (!first) s += ","; first = false; };
+  for (size_t i = 0; i < P->gops.size(); ++i) {
+    const GOp& op = P->gops[i];
+    switch (op.kind) {
+      case G_INPUT: {
+        const Value& v = P->values[op.value_out];
+        for (int b : v.bufs) { sep(); describe_import(P, i, b, op.slot, op.C_src, op.c_off, 0, ACT_NONE, v.exact_bf16 ? 1 : 0, s); }
+        break;
+      }
+      case G_CONV: case G_CONV_ACT: case G_HEAD: sep(); describe_pack(P, i, s); break;
+      case G_EXPORT: sep(); describe_export(P, i, P->values[op.value_in].bufs[0], 0, s); break;
+      case G_CONCAT: {
+        for (int b : P->values[op.value_out].bufs) {
+          int c_off = 0;
+          for (int src : op.cat_in) {
+            const ActDesc& a = P->acts[P->values[src].bufs[0]], &o = P->acts[b];
+            sep();
+            snprintf(t, sizeof(t), "{\"kind\":\"copy\",\"gop\":%zu,\"in_buf\":%d,\"buf\":%d,\"c_off\":%d,\"Cvalid\":%d,\"pad_mode\":%d,"
+                     "\"in_split\":%d,\"split\":%d,\"parity\":%d}",
+                     i, P->values[src].bufs[0], b, c_off, a.Cvalid, P->act_pad_mode[b], a.split, o.split, o.parity);
+            s += t;
+            c_off += P->values[src].C;
+          }
+        }
+        break;
+      }
+      case G_CORR: {
+        sep(); describe_export(P, i, P->values[op.value_in].bufs[0], 1, s);
+        sep(); describe_export(P, i, P->values[op.value_in2].bufs[0], 1, s);
+        const Value& vo = P->values[op.value_out];
+        for (int b : vo.bufs) { sep(); describe_import(P, i, b, 0, vo.C, 0, 1, op.act, 0, s); }
+        break;
+      }
+      default: break;
+    }
+  }
+  if (!P->train) return;
+  for (size_t i = 0; i < P->gops.size(); ++i) {
+    const GOp& op = P->gops[i];
+    if (!P->op_live[i]) continue;
+    if (op.kind == G_EXPORT) { const Value& v = P->values[op.value_in]; sep(); describe_grad_layout("grad_import", i, v, v.C, 0, s); }
+    if (op.kind == G_INPUT) { sep(); describe_grad_layout("grad_export", i, P->values[op.value_out], op.C_src, op.c_off, s); }
+  }
+}
+
 // The forward epilogue of the plan's norm layers, as finalize emits it (the same host functions choose it), three kinds of
 // record:
 //   stats     one per conv whose raw a norm layer reads: how conv_umma_kernel accumulates the statistics rows (async_epi, MG,
@@ -976,6 +1087,7 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
   if (!P) return 0;
   if (!P->lowered && lower(P)) return -1;
   std::string s = "{\"values\":[";
+  std::string bwd_layout;            // training plans: the backward units' layout records, appended to "layout"
   char t[512];
   for (size_t i = 0; i < P->values.size(); ++i) {
     const Value& v = P->values[i];
@@ -1002,14 +1114,19 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
     s += "],\"backward\":[";
     first = true;
     if (P->finalized) {
-      for (const BwdUnit& u : P->bwd) { if (!first) s += ","; describe_backward_unit(u, s); first = false; }
+      for (const BwdUnit& u : P->bwd) {
+        if (!first) s += ",";
+        describe_backward_unit(u, s);
+        describe_backward_layout(P, u, bwd_layout);
+        first = false;
+      }
     } else {
       for (size_t i = 0; i < P->gops.size(); ++i) {
         const GOp& op = P->gops[i];
         if (!(op.kind == G_CONV || op.kind == G_CONV_ACT || op.kind == G_HEAD) || !P->op_live[i]) continue;
         BwdUnit u;
         const int rc = choose_backward_unit(P, (int)i, u);
-        if (!rc) { if (!first) s += ","; describe_backward_unit(u, s); first = false; }
+        if (!rc) { if (!first) s += ","; describe_backward_unit(u, s); describe_backward_layout(P, u, bwd_layout); first = false; }
         if (u.child) v2v_plan_destroy(u.child);
         if (rc) return -1;
       }
@@ -1021,6 +1138,11 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
   s += "],\"epilogue_forward\":[";
   if (!P->sized && size_arena(P)) return -1;          // the raw tensors' element type and channel stride (host-only)
   describe_epilogue_forward(P, s);
+  s += "],\"buffers\":[";
+  describe_buffers(P, s);
+  s += "],\"layout\":[";
+  describe_layout(P, s);
+  s += s.back() == '[' ? bwd_layout.substr(bwd_layout.empty() ? 0 : 1) : bwd_layout;
   // ops the backward visits (0 for the forward-only branch of a feature L1 target) and values without a gradient buffer
   int bwd_ops = 0, detached = 0;
   for (char l : P->op_live) bwd_ops += l;

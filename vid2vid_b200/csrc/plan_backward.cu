@@ -96,6 +96,11 @@ int choose_backward_unit(v2v_plan* P, int i, BwdUnit& u) {
     u.mode = 1; cd.stride = 1; cd.pad = c.kh - 1;
   } else if (c.transposed && c.Cout2 == 0) {
     u.mode = 2; cd.stride = 2; cd.pad = c.pad;
+  } else if (!c.transposed && c.stride == 2 && c.pad_mode == V2V_PAD_REFLECT && c.pad > 0) {
+    // mode 3 crops the transposed conv's output to the interior: the gradient of the reflected halo rows and columns would be
+    // dropped instead of mirrored back (the SIMT data gradient folds it)
+    u.simt = "stride-2 conv behind a reflect halo: the cropped transposed conv cannot fold the mirrored halo";
+    return 0;
   } else if (!c.transposed && c.stride == 2 && c.Cout2 == 0 && c.kh == c.kw && 2 + 2 * c.pad - c.kh >= 0 && 2 * oh >= vin.H && 2 * ow >= vin.W) {
     // the transposed conv is asked for exactly 2 oh x 2 ow outputs (output_padding 2 + 2 pad - k; for 4x4 / pad 2 that is one
     // row more than nn.ConvTranspose2d would accept, the extra rows are simply cropped by fold_add)
@@ -379,6 +384,34 @@ void describe_backward_unit(const BwdUnit& u, std::string& s) {
     s += t;
   } else {
     s += "null}";
+  }
+}
+
+// The layout launches of one tensor-core backward unit as run_backward makes them (each record with a leading comma): the
+// packing of the sub-plan's weights (the dgrad packing in mode 1), the fold of the data gradient into dX (crop: the sub-plan's
+// output extends past the padded input; overlap: a reflect halo so deep that the top and bottom, or left and right, mirrors
+// reach the same pixel) and the unstage of the weight gradient.
+void describe_backward_layout(const v2v_plan* P, const BwdUnit& u, std::string& s) {
+  if (!u.mode) return;
+  char t[512];
+  s += ",";
+  describe_pack(u.child, 1, s);
+  const GOp& op = P->gops[u.gop];
+  const Value& vin = P->values[op.value_in];
+  const Raw& cr = u.child->raws[u.child_raw];
+  const int pad = u.mode == 1 ? op.conv.pad : 0;
+  const int reflect = (op.conv.pad_mode == V2V_PAD_REFLECT && pad > 0) ? 1 : 0;
+  const int crop = cr.H > vin.H + 2 * pad || cr.W > vin.W + 2 * pad;
+  const int overlap = reflect && (pad >= vin.H - 1 - pad || pad >= vin.W - 1 - pad);
+  snprintf(t, sizeof(t),
+           ",{\"kind\":\"fold\",\"gop\":%d,\"mode\":%d,\"pad\":%d,\"reflect\":%d,\"crop\":%d,\"overlap\":%d,\"N\":%d,\"H\":%d,\"W\":%d,"
+           "\"C\":%d,\"PH\":%d,\"PW\":%d,\"Cs\":%d}",
+           u.gop, u.mode, pad, reflect, crop, overlap, vin.N, vin.H, vin.W, op.conv.Cin, cr.H, cr.W, cr.desc.C);
+  s += t;
+  if (u.wgrad) {
+    snprintf(t, sizeof(t), ",{\"kind\":\"unstage\",\"gop\":%d,\"swap\":%d,\"R\":%d,\"R1\":%d,\"Cc\":%d,\"taps\":%d,\"Mp\":%d,\"Np\":%d}",
+             u.gop, u.wg.swap, u.M, u.M1, u.Nv, u.wg.ntaps, u.wg.Mp, u.wg.Np);
+    s += t;
   }
 }
 

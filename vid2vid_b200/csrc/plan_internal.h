@@ -205,8 +205,10 @@ int conv_geometry(const v2v_conv_desc& c, int Cp, int head, int N, int H, int W,
 void fill_conv_params(v2v_plan* P, GOp& op);
 int make_tmap_act(CUtensorMap* tm, const ActDesc& a, int box_w, int box_h, int kc);
 int make_tmap_w(CUtensorMap* tm, bf16* w, int Ktotal, int Cout, int BN, int kc);
+PackParams pack_params(const GOp& op);
 int pack_one(const GOp& op, cudaStream_t stream);
 void describe_conv(v2v_plan* P, const GOp& op, std::string& s);
+void describe_pack(const v2v_plan* P, size_t i, std::string& s);
 
 // plan.cu
 int new_value(v2v_plan* p, int N, int H, int W, int C);
@@ -216,6 +218,8 @@ FeatL1Params featl1_params(const v2v_plan* P, const GOp& op);
 std::vector<int> finalize_sites(const v2v_plan* P);
 ApplyParams apply_params(const v2v_plan* P, const GOp& op, size_t m);
 void describe_epilogue_forward(v2v_plan* P, std::string& s);
+void describe_buffers(const v2v_plan* P, std::string& s);
+void describe_layout(const v2v_plan* P, std::string& s);
 
 // plan_backward.cu
 int alloc_training(v2v_plan* P, cudaStream_t stream);
@@ -225,5 +229,6 @@ int run_backward(v2v_plan* P, void* const* io, void* const* gio, const std::unor
                  cudaStream_t s);
 void describe_backward_unit(const BwdUnit& u, std::string& s);
 void describe_epilogue_backward(const v2v_plan* P, std::string& s);
+void describe_backward_layout(const v2v_plan* P, const BwdUnit& u, std::string& s);
 
 }  // namespace v2v

@@ -290,6 +290,8 @@ NormApplyLaunch norm_apply_launch(const ApplyParams& p);
 cudaError_t launch_import_nchw(const ImportParams& p, cudaStream_t stream);
 cudaError_t launch_export_nchw(const ExportParams& p, cudaStream_t stream);
 cudaError_t launch_pack_weights(const PackParams& p, cudaStream_t stream);
+int import_tile_channels(const ActDesc& o);      // CT of the import_nchw_kernel launch: 16 or 64
+int pack_weights_tiling(const PackParams& p);    // TC of pack_weights_tiled_kernel, 0: the elementwise pack_weights_kernel
 cudaError_t launch_act_copy(const CopyParams& p, cudaStream_t stream);
 cudaError_t launch_bias_affine(float* scale, float* shift, const float* bias, int N, int C, int stride, cudaStream_t stream);
 cudaError_t launch_correlation(const float*, const float*, float*, int, int, int, int, int, int, int, int, int, cudaStream_t);
