@@ -122,21 +122,26 @@ def test_device_reference_matches_cpu():
 
 
 def _backward_records(describe):
+    """The plan's description on the host, and read from what finalize built."""
     p = Plan(0, precision='precise', train=True)
     describe(p)
-    before = p.describe()['backward']
+    before = p.describe()
     p.finalize()
-    return before, p.describe()['backward']
+    return before, p.describe()
 
 
 def test_describe_matches_finalized_backward():
-    """The "backward" records v2v_plan_describe derives on the host equal the ones read from the units finalize built."""
+    """The description v2v_plan_describe derives on the host equals the one read from the plan finalize built: the backward
+    units, and the forward launch list's layout and epilogue records (imports, packs, statistics, tail finalisations and
+    normalise passes)."""
     runner = _runner(lambda: [nn.ReflectionPad2d(3), _c(6, 64, 7, 1, 0), BN(64), _c(64, 128, 3, 2, 1), BN(128), _t(128, 64), BN(64)],
                      _tanh(64), 1.0, False)
     before, after = _backward_records(lambda p: runner._describe(p, 1, 6, 32, 64))
-    assert len(before) == 4 and {b['mode'] for b in before} == {1, 2, 3}, before
+    assert len(before['backward']) == 4 and {b['mode'] for b in before['backward']} == {1, 2, 3}, before['backward']
+    assert {r['kind'] for r in before['epilogue_forward']} == {'stats', 'finalize', 'apply'}, before['epilogue_forward']
+    assert {'import', 'pack'} <= {r['kind'] for r in before['layout']}, before['layout']
     assert before == after
     d = NW.define_D(39, 64, 3, 'batch', 1, True, []).cuda()
     before, after = _backward_records(lambda p: d._describe(p, 0, 1, 64, 128))
-    assert len(before) >= 4 and any(b['wgrad'] for b in before), before
+    assert len(before['backward']) >= 4 and any(b['wgrad'] for b in before['backward']), before['backward']
     assert before == after

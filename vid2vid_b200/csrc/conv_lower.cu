@@ -382,6 +382,16 @@ void fill_conv_params(v2v_plan* P, GOp& op) {
   kp.bias = c.bias;
   kp.lrelu_slope = op.slope;
   kp.act = op.act;
+  if (op.kind == G_HEAD) {          // each channel's destination in its IO slot (the head backward reads the same offsets)
+    kp.epi = EPI_HEAD_F32;
+    kp.bias2 = c.Cout2 > 0 ? c.bias2 : nullptr; kp.Cout1 = c.Cout - c.Cout2;
+    for (int j = 0; j < c.Cout; ++j) {
+      kp.head_slot[j] = op.head[j].slot;
+      kp.head_off[j] = (long long)op.head[j].channel * g.out_h * g.out_w;
+      kp.head_bstride[j] = (long long)op.head[j].dst_C * g.out_h * g.out_w;
+      kp.head_act[j] = op.head[j].act; kp.head_scale[j] = op.head[j].scale;
+    }
+  }
   op.Cp = kp.Cp; op.Ktotal = (g.headkx ? c.kh : c.kh * c.kw) * kp.Cp;
   kp.Khalf = op.Ktotal;
 }
@@ -419,14 +429,12 @@ void describe_pack(const v2v_plan* P, size_t i, std::string& s) {
   s += t;
 }
 
-// One conv record of v2v_plan_describe: the conv, its geometry and the kernel configuration fill_conv_params chooses (host-only
-// logic; no device state needed).
-void describe_conv(v2v_plan* P, const GOp& op, std::string& s) {
+// One conv record of v2v_plan_describe: the conv, its geometry and the kernel configuration fill_conv_params chose (needs the
+// arena sized).
+void describe_conv(const v2v_plan* P, const GOp& op, std::string& s) {
   char t[512];
   const ConvGeom& g = op.geom;
-  GOp tmp = op;                                  // kernel configuration (host-only logic; no device state needed)
-  fill_conv_params(const_cast<v2v_plan*>(P), tmp);
-  const ConvKernelParams& kp = tmp.kp;
+  const ConvKernelParams& kp = op.kp;
   // EG: epilogue groups per tile, always 1 (one 256-thread epilogue stores every tile; async_epi: which threads run it)
   snprintf(t, sizeof(t),
            "{\"kind\":%d,\"Cin\":%d,\"Cout\":%d,\"k\":[%d,%d],\"stride\":%d,\"transposed\":%d,\"in\":%d,\"TH\":%d,\"TW\":%d,"

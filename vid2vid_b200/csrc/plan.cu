@@ -205,8 +205,8 @@ int run_xop(v2v_plan* P, const XOp& x, cudaStream_t s) {
     case X_FEATL1: V2V_CUDA(launch_feature_l1(x.fl1, s)); break;
     case X_CONV: {
       const GOp& op = P->gops[x.gop];
-      if (P->impl == V2V_IMPL_UMMA) V2V_CUDA(launch_conv_umma(op.tmA, op.tmB, op.kp, s));
-      else V2V_CUDA(launch_conv_simt(P->acts[P->values[op.value_in].bufs[op.req_index]], op.wpacked, op.Ktotal, op.kp, s));
+      if (P->impl == V2V_IMPL_UMMA) V2V_CUDA(launch_conv_umma(op.tmA, op.tmB, x.kp, s));
+      else V2V_CUDA(launch_conv_simt(P->acts[P->values[op.value_in].bufs[op.req_index]], op.wpacked, op.Ktotal, x.kp, s));
       break;
     }
   }
@@ -222,26 +222,14 @@ FeatL1Params featl1_params(const v2v_plan* P, const GOp& op) {
   return f;
 }
 
-// Where the statistics of each (raw, channel slice) are finalised, per graph op: 0 / 1 = the tail slot of the producing
-// tensor-core conv launch (the CTA that takes its last ticket, conv_umma.cu), 2 = a stand-alone stats_finalize launch (the
-// SIMT implementation, a third slice of one raw), -1 = nothing (not a normalising op, or a later pass over a slice an earlier
-// op finalises: a second output layout, defer_last).  The side effects happen once per slice, however many passes read it.
-std::vector<int> finalize_sites(const v2v_plan* P) {
-  std::vector<int> site(P->gops.size(), -1);
-  std::vector<std::vector<int>> done(P->raws.size());          // per raw: the slice offsets finalised so far
-  for (size_t i = 0; i < P->gops.size(); ++i) {
-    const GOp& op = P->gops[i];
-    if (op.kind != G_NORM_ACT || op.norm.kind == V2V_NORM_NONE) continue;
-    std::vector<int>& d = done[op.raw];
-    if (std::find(d.begin(), d.end(), op.n_off) != d.end()) continue;
-    site[i] = (P->impl == V2V_IMPL_UMMA && d.size() < 2) ? (int)d.size() : 2;
-    d.push_back(op.n_off);
-  }
-  return site;
+// Address `off` bytes into the plan's arena.  Integer arithmetic: before finalize binds the arena (null) an address is its
+// offset, so the host-only emission never offsets a null pointer.
+template <class T> static T* arena_at(const v2v_plan* P, size_t off) {
+  return reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(P->arena) + off);
 }
 
 // The finalisation of the slice a normalising G_NORM_ACT reads, with its train-mode side effects (running statistics; the
-// scale / shift / mean / rstd arrays the normalise passes and the backward read).  Arena pointers are valid after size_arena.
+// scale / shift / mean / rstd arrays the normalise passes and the backward read).
 static int finalize_params(const v2v_plan* P, const GOp& op, FinalizeParams& fp) {
   const Raw& r = P->raws[op.raw];
   const GOp& cop = P->gops[r.conv_op];
@@ -263,8 +251,8 @@ static int finalize_params(const v2v_plan* P, const GOp& op, FinalizeParams& fp)
 
 // The normalise pass of a G_NORM_ACT (or the plain conversion of a G_RAWIN) into output layout m of its value.  The raw is
 // read through the op's channel slice at the full row stride; scale / shift are the slice's (null: identity, G_RAWIN and
-// norm-less unbiased convs).  Arena pointers are valid after finalize; the launch shape depends on the layouts only.
-ApplyParams apply_params(const v2v_plan* P, const GOp& op, size_t m) {
+// norm-less unbiased convs).  The launch shape depends on the layouts only.
+static ApplyParams apply_params(const v2v_plan* P, const GOp& op, size_t m) {
   const Value& vo = P->values[op.value_out];
   ApplyParams ap{};
   if (op.kind == G_RAWIN) {
@@ -273,12 +261,14 @@ ApplyParams apply_params(const v2v_plan* P, const GOp& op, size_t m) {
     ap.scale = nullptr; ap.shift = nullptr; ap.scale_stride = 0; ap.act = ACT_NONE; ap.slope = 0.f; ap.n_add = 0;
   } else {
     const Raw& r = P->raws[op.raw];
+    const v2v_plan::RawOff& o = P->raw_off[op.raw];
     const GOp& cop = P->gops[r.conv_op];
     ap.raw = r.desc;
-    ap.raw.base = reinterpret_cast<uint8_t*>(r.desc.base) + (size_t)op.n_off * r.desc.elem_bytes();
+    ap.raw.base = arena_at<void>(P, o.raw + (size_t)op.n_off * r.desc.elem_bytes());
     ap.raw.Cvalid = op.cC;                                               // channel slice, full row stride
-    ap.scale = (op.norm.kind != V2V_NORM_NONE || cop.conv.bias != nullptr) ? r.scale + op.n_off : nullptr;
-    ap.shift = r.shift + op.n_off;
+    const bool scaled = op.norm.kind != V2V_NORM_NONE || cop.conv.bias != nullptr;
+    ap.scale = scaled ? arena_at<float>(P, o.scale + op.n_off * sizeof(float)) : nullptr;
+    ap.shift = arena_at<float>(P, o.shift + op.n_off * sizeof(float));
     ap.scale_stride = r.C;
     ap.act = op.act; ap.slope = op.slope;
     ap.n_add = 0;
@@ -288,11 +278,171 @@ ApplyParams apply_params(const v2v_plan* P, const GOp& op, size_t m) {
   return ap;
 }
 
+// Host-only: the forward launch list of a sized plan, in launch order, with every launch's parameters.  Arena addresses come
+// from the buffers finalize binds and from arena_at, so on an unbound plan the list differs from the finalized one in its
+// addresses only.  v2v_plan_finalize runs this list and v2v_plan_describe reports it: both refuse the same plans.
+static int emit_forward(const v2v_plan* P, std::vector<XOp>& xops) {
+  if (P->stats_end > P->stats_begin) {
+    XOp m; m.kind = X_MEMSET; m.ms_ptr = arena_at<void>(P, P->stats_begin); m.ms_bytes = P->stats_end - P->stats_begin;
+    xops.push_back(m);
+  }
+  std::vector<int> conv_x(P->gops.size(), -1);                 // per conv op: its launch in xops
+  std::vector<std::vector<int>> read(P->raws.size()), fin(P->raws.size());   // per raw: the slices normalised / finalised so far
+  for (size_t i = 0; i < P->gops.size(); ++i) {
+    const GOp& op = P->gops[i];
+    switch (op.kind) {
+      case G_INPUT: {
+        const Value& v = P->values[op.value_out];
+        for (size_t m = 0; m < v.bufs.size(); ++m) {
+          XOp x; x.kind = X_IMPORT; x.gop = (int)i; x.buf = v.bufs[m];
+          x.imp.io = reinterpret_cast<const void* const*>(P->io_dev); x.imp.slot = op.slot;
+          x.imp.c_off = op.c_off; x.imp.C_src = op.C_src;
+          x.imp.out = P->acts[v.bufs[m]]; x.imp.pad_mode = P->act_pad_mode[v.bufs[m]];
+          x.imp.skip_lo = v.exact_bf16 ? 1 : 0;
+          xops.push_back(x);
+        }
+        break;
+      }
+      case G_CONV: case G_CONV_ACT: case G_HEAD: {
+        const ActDesc& ain = P->acts[P->values[op.value_in].bufs[op.req_index]];
+        XOp x; x.kind = X_CONV; x.gop = (int)i;
+        ConvKernelParams& kp = x.kp;
+        kp = op.kp;
+        // the kernel addresses the lo half of the input at channel coordinate Cp: the buffer must be padded to exactly that
+        V2V_REQUIRE(kp.Cp == ain.C, V2V_ERR_STATE, "internal: conv of op %zu reads %d padded channels from a %d-channel buffer", i,
+                    kp.Cp, ain.C);
+        kp.io = P->io_dev;
+        if (op.kind == G_CONV) {
+          const Raw& r = P->raws[op.raw];
+          kp.epi = EPI_RAW_STATS; kp.out = r.desc.base; kp.out_C = r.desc.C; kp.out_f32 = r.desc.f32;
+          kp.stats = r.no_stats ? nullptr : r.stats; kp.stats_C = r.C; kp.bias = nullptr;
+        } else if (op.kind == G_CONV_ACT) {
+          const Value& vo = P->values[op.value_out];
+          V2V_REQUIRE(vo.bufs.size() == 1 && P->act_pad_mode[vo.bufs[0]] != PAD_REFLECT, V2V_ERR_UNSUPPORTED,
+                      "conv_act output needs a single zero/none-padded consumer layout");
+          kp.epi = EPI_ACT_BF16; kp.out_act = P->acts[vo.bufs[0]]; kp.out_C = kp.out_act.C;
+        }
+        conv_x[i] = (int)xops.size();
+        xops.push_back(x);
+        if (op.kind == G_CONV && P->impl == V2V_IMPL_SIMT) {
+          XOp s; s.kind = X_RAWSTATS; s.gop = (int)i;
+          s.rawd = P->raws[op.raw].desc; s.stats = P->raws[op.raw].stats; s.stats_C = P->raws[op.raw].C;
+          xops.push_back(s);
+        }
+        break;
+      }
+      case G_NORM_ACT: case G_RAWIN: {      // normalise passes (of a G_RAWIN: a plain conversion)
+        bool repeat = false;
+        if (op.kind == G_NORM_ACT) {
+          const Raw& r = P->raws[op.raw];
+          const GOp& cop = P->gops[r.conv_op];
+          const bool has_norm = op.norm.kind != V2V_NORM_NONE;
+          // a norm-less biased conv (FlowNet2's conv / deconv / predict_flow units) is normalised with scale 1 and shift =
+          // bias (finalize's bias affines), which cover the whole raw
+          V2V_REQUIRE(has_norm || cop.conv.bias == nullptr || (op.n_off == 0 && cop.conv.Cout2 == 0), V2V_ERR_UNSUPPORTED,
+                      "biased norm-less conv cannot be sliced");
+          std::vector<int>& rd = read[op.raw], &fd = fin[op.raw];
+          repeat = std::find(rd.begin(), rd.end(), op.n_off) != rd.end();
+          if (!repeat) rd.push_back(op.n_off);
+          if (has_norm && std::find(fd.begin(), fd.end(), op.n_off) == fd.end()) {
+            // the slice's first normalising pass finalises its statistics, with the side effects, once however many passes
+            // read it: in a tail slot of the producing tensor-core conv launch (the CTA that takes its last ticket,
+            // conv_umma.cu) while one is free, else in a stand-alone stats_finalize launch (the SIMT implementation, a third
+            // slice of one raw)
+            fd.push_back(op.n_off);
+            XOp f; f.kind = X_FINALIZE; f.gop = (int)i;
+            int rc = finalize_params(P, op, f.fin); if (rc) return rc;
+            ConvKernelParams& ckp = xops[conv_x[r.conv_op]].kp;
+            if (P->impl == V2V_IMPL_UMMA && ckp.n_fin < 2) {
+              xops[conv_x[r.conv_op]].fin_gop[ckp.n_fin] = (int)i;
+              ckp.fin[ckp.n_fin++] = f.fin;
+              ckp.fin_counter = arena_at<unsigned int>(P, P->raw_off[op.raw].stats + (size_t)r.N * 2 * r.C * sizeof(stat_t));
+            } else {
+              xops.push_back(f);
+            }
+          }
+        }
+        const Value& vo = P->values[op.value_out];
+        for (size_t m = 0; m < vo.bufs.size(); ++m) {
+          XOp a; a.kind = X_APPLY; a.gop = (int)i; a.buf = vo.bufs[m]; a.repeat = repeat; a.app = apply_params(P, op, m);
+          xops.push_back(a);
+        }
+        break;
+      }
+      case G_EXPORT: {
+        XOp x; x.kind = X_EXPORT; x.gop = (int)i; x.buf = P->values[op.value_in].bufs[0];
+        x.exp.io = P->io_dev; x.exp.slot = op.slot; x.exp.in = P->acts[x.buf];
+        xops.push_back(x);
+        break;
+      }
+      case G_COMPOSITE: {
+        XOp x; x.kind = X_COMPOSITE; x.gop = (int)i; x.comp = op.comp; x.comp.io = P->io_dev; x.comp.s_flags = P->flags_slot;
+        xops.push_back(x);
+        break;
+      }
+      case G_CONCAT: {
+        const Value& vo = P->values[op.value_out];
+        for (size_t m = 0; m < vo.bufs.size(); ++m) {
+          int c_off = 0;
+          for (int src : op.cat_in) {
+            XOp x; x.kind = X_COPY; x.gop = (int)i; x.buf = vo.bufs[m]; x.in_buf = P->values[src].bufs[0];
+            x.copy.in = P->acts[x.in_buf];
+            x.copy.out = P->acts[x.buf];
+            x.copy.c_off = c_off; x.copy.pad_mode = P->act_pad_mode[x.buf];
+            c_off += P->values[src].C;
+            xops.push_back(x);
+          }
+        }
+        break;
+      }
+      case G_MAXPOOL: {
+        const Value& vo = P->values[op.value_out];
+        for (size_t m = 0; m < vo.bufs.size(); ++m) {
+          V2V_REQUIRE(P->act_pad_mode[vo.bufs[m]] != PAD_REFLECT, V2V_ERR_UNSUPPORTED, "max-pool output needs a zero / no halo");
+          XOp x; x.kind = X_MAXPOOL; x.gop = (int)i;
+          x.pool.in = P->acts[P->values[op.value_in].bufs[0]]; x.pool.out = P->acts[vo.bufs[m]];
+          xops.push_back(x);
+        }
+        break;
+      }
+      case G_FEATL1: {
+        XOp x; x.kind = X_FEATL1; x.gop = (int)i;
+        x.fl1 = featl1_params(P, op);
+        x.fl1.partials = arena_at<double>(P, P->l1_off[i]);
+        xops.push_back(x);
+        break;
+      }
+      case G_CORR: {
+        const Value& va = P->values[op.value_in], &vb = P->values[op.value_in2], &vo = P->values[op.value_out];
+        const size_t bytes = (size_t)va.N * va.C * va.H * va.W * sizeof(float);
+        float* sa = arena_at<float>(P, P->corr_off[i]);
+        float* sb = arena_at<float>(P, P->corr_off[i] + bytes);
+        float* so = arena_at<float>(P, P->corr_off[i] + 2 * bytes);
+        XOp ea; ea.kind = X_EXPORT; ea.gop = (int)i; ea.buf = va.bufs[0];
+        ea.exp.io = P->io_dev; ea.exp.slot = 0; ea.exp.direct = sa; ea.exp.in = P->acts[va.bufs[0]];
+        XOp eb = ea; eb.buf = vb.bufs[0]; eb.exp.direct = sb; eb.exp.in = P->acts[vb.bufs[0]];
+        xops.push_back(ea); xops.push_back(eb);
+        XOp c; c.kind = X_CORR; c.gop = (int)i;
+        c.corr = CorrParams{sa, sb, so, va.N, va.C, va.H, va.W, op.corr[0], op.corr[1], op.corr[2], op.corr[3], op.corr[4]};
+        xops.push_back(c);
+        for (size_t m = 0; m < vo.bufs.size(); ++m) {
+          XOp x; x.kind = X_IMPORT; x.gop = (int)i; x.buf = vo.bufs[m];
+          x.imp.io = reinterpret_cast<const void* const*>(P->io_dev); x.imp.slot = 0; x.imp.direct = so;
+          x.imp.c_off = 0; x.imp.C_src = vo.C; x.imp.act = op.act; x.imp.slope = op.slope;
+          x.imp.out = P->acts[vo.bufs[m]]; x.imp.pad_mode = P->act_pad_mode[vo.bufs[m]];
+          xops.push_back(x);
+        }
+        break;
+      }
+    }
+  }
+  return 0;
+}
 
 // The arena layout of v2v_plan_describe (host-only: needs the arena sized): one "buffers" record per activation buffer (its byte
 // offset in the arena and the ActDesc fields that place element (n, c, y, x)), and one "scratch" record per correlation's fp32
 // scratch [in1 | in2 | out], each NCHW.  A caller that finalizes into its own workspace can decode every buffer from these.
-void describe_buffers(const v2v_plan* P, std::string& s) {
+static void describe_buffers(const v2v_plan* P, std::string& s) {
   char t[512];
   bool first = true;
   for (size_t v = 0; v < P->values.size(); ++v)
@@ -320,23 +470,34 @@ void describe_buffers(const v2v_plan* P, std::string& s) {
   }
 }
 
-static void describe_import(const v2v_plan* P, size_t i, int buf, int slot, int C_src, int c_off, int direct, int act, int skip_lo,
-                            std::string& s) {
-  const ActDesc& o = P->acts[buf];
+// The record writers of the forward launch list, one per launch kind.  An import or export of a correlation (direct) moves its
+// fp32 scratch instead of a caller tensor.
+static void describe_import(const v2v_plan* P, const XOp& x, std::string& s) {
+  const ImportParams& p = x.imp;
+  const ActDesc& o = p.out;
   char t[512];
   snprintf(t, sizeof(t),
-           "{\"kind\":\"import\",\"gop\":%zu,\"buf\":%d,\"slot\":%d,\"direct\":%d,\"C_src\":%d,\"c_off\":%d,\"act\":%d,\"pad_mode\":%d,"
+           "{\"kind\":\"import\",\"gop\":%d,\"buf\":%d,\"slot\":%d,\"direct\":%d,\"C_src\":%d,\"c_off\":%d,\"act\":%d,\"pad_mode\":%d,"
            "\"skip_lo\":%d,\"split\":%d,\"parity\":%d,\"N\":%d,\"H\":%d,\"W\":%d,\"C\":%d,\"Cvalid\":%d,\"Wpad\":%d,\"CT\":%d}",
-           i, buf, slot, direct, C_src, c_off, act, P->act_pad_mode[buf], skip_lo, o.split, o.parity, o.N, o.H, o.W, o.C, o.Cvalid,
-           o.W + o.pad_l + o.pad_r, import_tile_channels(o));
+           x.gop, x.buf, p.slot, P->gops[x.gop].kind == G_CORR, p.C_src, p.c_off, p.act, p.pad_mode, p.skip_lo, o.split, o.parity,
+           o.N, o.H, o.W, o.C, o.Cvalid, o.W + o.pad_l + o.pad_r, import_tile_channels(o));
   s += t;
 }
 
-static void describe_export(const v2v_plan* P, size_t i, int buf, int direct, std::string& s) {
-  const ActDesc& a = P->acts[buf];
+static void describe_export(const v2v_plan* P, const XOp& x, std::string& s) {
+  const ActDesc& a = x.exp.in;
   char t[320];
-  snprintf(t, sizeof(t), "{\"kind\":\"export\",\"gop\":%zu,\"buf\":%d,\"direct\":%d,\"split\":%d,\"N\":%d,\"H\":%d,\"W\":%d,\"C\":%d,\"Cvalid\":%d}",
-           i, buf, direct, a.split, a.N, a.H, a.W, a.C, a.Cvalid);
+  snprintf(t, sizeof(t), "{\"kind\":\"export\",\"gop\":%d,\"buf\":%d,\"direct\":%d,\"split\":%d,\"N\":%d,\"H\":%d,\"W\":%d,\"C\":%d,\"Cvalid\":%d}",
+           x.gop, x.buf, P->gops[x.gop].kind == G_CORR, a.split, a.N, a.H, a.W, a.C, a.Cvalid);
+  s += t;
+}
+
+static void describe_copy(const XOp& x, std::string& s) {
+  const CopyParams& p = x.copy;
+  char t[320];
+  snprintf(t, sizeof(t), "{\"kind\":\"copy\",\"gop\":%d,\"in_buf\":%d,\"buf\":%d,\"c_off\":%d,\"Cvalid\":%d,\"pad_mode\":%d,"
+           "\"in_split\":%d,\"split\":%d,\"parity\":%d}",
+           x.gop, x.in_buf, x.buf, p.c_off, p.in.Cvalid, p.pad_mode, p.in.split, p.out.split, p.out.parity);
   s += t;
 }
 
@@ -348,46 +509,79 @@ static void describe_grad_layout(const char* kind, size_t i, const Value& v, int
   s += t;
 }
 
-// The "layout" records of v2v_plan_describe, in the order finalize emits the launches: every import (caller tensor or
-// correlation scratch), export, concat copy and weight pack, with the fields that select its code path.  Training plans add
-// the gradient import of every export and the gradient export of every input (assuming the caller passes both gradients),
-// and per tensor-core backward unit its fold, dgrad pack and unstage (describe_backward_layout).
-void describe_layout(const v2v_plan* P, std::string& s) {
-  char t[320];
+static const char* kFinSite[] = {"tail0", "tail1", "standalone"};
+struct FinRecord { int gop, site; const FinalizeParams* fp; };
+
+// stats: how conv_umma_kernel accumulates the statistics rows of a conv whose raw a norm layer reads (async_epi, MG, BN,
+// phases, units over ctas persistent CTAs) or raw_stats_kernel (SIMT), and where each of its slices is finalised
+static void describe_stats(const v2v_plan* P, const XOp& x, const std::string& sites, std::string& s) {
+  const GOp& op = P->gops[x.gop];
+  const Raw& r = P->raws[op.raw];
+  const ConvKernelParams& kp = x.kp;
+  char t[512];
+  snprintf(t, sizeof(t),
+           "{\"kind\":\"stats\",\"gop\":%d,\"raw\":%d,\"N\":%d,\"C\":%d,\"H\":%d,\"W\":%d,\"raw_f32\":%d,\"impl\":\"%s\","
+           "\"async_epi\":%d,\"MG\":%d,\"BN\":%d,\"phases\":%d,\"n_tiles\":%d,\"m_total\":%d,\"units\":%d,\"ctas\":%d,\"fin\":[",
+           x.gop, op.raw, r.N, r.C, r.H, r.W, r.desc.f32, P->impl == V2V_IMPL_UMMA ? "umma" : "simt", conv_umma_async_epilogue(kp),
+           kp.MG, kp.BN, kp.num_phases, kp.n_tiles, kp.m_total, kp.total_units, kp.grid);
+  s += t + sites + "]}";
+}
+
+// finalize: batch / instance / per-sample statistics, image flags, running buffers, conv bias, the saved mean / rstd of training
+// plans, the slice
+static void describe_finalize(const v2v_plan* P, const FinRecord& f, std::string& s) {
+  const FinalizeParams& fp = *f.fp;
+  char t[512];
+  snprintf(t, sizeof(t),
+           "{\"kind\":\"finalize\",\"gop\":%d,\"raw\":%d,\"site\":\"%s\",\"stats\":\"%s\",\"N\":%d,\"flags\":%d,"
+           "\"running\":%d,\"bias\":%d,\"mean_rstd\":%d,\"c_off\":%d,\"C\":%d}",
+           f.gop, P->gops[f.gop].raw, kFinSite[f.site], fp.sample_running ? "sample" : (fp.instance ? "instance" : "batch"), fp.N,
+           fp.flags_slot >= 0, fp.running_mean != nullptr, fp.conv_bias != nullptr, P->train ? 1 : 0, fp.c_off, fp.C);
+  s += t;
+}
+
+// apply: the norm_apply_launch choice of one normalise pass into one output layout, and what the kernel reads and writes
+static void describe_apply(const v2v_plan* P, const XOp& x, std::string& s) {
+  const GOp& op = P->gops[x.gop];
+  const std::vector<int>& bufs = P->values[op.value_out].bufs;
+  const size_t layout = std::find(bufs.begin(), bufs.end(), x.buf) - bufs.begin();
+  const char* scale = op.kind == G_RAWIN ? "none" : (op.norm.kind != V2V_NORM_NONE ? "norm" :
+                      (P->gops[P->raws[op.raw].conv_op].conv.bias != nullptr ? "bias" : "none"));
+  const ApplyParams& ap = x.app;
+  const NormApplyLaunch l = norm_apply_launch(ap);
+  const ActDesc& o = ap.out;
+  const int Wpad = o.W + o.pad_l + o.pad_r;
+  char t[768];
+  snprintf(t, sizeof(t),
+           "{\"kind\":\"apply\",\"gop\":%d,\"op\":\"%s\",\"raw\":%d,\"layout\":%zu,\"repeat\":%d,\"kernel\":\"%s\",\"prec\":%d,"
+           "\"nadd\":%d,\"vecs\":%d,\"ppb\":%d,\"xt\":%d,\"grid\":[%d,%d],\"idle\":%d,\"ragged\":%d,\"N\":%d,\"H\":%d,"
+           "\"W\":%d,\"C\":%d,\"Cvalid\":%d,\"raw_C\":%d,\"c_off\":%d,\"pad_mode\":%d,\"pads\":[%d,%d,%d,%d],\"parity\":%d,"
+           "\"split\":%d,\"scale\":\"%s\",\"act\":%d,\"adds\":[",
+           x.gop, op.kind == G_RAWIN ? "rawin" : "norm_act", op.raw, layout, x.repeat ? 1 : 0, l.rows ? "rows" : "grid_stride",
+           ap.raw.f32, ap.n_add, l.vecs, l.ppb, l.xt, l.grid[0], l.grid[1], l.rows && 256 % l.vecs != 0,
+           l.rows && Wpad % l.xt != 0, o.N, o.H, o.W, o.C, ap.raw.Cvalid, ap.raw.C, op.kind == G_RAWIN ? 0 : op.n_off,
+           ap.pad_mode, o.pad_t, o.pad_l, o.pad_b, o.pad_r, o.parity, o.split, scale, ap.act);
+  s += t;
+  for (int a = 0; a < ap.n_add; ++a) {
+    snprintf(t, sizeof(t), "%s{\"parity\":%d,\"split\":%d,\"C\":%d}", a ? "," : "", ap.add[a].parity, ap.add[a].split, ap.add[a].C);
+    s += t;
+  }
+  s += "]}";
+}
+
+// The "layout" records of v2v_plan_describe, in launch order: every import (caller tensor or correlation scratch), export,
+// concat copy and the weight pack of every conv launch, with the fields that select its code path.  Training plans add the
+// gradient import of every export and the gradient export of every input (assuming the caller passes both gradients), and per
+// tensor-core backward unit its fold, dgrad pack and unstage (describe_backward_layout).
+static void describe_layout(const v2v_plan* P, const std::vector<XOp>& xops, std::string& s) {
   bool first = true;
   auto sep = [&]() { if (!first) s += ","; first = false; };
-  for (size_t i = 0; i < P->gops.size(); ++i) {
-    const GOp& op = P->gops[i];
-    switch (op.kind) {
-      case G_INPUT: {
-        const Value& v = P->values[op.value_out];
-        for (int b : v.bufs) { sep(); describe_import(P, i, b, op.slot, op.C_src, op.c_off, 0, ACT_NONE, v.exact_bf16 ? 1 : 0, s); }
-        break;
-      }
-      case G_CONV: case G_CONV_ACT: case G_HEAD: sep(); describe_pack(P, i, s); break;
-      case G_EXPORT: sep(); describe_export(P, i, P->values[op.value_in].bufs[0], 0, s); break;
-      case G_CONCAT: {
-        for (int b : P->values[op.value_out].bufs) {
-          int c_off = 0;
-          for (int src : op.cat_in) {
-            const ActDesc& a = P->acts[P->values[src].bufs[0]], &o = P->acts[b];
-            sep();
-            snprintf(t, sizeof(t), "{\"kind\":\"copy\",\"gop\":%zu,\"in_buf\":%d,\"buf\":%d,\"c_off\":%d,\"Cvalid\":%d,\"pad_mode\":%d,"
-                     "\"in_split\":%d,\"split\":%d,\"parity\":%d}",
-                     i, P->values[src].bufs[0], b, c_off, a.Cvalid, P->act_pad_mode[b], a.split, o.split, o.parity);
-            s += t;
-            c_off += P->values[src].C;
-          }
-        }
-        break;
-      }
-      case G_CORR: {
-        sep(); describe_export(P, i, P->values[op.value_in].bufs[0], 1, s);
-        sep(); describe_export(P, i, P->values[op.value_in2].bufs[0], 1, s);
-        const Value& vo = P->values[op.value_out];
-        for (int b : vo.bufs) { sep(); describe_import(P, i, b, 0, vo.C, 0, 1, op.act, 0, s); }
-        break;
-      }
+  for (const XOp& x : xops) {
+    switch (x.kind) {
+      case X_IMPORT: sep(); describe_import(P, x, s); break;
+      case X_CONV: sep(); describe_pack(P, x.gop, s); break;
+      case X_EXPORT: sep(); describe_export(P, x, s); break;
+      case X_COPY: sep(); describe_copy(x, s); break;
       default: break;
     }
   }
@@ -400,90 +594,28 @@ void describe_layout(const v2v_plan* P, std::string& s) {
   }
 }
 
-// The forward epilogue of the plan's norm layers, as finalize emits it (the same host functions choose it), three kinds of
-// record:
-//   stats     one per conv whose raw a norm layer reads: how conv_umma_kernel accumulates the statistics rows (async_epi, MG,
-//             BN, phases, units over ctas persistent CTAs) or raw_stats_kernel (SIMT), and where each slice is finalised;
-//   finalize  one per (raw, slice): batch / instance / per-sample statistics, image flags, running buffers, conv bias, the
-//             saved mean / rstd of training plans, the slice;
-//   apply     one per normalise pass and output layout: the norm_apply_launch choice and what the kernel reads and writes.
-void describe_epilogue_forward(v2v_plan* P, std::string& s) {
-  static const char* kSite[] = {"tail0", "tail1", "standalone"};
-  const std::vector<int> site = finalize_sites(P);
-  std::vector<std::vector<int>> slices(P->raws.size());      // per raw: finalising ops, in order
-  for (size_t i = 0; i < P->gops.size(); ++i) if (site[i] >= 0) slices[P->gops[i].raw].push_back((int)i);
-  char t[768];
+// The "epilogue_forward" records of v2v_plan_describe: every stats record (in launch order), every finalize record (in the
+// order of the passes they serve) and every apply record (in launch order).
+static void describe_epilogue_forward(const v2v_plan* P, const std::vector<XOp>& xops, std::string& s) {
+  std::vector<FinRecord> fins;
+  for (const XOp& x : xops) {
+    if (x.kind == X_CONV) for (int q = 0; q < x.kp.n_fin; ++q) fins.push_back({x.fin_gop[q], q, &x.kp.fin[q]});
+    if (x.kind == X_FINALIZE) fins.push_back({x.gop, 2, &x.fin});
+  }
+  std::sort(fins.begin(), fins.end(), [](const FinRecord& a, const FinRecord& b) { return a.gop < b.gop; });
+  std::vector<std::string> sites(P->raws.size());      // per raw: the sites of its slices, as its stats record lists them
+  for (const FinRecord& f : fins) {
+    std::string& l = sites[P->gops[f.gop].raw];
+    l += std::string(l.empty() ? "\"" : ",\"") + kFinSite[f.site] + "\"";
+  }
   bool first = true;
   auto sep = [&]() { if (!first) s += ","; first = false; };
-  for (size_t i = 0; i < P->gops.size(); ++i) {
-    const GOp& op = P->gops[i];
-    if (op.kind != G_CONV || slices[op.raw].empty()) continue;
-    const Raw& r = P->raws[op.raw];
-    GOp tmp = op;
-    fill_conv_params(P, tmp);
-    const ConvKernelParams& kp = tmp.kp;
-    sep();
-    snprintf(t, sizeof(t),
-             "{\"kind\":\"stats\",\"gop\":%zu,\"raw\":%d,\"N\":%d,\"C\":%d,\"H\":%d,\"W\":%d,\"raw_f32\":%d,\"impl\":\"%s\","
-             "\"async_epi\":%d,\"MG\":%d,\"BN\":%d,\"phases\":%d,\"n_tiles\":%d,\"m_total\":%d,\"units\":%d,\"ctas\":%d,\"fin\":[",
-             i, op.raw, r.N, r.C, r.H, r.W, r.desc.f32, P->impl == V2V_IMPL_UMMA ? "umma" : "simt", conv_umma_async_epilogue(kp),
-             kp.MG, kp.BN, kp.num_phases, kp.n_tiles, kp.m_total, kp.total_units, kp.grid);
-    s += t;
-    for (size_t k = 0; k < slices[op.raw].size(); ++k) {
-      snprintf(t, sizeof(t), "%s\"%s\"", k ? "," : "", kSite[site[slices[op.raw][k]]]);
-      s += t;
-    }
-    s += "]}";
+  for (const XOp& x : xops) {
+    if (x.kind != X_CONV || P->gops[x.gop].kind != G_CONV || sites[P->gops[x.gop].raw].empty()) continue;
+    sep(); describe_stats(P, x, sites[P->gops[x.gop].raw], s);
   }
-  for (size_t i = 0; i < P->gops.size(); ++i) {
-    if (site[i] < 0) continue;
-    const GOp& op = P->gops[i];
-    FinalizeParams fp{};
-    finalize_params(P, op, fp);
-    sep();
-    snprintf(t, sizeof(t),
-             "{\"kind\":\"finalize\",\"gop\":%zu,\"raw\":%d,\"site\":\"%s\",\"stats\":\"%s\",\"N\":%d,\"flags\":%d,"
-             "\"running\":%d,\"bias\":%d,\"mean_rstd\":%d,\"c_off\":%d,\"C\":%d}",
-             i, op.raw, kSite[site[i]], fp.sample_running ? "sample" : (fp.instance ? "instance" : "batch"), fp.N,
-             fp.flags_slot >= 0, fp.running_mean != nullptr, fp.conv_bias != nullptr, P->train ? 1 : 0, fp.c_off, fp.C);
-    s += t;
-  }
-  std::vector<std::pair<int, int>> read;                     // (raw, slice) pairs an earlier normalise pass has read
-  for (size_t i = 0; i < P->gops.size(); ++i) {
-    const GOp& op = P->gops[i];
-    if (op.kind != G_NORM_ACT && op.kind != G_RAWIN) continue;
-    bool repeat = false;
-    if (op.kind == G_NORM_ACT) {
-      const std::pair<int, int> key(op.raw, op.n_off);
-      repeat = std::find(read.begin(), read.end(), key) != read.end();
-      if (!repeat) read.push_back(key);
-    }
-    const char* scale = op.kind == G_RAWIN ? "none" : (op.norm.kind != V2V_NORM_NONE ? "norm" :
-                        (P->gops[P->raws[op.raw].conv_op].conv.bias != nullptr ? "bias" : "none"));
-    const Value& vo = P->values[op.value_out];
-    for (size_t m = 0; m < vo.bufs.size(); ++m) {
-      const ApplyParams ap = apply_params(P, op, m);
-      const NormApplyLaunch l = norm_apply_launch(ap);
-      const ActDesc& o = ap.out;
-      const int Wpad = o.W + o.pad_l + o.pad_r;
-      sep();
-      snprintf(t, sizeof(t),
-               "{\"kind\":\"apply\",\"gop\":%zu,\"op\":\"%s\",\"raw\":%d,\"layout\":%zu,\"repeat\":%d,\"kernel\":\"%s\",\"prec\":%d,"
-               "\"nadd\":%d,\"vecs\":%d,\"ppb\":%d,\"xt\":%d,\"grid\":[%d,%d],\"idle\":%d,\"ragged\":%d,\"N\":%d,\"H\":%d,"
-               "\"W\":%d,\"C\":%d,\"Cvalid\":%d,\"raw_C\":%d,\"c_off\":%d,\"pad_mode\":%d,\"pads\":[%d,%d,%d,%d],\"parity\":%d,"
-               "\"split\":%d,\"scale\":\"%s\",\"act\":%d,\"adds\":[",
-               i, op.kind == G_RAWIN ? "rawin" : "norm_act", op.raw, m, repeat ? 1 : 0, l.rows ? "rows" : "grid_stride",
-               ap.raw.f32, ap.n_add, l.vecs, l.ppb, l.xt, l.grid[0], l.grid[1], l.rows && 256 % l.vecs != 0,
-               l.rows && Wpad % l.xt != 0, o.N, o.H, o.W, o.C, ap.raw.Cvalid, ap.raw.C, op.kind == G_RAWIN ? 0 : op.n_off,
-               ap.pad_mode, o.pad_t, o.pad_l, o.pad_b, o.pad_r, o.parity, o.split, scale, ap.act);
-      s += t;
-      for (int a = 0; a < ap.n_add; ++a) {
-        snprintf(t, sizeof(t), "%s{\"parity\":%d,\"split\":%d,\"C\":%d}", a ? "," : "", ap.add[a].parity, ap.add[a].split, ap.add[a].C);
-        s += t;
-      }
-      s += "]}";
-    }
-  }
+  for (const FinRecord& f : fins) { sep(); describe_finalize(P, f, s); }
+  for (const XOp& x : xops) if (x.kind == X_APPLY) { sep(); describe_apply(P, x, s); }
 }
 
 }  // namespace v2v
@@ -754,11 +886,7 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
   V2V_REQUIRE(P && !P->finalized, V2V_ERR_STATE, "plan null or already finalized");
   int rc = size_arena(P); if (rc) return rc;
   DeviceGuard guard(P->device);
-  const std::vector<size_t>& act_off = P->act_off;
-  const std::vector<v2v_plan::RawOff>& raw_off = P->raw_off;
-  const std::vector<size_t>& w_off = P->w_off;
-  const std::vector<size_t>& corr_off = P->corr_off;
-  const size_t stats_begin = P->stats_begin, stats_end = P->stats_end;
+  // ---- allocate
   if (workspace) {
     // caller-owned arena (v2v_plan_workspace_bytes before this call): not freed by v2v_plan_destroy
     V2V_REQUIRE(workspace_bytes >= P->arena_bytes && (reinterpret_cast<uintptr_t>(workspace) & 1023) == 0, V2V_ERR_INVALID,
@@ -769,17 +897,7 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
   }
   V2V_CUDA(cudaMemsetAsync(P->arena, 0, P->arena_bytes, stream));
   V2V_CUDA(cudaMalloc(reinterpret_cast<void**>(&P->io_dev), sizeof(void*) * std::max(1, P->n_slots)));
-  uint8_t* base = reinterpret_cast<uint8_t*>(P->arena);
-  for (size_t i = 0; i < P->acts.size(); ++i) P->acts[i].base = reinterpret_cast<bf16*>(base + act_off[i]);
-  for (size_t i = 0; i < P->raws.size(); ++i) {
-    Raw& r = P->raws[i];
-    r.desc.base = base + raw_off[i].raw;
-    r.stats = reinterpret_cast<stat_t*>(base + raw_off[i].stats);
-    r.scale = reinterpret_cast<float*>(base + raw_off[i].scale);
-    r.shift = reinterpret_cast<float*>(base + raw_off[i].shift);
-  }
-
-  if (P->train) {                       // saved batch statistics (the finalize launches below write them)
+  if (P->train) {                       // saved batch statistics (the finalize launches write them)
     size_t tot = 0;
     for (auto& r : P->raws) tot += 2 * (size_t)r.N * r.C;
     float* st = nullptr;
@@ -788,172 +906,39 @@ static int finalize_impl(v2v_plan* P, void* workspace, size_t workspace_bytes, c
     P->train_stats = st;
     for (auto& r : P->raws) { r.mean = st; st += (size_t)r.N * r.C; r.rstd = st; st += (size_t)r.N * r.C; }
   }
-  // ---- emit executable ops
-  if (stats_end > stats_begin) {
-    XOp m; m.kind = X_MEMSET; m.ms_ptr = base + stats_begin; m.ms_bytes = stats_end - stats_begin;
-    P->xops.push_back(m);
+  // ---- bind: the arena addresses of the buffers the launches and the backward read
+  for (size_t i = 0; i < P->acts.size(); ++i) P->acts[i].base = arena_at<bf16>(P, P->act_off[i]);
+  for (size_t i = 0; i < P->raws.size(); ++i) {
+    Raw& r = P->raws[i];
+    r.desc.base = arena_at<void>(P, P->raw_off[i].raw);
+    r.stats = arena_at<stat_t>(P, P->raw_off[i].stats);
+    r.scale = arena_at<float>(P, P->raw_off[i].scale);
+    r.shift = arena_at<float>(P, P->raw_off[i].shift);
   }
-  const std::vector<int> fin_site = finalize_sites(P);
-  for (size_t i = 0; i < P->gops.size(); ++i) {
-    GOp& op = P->gops[i];
-    switch (op.kind) {
-      case G_INPUT: {
-        const Value& v = P->values[op.value_out];
-        for (size_t m = 0; m < v.bufs.size(); ++m) {
-          XOp x; x.kind = X_IMPORT; x.gop = (int)i;
-          x.imp.io = reinterpret_cast<const void* const*>(P->io_dev); x.imp.slot = op.slot;
-          x.imp.c_off = op.c_off; x.imp.C_src = op.C_src;
-          x.imp.out = P->acts[v.bufs[m]]; x.imp.pad_mode = P->act_pad_mode[v.bufs[m]];
-          x.imp.skip_lo = v.exact_bf16 ? 1 : 0;
-          P->xops.push_back(x);
-        }
-        break;
-      }
-      case G_CONV: case G_CONV_ACT: case G_HEAD: {
-        const Value& vin = P->values[op.value_in];
-        const ActDesc& ain = P->acts[vin.bufs[op.req_index]];
-        op.wpacked = reinterpret_cast<bf16*>(base + w_off[i]);
-        ConvKernelParams& kp = op.kp;
-        // the kernel addresses the lo half of the input at channel coordinate Cp: the buffer must be padded to exactly that
-        V2V_REQUIRE(kp.Cp == ain.C, V2V_ERR_STATE, "internal: conv of op %zu reads %d padded channels from a %d-channel buffer", i,
-                    kp.Cp, ain.C);
-        kp.io = P->io_dev;
-        if (op.kind == G_CONV) {
-          Raw& r = P->raws[op.raw];
-          kp.epi = EPI_RAW_STATS; kp.out = r.desc.base; kp.out_C = r.desc.C; kp.out_f32 = r.desc.f32;
-          kp.stats = r.no_stats ? nullptr : r.stats; kp.stats_C = r.C; kp.bias = nullptr;
-        } else if (op.kind == G_CONV_ACT) {
-          const Value& vo = P->values[op.value_out];
-          V2V_REQUIRE(vo.bufs.size() == 1 && P->act_pad_mode[vo.bufs[0]] != PAD_REFLECT, V2V_ERR_UNSUPPORTED,
-                      "conv_act output needs a single zero/none-padded consumer layout");
-          kp.epi = EPI_ACT_BF16; kp.out_act = P->acts[vo.bufs[0]]; kp.out_C = kp.out_act.C;
-        } else {
-          kp.epi = EPI_HEAD_F32;
-          kp.bias2 = op.conv.Cout2 > 0 ? op.conv.bias2 : nullptr; kp.Cout1 = op.conv.Cout - op.conv.Cout2;
-          for (int j = 0; j < op.conv.Cout; ++j) {
-            kp.head_slot[j] = op.head[j].slot;
-            kp.head_off[j] = (long long)op.head[j].channel * op.geom.out_h * op.geom.out_w;
-            kp.head_bstride[j] = (long long)op.head[j].dst_C * op.geom.out_h * op.geom.out_w;
-            kp.head_act[j] = op.head[j].act; kp.head_scale[j] = op.head[j].scale;
-          }
-        }
-        if (P->impl == V2V_IMPL_UMMA) {
-          rc = make_tmap_act(&op.tmA, ain, kp.PW, kp.PH, kp.kc); if (rc) return rc;
-          rc = make_tmap_w(&op.tmB, op.wpacked, P->sp() * op.Ktotal, op.geom.headkx ? op.geom.headkx * op.conv.Cout : op.conv.Cout, kp.BN,
-                           kp.kc); if (rc) return rc;
-        }
-        rc = pack_one(op, stream); if (rc) return rc;
-        XOp x; x.kind = X_CONV; x.gop = (int)i;
-        P->xops.push_back(x);
-        if (op.kind == G_CONV && P->impl == V2V_IMPL_SIMT) {
-          XOp s; s.kind = X_RAWSTATS; s.rawd = P->raws[op.raw].desc; s.stats = P->raws[op.raw].stats; s.stats_C = P->raws[op.raw].C;
-          P->xops.push_back(s);
-        }
-        break;
-      }
-      case G_NORM_ACT: {
-        Raw& r = P->raws[op.raw];
-        const GOp& cop = P->gops[r.conv_op];
-        const bool has_norm = op.norm.kind != V2V_NORM_NONE;
-        if (!has_norm && cop.conv.bias != nullptr) {
-          // norm-less biased conv (FlowNet2's conv / deconv / predict_flow units): the normalise pass runs with scale 1 and
-          // shift = bias, written here and after every repack
-          V2V_REQUIRE(op.n_off == 0 && cop.conv.Cout2 == 0, V2V_ERR_UNSUPPORTED, "biased norm-less conv cannot be sliced");
-          v2v_plan::BiasAffine ba{r.scale, r.shift, cop.conv.bias, r.N, r.C, r.C};
-          P->bias_affines.push_back(ba);
-          V2V_CUDA(launch_bias_affine(ba.scale, ba.shift, ba.bias, ba.N, ba.C, ba.stride, stream));
-        }
-        const Value& vo = P->values[op.value_out];
-        for (size_t m = 0; m < vo.bufs.size(); ++m) {
-          if (m == 0 && fin_site[i] >= 0) {
-            FinalizeParams side{};
-            rc = finalize_params(P, op, side); if (rc) return rc;
-            if (fin_site[i] < 2) {
-              GOp& prod = P->gops[r.conv_op];
-              prod.kp.fin[fin_site[i]] = side;
-              prod.kp.n_fin = fin_site[i] + 1;
-              prod.kp.fin_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<uint8_t*>(r.stats) + (size_t)r.N * 2 * r.C * sizeof(stat_t));
-            } else {
-              XOp f; f.kind = X_FINALIZE; f.fin = side; P->xops.push_back(f);
-            }
-          }
-          XOp a; a.kind = X_APPLY; a.app = apply_params(P, op, m);
-          P->xops.push_back(a);
-        }
-        break;
-      }
-      case G_RAWIN: {
-        const Value& vo = P->values[op.value_out];
-        for (size_t m = 0; m < vo.bufs.size(); ++m) {
-          XOp a; a.kind = X_APPLY; a.app = apply_params(P, op, m);
-          P->xops.push_back(a);
-        }
-        break;
-      }
-      case G_EXPORT: {
-        XOp x; x.kind = X_EXPORT; x.exp.io = P->io_dev; x.exp.slot = op.slot; x.exp.in = P->acts[P->values[op.value_in].bufs[0]];
-        P->xops.push_back(x);
-        break;
-      }
-      case G_COMPOSITE: {
-        XOp x; x.kind = X_COMPOSITE; x.comp = op.comp; x.comp.io = P->io_dev; x.comp.s_flags = P->flags_slot;
-        P->xops.push_back(x);
-        break;
-      }
-      case G_CONCAT: {
-        const Value& vo = P->values[op.value_out];
-        for (size_t m = 0; m < vo.bufs.size(); ++m) {
-          int c_off = 0;
-          for (int src : op.cat_in) {
-            XOp x; x.kind = X_COPY;
-            x.copy.in = P->acts[P->values[src].bufs[0]];
-            x.copy.out = P->acts[vo.bufs[m]];
-            x.copy.c_off = c_off; x.copy.pad_mode = P->act_pad_mode[vo.bufs[m]];
-            c_off += P->values[src].C;
-            P->xops.push_back(x);
-          }
-        }
-        break;
-      }
-      case G_MAXPOOL: {
-        const Value& vo = P->values[op.value_out];
-        for (size_t m = 0; m < vo.bufs.size(); ++m) {
-          V2V_REQUIRE(P->act_pad_mode[vo.bufs[m]] != PAD_REFLECT, V2V_ERR_UNSUPPORTED, "max-pool output needs a zero / no halo");
-          XOp x; x.kind = X_MAXPOOL; x.gop = (int)i;
-          x.pool.in = P->acts[P->values[op.value_in].bufs[0]]; x.pool.out = P->acts[vo.bufs[m]];
-          P->xops.push_back(x);
-        }
-        break;
-      }
-      case G_FEATL1: {
-        XOp x; x.kind = X_FEATL1; x.gop = (int)i;
-        x.fl1 = featl1_params(P, op);
-        x.fl1.partials = reinterpret_cast<double*>(base + P->l1_off[i]);
-        P->xops.push_back(x);
-        break;
-      }
-      case G_CORR: {
-        const Value& va = P->values[op.value_in], &vb = P->values[op.value_in2], &vo = P->values[op.value_out];
-        float* sa = reinterpret_cast<float*>(base + corr_off[i]);
-        float* sb = sa + (size_t)va.N * va.C * va.H * va.W;
-        float* so = sb + (size_t)va.N * va.C * va.H * va.W;
-        XOp ea; ea.kind = X_EXPORT; ea.exp.io = P->io_dev; ea.exp.slot = 0; ea.exp.direct = sa; ea.exp.in = P->acts[va.bufs[0]];
-        XOp eb = ea; eb.exp.direct = sb; eb.exp.in = P->acts[vb.bufs[0]];
-        P->xops.push_back(ea); P->xops.push_back(eb);
-        XOp c; c.kind = X_CORR;
-        c.corr = CorrParams{sa, sb, so, va.N, va.C, va.H, va.W, op.corr[0], op.corr[1], op.corr[2], op.corr[3], op.corr[4]};
-        P->xops.push_back(c);
-        for (size_t m = 0; m < vo.bufs.size(); ++m) {
-          XOp x; x.kind = X_IMPORT; x.gop = (int)i;
-          x.imp.io = reinterpret_cast<const void* const*>(P->io_dev); x.imp.slot = 0; x.imp.direct = so;
-          x.imp.c_off = 0; x.imp.C_src = vo.C; x.imp.act = op.act; x.imp.slope = op.slope;
-          x.imp.out = P->acts[vo.bufs[m]]; x.imp.pad_mode = P->act_pad_mode[vo.bufs[m]];
-          P->xops.push_back(x);
-        }
-        break;
-      }
+  // ---- emit
+  rc = emit_forward(P, P->xops); if (rc) return rc;
+  // ---- device work: every conv launch's packed weights and tensor maps
+  for (const XOp& x : P->xops) {
+    if (x.kind != X_CONV) continue;
+    GOp& op = P->gops[x.gop];
+    op.wpacked = arena_at<bf16>(P, P->w_off[x.gop]);
+    if (P->impl == V2V_IMPL_UMMA) {
+      const ActDesc& ain = P->acts[P->values[op.value_in].bufs[op.req_index]];
+      rc = make_tmap_act(&op.tmA, ain, x.kp.PW, x.kp.PH, x.kp.kc); if (rc) return rc;
+      rc = make_tmap_w(&op.tmB, op.wpacked, P->sp() * op.Ktotal, op.geom.headkx ? op.geom.headkx * op.conv.Cout : op.conv.Cout,
+                       x.kp.BN, x.kp.kc); if (rc) return rc;
     }
+    rc = pack_one(op, stream); if (rc) return rc;
   }
+  // a norm-less biased conv (FlowNet2's conv / deconv / predict_flow units) is normalised with scale 1 and shift = bias, written
+  // here and after every repack
+  for (const GOp& op : P->gops) {
+    if (op.kind != G_NORM_ACT || op.norm.kind != V2V_NORM_NONE) continue;
+    const Raw& r = P->raws[op.raw];
+    const float* bias = P->gops[r.conv_op].conv.bias;
+    if (bias) P->bias_affines.push_back(v2v_plan::BiasAffine{r.scale, r.shift, bias, r.N, r.C, r.C});
+  }
+  for (const auto& ba : P->bias_affines) V2V_CUDA(launch_bias_affine(ba.scale, ba.shift, ba.bias, ba.N, ba.C, ba.stride, stream));
   if (P->train) {
     rc = alloc_training(P, stream); if (rc) return rc;
     rc = build_backward_units(P, stream); if (rc) return rc;
@@ -993,6 +978,14 @@ static int check_composite_alignment(const v2v_plan* P, void* const* io_ptrs) {
   return 0;
 }
 
+// A launch without the running-statistics updates of its finalisations (stand-alone, or in a conv launch's tail).
+static XOp without_running_stats(XOp x) {
+  auto strip = [](FinalizeParams& f) { f.running_mean = nullptr; f.running_var = nullptr; f.num_batches_tracked = nullptr; };
+  if (x.kind == X_FINALIZE) strip(x.fin);
+  if (x.kind == X_CONV) for (int q = 0; q < x.kp.n_fin; ++q) strip(x.kp.fin[q]);
+  return x;
+}
+
 int v2v_plan_run(v2v_plan* P, void* const* io_ptrs, int n_io, int use_graph, v2v_stream_t stream_) {
   V2V_REQUIRE(P && P->finalized, V2V_ERR_STATE, "plan not finalized");
   V2V_REQUIRE(n_io >= P->n_slots && io_ptrs, V2V_ERR_INVALID, "need %d io pointers, got %d", P->n_slots, n_io);
@@ -1001,17 +994,7 @@ int v2v_plan_run(v2v_plan* P, void* const* io_ptrs, int n_io, int use_graph, v2v
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   V2V_CUDA(cudaMemcpyAsync(P->io_dev, io_ptrs, sizeof(void*) * P->n_slots, cudaMemcpyHostToDevice, stream));
   if (use_graph & 2) {        // recomputation before a backward: same results, no running-statistics side effect
-    for (const XOp& x : P->xops) {
-      if (x.kind == X_FINALIZE) {
-        XOp y = x; y.fin.running_mean = nullptr; y.fin.running_var = nullptr; y.fin.num_batches_tracked = nullptr;
-        int rc = run_xop(P, y, stream); if (rc) return rc;
-      } else if (x.kind == X_CONV && P->impl == V2V_IMPL_UMMA && P->gops[x.gop].kp.n_fin > 0) {
-        const GOp& op = P->gops[x.gop];
-        ConvKernelParams kp = op.kp;
-        for (int q = 0; q < kp.n_fin; ++q) { kp.fin[q].running_mean = nullptr; kp.fin[q].running_var = nullptr; kp.fin[q].num_batches_tracked = nullptr; }
-        V2V_CUDA(launch_conv_umma(op.tmA, op.tmB, kp, stream));
-      } else { int rc = run_xop(P, x, stream); if (rc) return rc; }
-    }
+    for (const XOp& x : P->xops) { int rc = run_xop(P, without_running_stats(x), stream); if (rc) return rc; }
     return 0;
   }
   if (!use_graph) {
@@ -1085,7 +1068,10 @@ extern "C" {
 int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
   v2v_plan* P = const_cast<v2v_plan*>(P_);
   if (!P) return 0;
-  if (!P->lowered && lower(P)) return -1;
+  if (!P->sized && size_arena(P)) return -1;          // lowers the graph and chooses every conv's kernel parameters
+  std::vector<XOp> emitted;                           // an unfinalized plan: the launch list finalize would run
+  if (!P->finalized && emit_forward(P, emitted)) return -1;
+  const std::vector<XOp>& xops = P->finalized ? P->xops : emitted;
   std::string s = "{\"values\":[";
   std::string bwd_layout;            // training plans: the backward units' layout records, appended to "layout"
   char t[512];
@@ -1132,16 +1118,14 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
       }
     }
     s += "],\"epilogue_backward\":[";
-    if (!P->sized && size_arena(P)) return -1;        // the raw tensors' element type and channel stride (host-only)
     describe_epilogue_backward(P, s);
   }
   s += "],\"epilogue_forward\":[";
-  if (!P->sized && size_arena(P)) return -1;          // the raw tensors' element type and channel stride (host-only)
-  describe_epilogue_forward(P, s);
+  describe_epilogue_forward(P, xops, s);
   s += "],\"buffers\":[";
   describe_buffers(P, s);
   s += "],\"layout\":[";
-  describe_layout(P, s);
+  describe_layout(P, xops, s);
   s += s.back() == '[' ? bwd_layout.substr(bwd_layout.empty() ? 0 : 1) : bwd_layout;
   // ops the backward visits (0 for the forward-only branch of a feature L1 target) and values without a gradient buffer
   int bwd_ops = 0, detached = 0;

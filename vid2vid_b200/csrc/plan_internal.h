@@ -106,13 +106,20 @@ struct GOp {
   float* gdz = nullptr;      // training plans: G_HEAD / G_CONV_ACT pre-activation gradient, dense NHWC fp32 [.][Cout]
   double macs = 0.0;
   CUtensorMap tmA{}, tmB{};
-  ConvKernelParams kp{};
+  ConvKernelParams kp{};     // fill_conv_params: every parameter without an arena address (the launch's XOp::kp adds those)
 };
 
 enum XKind { X_IMPORT, X_CONV, X_RAWSTATS, X_FINALIZE, X_APPLY, X_EXPORT, X_COMPOSITE, X_MEMSET, X_COPY, X_CORR, X_MAXPOOL, X_FEATL1 };
+// One launch of the forward list (emit_forward).  Besides its parameters it keeps what v2v_plan_describe reports and the
+// parameters do not say.
 struct XOp {
   XKind kind;
-  int gop = -1;
+  int gop = -1;              // the graph op the launch belongs to (-1: the statistics memset)
+  int buf = -1;              // import, copy, apply: the activation buffer written; export: the buffer read
+  int in_buf = -1;           // copy: the buffer read
+  bool repeat = false;       // apply: an earlier normalise pass read the same raw slice
+  int fin_gop[2] = {-1, -1};   // conv: the normalising op each tail finalisation kp.fin[q] serves
+  ConvKernelParams kp{};
   ImportParams imp{};
   ExportParams exp{};
   FinalizeParams fin{};
@@ -207,7 +214,7 @@ int make_tmap_act(CUtensorMap* tm, const ActDesc& a, int box_w, int box_h, int k
 int make_tmap_w(CUtensorMap* tm, bf16* w, int Ktotal, int Cout, int BN, int kc);
 PackParams pack_params(const GOp& op);
 int pack_one(const GOp& op, cudaStream_t stream);
-void describe_conv(v2v_plan* P, const GOp& op, std::string& s);
+void describe_conv(const v2v_plan* P, const GOp& op, std::string& s);
 void describe_pack(const v2v_plan* P, size_t i, std::string& s);
 
 // plan.cu
@@ -215,11 +222,6 @@ int new_value(v2v_plan* p, int N, int H, int W, int C);
 int size_arena(v2v_plan* P);
 int run_xop(v2v_plan* P, const XOp& x, cudaStream_t s);
 FeatL1Params featl1_params(const v2v_plan* P, const GOp& op);
-std::vector<int> finalize_sites(const v2v_plan* P);
-ApplyParams apply_params(const v2v_plan* P, const GOp& op, size_t m);
-void describe_epilogue_forward(v2v_plan* P, std::string& s);
-void describe_buffers(const v2v_plan* P, std::string& s);
-void describe_layout(const v2v_plan* P, std::string& s);
 
 // plan_backward.cu
 int alloc_training(v2v_plan* P, cudaStream_t stream);
