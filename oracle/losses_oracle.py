@@ -25,11 +25,25 @@ def gan_loss(preds, target_is_real):
     return total
 
 
+# Sign source of every L1 term here.  None: mean |a - b|.  A callable sign(a, b) -> tensor shaped like a (entries +-1 or 0):
+# the term becomes mean(sign * (a - b)), which has the same value wherever the sign is that of a - b and the same gradient
+# away from a = b, but takes its kinks from the caller -- a gradient comparison with another implementation passes that
+# implementation's signs, so that elements where the two sit on opposite sides of a = b do not count as differences.
+L1_SIGN = None
+
+
+def l1_mean(a, b):
+    """mean |a - b| (nn.L1Loss), or mean(s * (a - b)) with s = L1_SIGN(a, b) when a sign source is set."""
+    if L1_SIGN is None:
+        return torch.mean(torch.abs(a - b))
+    return torch.mean(L1_SIGN(a.detach(), b.detach()) * (a - b))
+
+
 def masked_l1(inp, target, mask):
     """MaskedL1Loss.forward (networks.py:809-812): L1 over input*mask vs target*mask, mask broadcast over channels,
     averaged over ALL elements (masked-out pixels count as zeros, they are not excluded from the mean)."""
     m = mask.expand(-1, inp.size(1), -1, -1)
-    return torch.mean(torch.abs(inp * m - target * m))
+    return l1_mean(inp * m, target * m)
 
 
 def gan_and_fm_loss(pred_real, pred_fake, *, n_layers_D=3, num_D=2, lambda_feat=10.0, no_ganFeat=False):
@@ -42,7 +56,7 @@ def gan_and_fm_loss(pred_real, pred_fake, *, n_layers_D=3, num_D=2, lambda_feat=
         w = (4.0 / (n_layers_D + 1)) * (1.0 / num_D) * lambda_feat
         for i in range(min(len(pred_fake), num_D)):
             for j in range(len(pred_fake[i]) - 1):
-                fm = fm + w * torch.mean(torch.abs(pred_fake[i][j] - pred_real[i][j]))
+                fm = fm + w * l1_mean(pred_fake[i][j], pred_real[i][j])
     return g_gan, fm
 
 
