@@ -540,29 +540,23 @@ cudaError_t launch_conv_bwd(const BwdConv& p, cudaStream_t s) {
 
 int bias_grad_blocks(long long npix) { return (int)std::max(1LL, std::min(64LL, npix / 4096)); }
 
-cudaError_t launch_bias_grad(const float* dy, int dy_C, long long npix, int C, float* dbias, float* dbias2, int C1, cudaStream_t s) {
-  dim3 grid(C, (unsigned)bias_grad_blocks(npix));
-  bias_grad_kernel<<<grid, 256, 0, s>>>(dy, dy_C, npix, C, dbias, dbias2, C1);
-  return cudaGetLastError();
-}
-
 // The vectorised reduce aims at 4 blocks per SM of the H100 SXM (132 SMs) over the batch, each block summing at least 8
 // pixel rows per thread; the scalar kernel takes one block per channel and image, split over up to 32 slices of 8192 pixels.
-NormBwdLaunch norm_bwd_launch(int N, int H, int W, int C, int raw_C, int c_off, int has_norm, int param) {
+NormBwdLaunch norm_bwd_launch(const NormBwd& p) {
   NormBwdLaunch l{};
-  const long long HW = (long long)H * W;
-  l.param = param;
+  const long long HW = (long long)p.H * p.W;
+  l.param = (p.dgamma || p.dbeta) ? 1 : 0;
   l.grid[0] = l.grid[1] = l.grid[2] = 1;
-  if (!has_norm && !param) return l;               // norm-less unit without a bias gradient: draw = dz needs no sums
-  if (C % 4 == 0 && C <= 1024 && raw_C % 4 == 0 && c_off % 4 == 0) {
+  if (!p.has_norm && !l.param) return l;           // norm-less unit without a bias gradient: draw = dz needs no sums
+  if (p.C % 4 == 0 && p.C <= 1024 && p.raw.C % 4 == 0 && p.c_off % 4 == 0) {
     l.reduce = 1;
-    l.ppb = 256 / (C / 4);
-    const long long want_blocks = std::max(1LL, (4LL * 132) / N);
+    l.ppb = 256 / (p.C / 4);
+    const long long want_blocks = std::max(1LL, (4LL * 132) / p.N);
     l.chunk = std::max<long long>((long long)l.ppb * 8, (HW + want_blocks - 1) / want_blocks);
-    l.grid[0] = (int)((HW + l.chunk - 1) / l.chunk); l.grid[1] = N;
+    l.grid[0] = (int)((HW + l.chunk - 1) / l.chunk); l.grid[1] = p.N;
   } else {
     l.reduce = 2;
-    l.grid[0] = C; l.grid[1] = N; l.grid[2] = (int)std::max(1LL, std::min(32LL, HW / 8192));
+    l.grid[0] = p.C; l.grid[1] = p.N; l.grid[2] = (int)std::max(1LL, std::min(32LL, HW / 8192));
   }
   return l;
 }
@@ -570,7 +564,7 @@ NormBwdLaunch norm_bwd_launch(int N, int H, int W, int C, int raw_C, int c_off, 
 cudaError_t launch_norm_bwd(const NormBwd& p, cudaStream_t s) {
   cudaError_t e = cudaMemsetAsync(p.sums, 0, sizeof(float) * 2 * p.N * p.C, s);
   if (e != cudaSuccess) return e;
-  const NormBwdLaunch l = norm_bwd_launch(p.N, p.H, p.W, p.C, p.raw.C, p.c_off, p.has_norm, (p.dgamma || p.dbeta) ? 1 : 0);
+  const NormBwdLaunch l = norm_bwd_launch(p);
   const dim3 grid(l.grid[0], l.grid[1], l.grid[2]);
   if (l.reduce == 1) norm_bwd_reduce_vec_kernel<<<grid, 256, 2 * p.C * sizeof(float), s>>>(p, (int)l.chunk);
   else if (l.reduce == 2) norm_bwd_reduce_kernel<<<grid, 256, 0, s>>>(p);
@@ -590,26 +584,26 @@ cudaError_t launch_composite_bwd(const CompositeBwd& p, cudaStream_t s) {
 }
 // The gradient import / export transposes through 32 x 32 shared-memory tiles (grad_layout_tiled_kernel) when a tile row of
 // channels is worth it and the grid fits; narrow tensors (C < 8: the 3-channel images) take the elementwise kernels.
-int grad_layout_tiled(int N, int C, long long HW) { return C >= 8 && (HW + 31) / 32 <= 0x7fffffffLL && N <= 65535; }
+int grad_layout_tiled(const GradLayout& p) { return p.C >= 8 && ((long long)p.H * p.W + 31) / 32 <= 0x7fffffffLL && p.N <= 65535; }
 
-cudaError_t launch_grad_import(const float* g, float* dst, int N, int C_src, int c_off, int C, int H, int W, cudaStream_t s) {
-  const size_t HW = (size_t)H * W;
-  if (grad_layout_tiled(N, C, (long long)HW)) {
-    dim3 grid((unsigned)((HW + 31) / 32), (C + 31) / 32, N);
-    grad_layout_tiled_kernel<true><<<grid, 256, 0, s>>>(const_cast<float*>(g), dst, C_src, c_off, C, HW);
+cudaError_t launch_grad_import(const GradLayout& p, cudaStream_t s) {
+  const size_t HW = (size_t)p.H * p.W;
+  if (grad_layout_tiled(p)) {
+    dim3 grid((unsigned)((HW + 31) / 32), (p.C + 31) / 32, p.N);
+    grad_layout_tiled_kernel<true><<<grid, 256, 0, s>>>(p.g, p.v, p.C_src, p.c_off, p.C, HW);
     return cudaGetLastError();
   }
-  grad_import_kernel<<<grid1d((size_t)N * C * H * W), 256, 0, s>>>(g, dst, N, C_src, c_off, C, (size_t)H * W);
+  grad_import_kernel<<<grid1d((size_t)p.N * p.C * HW), 256, 0, s>>>(p.g, p.v, p.N, p.C_src, p.c_off, p.C, HW);
   return cudaGetLastError();
 }
-cudaError_t launch_grad_export(const float* src, float* g, int N, int C_src, int c_off, int C, int H, int W, cudaStream_t s) {
-  const size_t HW = (size_t)H * W;
-  if (grad_layout_tiled(N, C, (long long)HW)) {
-    dim3 grid((unsigned)((HW + 31) / 32), (C + 31) / 32, N);
-    grad_layout_tiled_kernel<false><<<grid, 256, 0, s>>>(g, const_cast<float*>(src), C_src, c_off, C, HW);
+cudaError_t launch_grad_export(const GradLayout& p, cudaStream_t s) {
+  const size_t HW = (size_t)p.H * p.W;
+  if (grad_layout_tiled(p)) {
+    dim3 grid((unsigned)((HW + 31) / 32), (p.C + 31) / 32, p.N);
+    grad_layout_tiled_kernel<false><<<grid, 256, 0, s>>>(p.g, p.v, p.C_src, p.c_off, p.C, HW);
     return cudaGetLastError();
   }
-  grad_export_kernel<<<grid1d((size_t)N * C * H * W), 256, 0, s>>>(src, g, N, C_src, c_off, C, (size_t)H * W);
+  grad_export_kernel<<<grid1d((size_t)p.N * p.C * HW), 256, 0, s>>>(p.v, p.g, p.N, p.C_src, p.c_off, p.C, HW);
   return cudaGetLastError();
 }
 cudaError_t launch_convact_bwd(const float* dy, const ActDesc& out, int act, float slope, float* dz, int C, int dz_C, cudaStream_t s) {

@@ -70,11 +70,16 @@ size_t wgrad_stage_bytes(const WgradParams& p);
 size_t wgrad_stage_smem_bytes(const WgradParams& p);
 cudaError_t launch_wgrad_umma(const CUtensorMap& tmOut, const CUtensorMap& tmIn, const WgradParams& p, int R, int R1, int Cc,
                               float* dw, float* dw2, cudaStream_t s);
-cudaError_t launch_fold_add(const float* src, int Cs, int PH, int PW, float* dx, int N, int H, int W, int C, int pad, int reflect,
-                            cudaStream_t s);
-cudaError_t launch_bias_grad(const float* dy, int dy_C, long long npix, int C, float* dbias, float* dbias2, int C1, cudaStream_t s);
+// dx [N][H][W][C] += the data gradient over the padded extent, src: dense NHWC fp32 (N, PH, PW, channel stride Cs) whose pixel
+// (pad, pad) is input pixel (0, 0); reflect: the halo mirrors back onto the interior (fold_add_kernel)
+struct FoldParams {
+  const float* src; int Cs, PH, PW;
+  float* dx; int N, H, W, C;
+  int pad, reflect;
+};
+cudaError_t launch_fold_add(const FoldParams& p, cudaStream_t s);
 
-// Launch shape of launch_norm_bwd, chosen on the host from the unit's extent alone (v2v_plan_describe reports the same).
+// Launch shape of launch_norm_bwd, chosen on the host from the unit's parameters alone (v2v_plan_describe reports the same).
 // param: norm_param_grad_kernel runs, i.e. the unit has gamma / beta (or, norm-less, a bias) whose gradient is requested.
 struct NormBwdLaunch {
   int reduce;                  // per-channel sums: 0 none (norm-less unit without a bias gradient), 1 vectorised, 2 scalar kernel
@@ -83,16 +88,23 @@ struct NormBwdLaunch {
   int grid[3];                 // reduce grid (vectorised: chunks x N x 1; scalar: C x N x pixel slices)
   int param;                   // norm_param_grad_kernel runs (norm_bwd_apply_kernel always does)
 };
-NormBwdLaunch norm_bwd_launch(int N, int H, int W, int C, int raw_C, int c_off, int has_norm, int param);
+NormBwdLaunch norm_bwd_launch(const NormBwd& p);
 int bias_grad_blocks(long long npix);          // bias_grad_kernel: blocks per channel (grid.y)
-int grad_layout_tiled(int N, int C, long long HW);   // 1: launch_grad_import / launch_grad_export take the tiled kernel
+
+// A caller's fp32 NCHW gradient tensor g (channels [c_off, c_off + C) of C_src) and a plan's dense NHWC fp32 gradient buffer
+// v [N][H][W][C]: launch_grad_import adds g onto v, launch_grad_export adds v onto g.
+struct GradLayout {
+  float* g; float* v;
+  int N, C_src, c_off, C, H, W;
+};
+int grad_layout_tiled(const GradLayout& p);   // 1: launch_grad_import / launch_grad_export take the tiled kernel
 
 cudaError_t launch_conv_bwd(const BwdConv& p, cudaStream_t s);
 cudaError_t launch_norm_bwd(const NormBwd& p, cudaStream_t s);
 cudaError_t launch_head_bwd(const HeadBwd& p, cudaStream_t s);
 cudaError_t launch_composite_bwd(const CompositeBwd& p, cudaStream_t s);
-cudaError_t launch_grad_import(const float* g, float* dst, int N, int C_src, int c_off, int C, int H, int W, cudaStream_t s);
-cudaError_t launch_grad_export(const float* src, float* g, int N, int C_src, int c_off, int C, int H, int W, cudaStream_t s);
+cudaError_t launch_grad_import(const GradLayout& p, cudaStream_t s);
+cudaError_t launch_grad_export(const GradLayout& p, cudaStream_t s);
 cudaError_t launch_convact_bwd(const float* dy, const ActDesc& out, int act, float slope, float* dz, int C, int dz_C, cudaStream_t s);
 
 }  // namespace v2v

@@ -417,44 +417,35 @@ int pack_one(const GOp& op, cudaStream_t stream) {
 
 // One "pack" layout record: the packed matrix [rows][split + 1][Ktotal] at arena offset w_off and the path that writes it
 // (TC of the tiled kernel, 0 for the elementwise one).  Needs the op lowered and the arena sized.
-void describe_pack(const v2v_plan* P, size_t i, std::string& s) {
+void describe_pack(const v2v_plan* P, size_t i, Json& j) {
   const GOp& op = P->gops[i];
   const PackParams pp = pack_params(op);
-  char t[512];
-  snprintf(t, sizeof(t),
-           "{\"kind\":\"pack\",\"gop\":%zu,\"w_off\":%zu,\"rows\":%d,\"Ktotal\":%d,\"Cout\":%d,\"Cin\":%d,\"k\":[%d,%d],\"ntaps\":%d,"
-           "\"Cp\":%d,\"split\":%d,\"transposed\":%d,\"headkx\":%d,\"dgrad\":%d,\"w2\":%d,\"Cout1\":%d,\"TC\":%d}",
-           i, P->w_off[i], pp.headkx ? pp.headkx * pp.Cout : pp.Cout, op.Ktotal, pp.Cout, pp.Cin, pp.kh, pp.kw, pp.ntaps, pp.Cp,
-           pp.split, pp.transposed, pp.headkx, pp.dgrad, pp.w2 != nullptr, pp.Cout1, pack_weights_tiling(pp));
-  s += t;
+  j.obj().kv("kind", "pack").kv("gop", i).kv("w_off", P->w_off[i]).kv("rows", pp.headkx ? pp.headkx * pp.Cout : pp.Cout)
+      .kv("Ktotal", op.Ktotal).kv("Cout", pp.Cout).kv("Cin", pp.Cin).kv("k", {pp.kh, pp.kw}).kv("ntaps", pp.ntaps).kv("Cp", pp.Cp)
+      .kv("split", pp.split).kv("transposed", pp.transposed).kv("headkx", pp.headkx).kv("dgrad", pp.dgrad)
+      .kv("w2", pp.w2 != nullptr).kv("Cout1", pp.Cout1).kv("TC", pack_weights_tiling(pp)).end();
 }
 
 // One conv record of v2v_plan_describe: the conv, its geometry and the kernel configuration fill_conv_params chose (needs the
 // arena sized).
-void describe_conv(const v2v_plan* P, const GOp& op, std::string& s) {
-  char t[512];
+void describe_conv(const v2v_plan* P, const GOp& op, Json& j) {
   const ConvGeom& g = op.geom;
   const ConvKernelParams& kp = op.kp;
   // EG: epilogue groups per tile, always 1 (one 256-thread epilogue stores every tile; async_epi: which threads run it)
-  snprintf(t, sizeof(t),
-           "{\"kind\":%d,\"Cin\":%d,\"Cout\":%d,\"k\":[%d,%d],\"stride\":%d,\"transposed\":%d,\"in\":%d,\"TH\":%d,\"TW\":%d,"
-           "\"R\":%d,\"groups\":%d,\"phases\":%d,\"grid\":[%d,%d],\"out\":[%d,%d],"
-           "\"BN\":%d,\"kc\":%d,\"MG\":%d,\"CG\":%d,\"SG\":%d,\"resident\":%d,\"EG\":1,\"units\":%d,\"split\":%d,\"ring2\":%d,\"TB\":%d,\"SBr\":%d,"
-           "\"p2d\":%d,\"a_exact\":%d,\"headkx\":%d,\"grad\":%d,",
-           (int)op.kind, op.conv.Cin, op.conv.Cout, op.conv.kh, op.conv.kw, op.conv.stride, op.conv.transposed,
-           op.value_in, g.TH, g.TW, g.R, g.n_groups, g.n_phases, g.grid_h, g.grid_w, g.out_h, g.out_w,
-           kp.BN, kp.kc, kp.MG, kp.CG, kp.SG, kp.b_resident, kp.total_units, kp.split, kp.ring2, kp.TB, kp.SBr,
-           g.patch2d_kc > 0 ? 1 : 0, kp.a_exact, kp.headkx, (int)P->op_live[&op - P->gops.data()]);
-  s += t;
+  j.obj().kv("kind", (int)op.kind).kv("Cin", op.conv.Cin).kv("Cout", op.conv.Cout).kv("k", {op.conv.kh, op.conv.kw})
+      .kv("stride", op.conv.stride).kv("transposed", op.conv.transposed).kv("in", op.value_in).kv("TH", g.TH).kv("TW", g.TW)
+      .kv("R", g.R).kv("groups", g.n_groups).kv("phases", g.n_phases).kv("grid", {g.grid_h, g.grid_w}).kv("out", {g.out_h, g.out_w})
+      .kv("BN", kp.BN).kv("kc", kp.kc).kv("MG", kp.MG).kv("CG", kp.CG).kv("SG", kp.SG).kv("resident", kp.b_resident).kv("EG", 1)
+      .kv("units", kp.total_units).kv("split", kp.split).kv("ring2", kp.ring2).kv("TB", kp.TB).kv("SBr", kp.SBr)
+      .kv("p2d", g.patch2d_kc > 0).kv("a_exact", kp.a_exact).kv("headkx", kp.headkx).kv("grad", (int)P->op_live[&op - P->gops.data()]);
   // the derived launch parameters the kernel reads (ctas: persistent CTAs launched; smem: dynamic shared memory)
-  snprintf(t, sizeof(t),
-           "\"tiles_x\":%d,\"tiles_y\":%d,\"tile_dx\":%d,\"Cp\":%d,\"cblocks\":%d,\"row_bytes\":%d,\"kmma\":%d,\"kmma_last\":%d,\"BNt\":%d,\"layout_type\":%d,"
-           "\"sbo_bytes\":%d,\"sbo_a_bytes\":%d,\"RW\":%d,\"PW\":%d,\"PH\":%d,\"a_half_bytes\":%d,\"a_slot_bytes\":%d,"
-           "\"b_half_bytes\":%d,\"b_slot_bytes\":%d,\"SB\":%d,\"n_tiles\":%d,\"m_total\":%d,\"ctas\":%d,\"Khalf\":%d,\"smem\":%zu,\"async_epi\":%d}",
-           kp.tiles_x, kp.tiles_y, kp.tile_dx, kp.Cp, kp.cblocks, kp.row_bytes, kp.kmma, kp.kmma_last, kp.BNt, kp.layout_type, kp.sbo_bytes,
-           kp.sbo_a_bytes, kp.RW, kp.PW, kp.PH, kp.a_half_bytes, kp.a_slot_bytes, kp.b_half_bytes, kp.b_slot_bytes, kp.SB,
-           kp.n_tiles, kp.m_total, kp.grid, kp.Khalf, conv_umma_smem_bytes(kp), conv_umma_async_epilogue(kp));
-  s += t;
+  j.kv("tiles_x", kp.tiles_x).kv("tiles_y", kp.tiles_y).kv("tile_dx", kp.tile_dx).kv("Cp", kp.Cp).kv("cblocks", kp.cblocks)
+      .kv("row_bytes", kp.row_bytes).kv("kmma", kp.kmma).kv("kmma_last", kp.kmma_last).kv("BNt", kp.BNt)
+      .kv("layout_type", kp.layout_type).kv("sbo_bytes", kp.sbo_bytes).kv("sbo_a_bytes", kp.sbo_a_bytes).kv("RW", kp.RW)
+      .kv("PW", kp.PW).kv("PH", kp.PH).kv("a_half_bytes", kp.a_half_bytes).kv("a_slot_bytes", kp.a_slot_bytes)
+      .kv("b_half_bytes", kp.b_half_bytes).kv("b_slot_bytes", kp.b_slot_bytes).kv("SB", kp.SB).kv("n_tiles", kp.n_tiles)
+      .kv("m_total", kp.m_total).kv("ctas", kp.grid).kv("Khalf", kp.Khalf).kv("smem", conv_umma_smem_bytes(kp))
+      .kv("async_epi", conv_umma_async_epilogue(kp)).end();
 }
 
 }  // namespace v2v

@@ -442,71 +442,47 @@ static int emit_forward(const v2v_plan* P, std::vector<XOp>& xops) {
 // The arena layout of v2v_plan_describe (host-only: needs the arena sized): one "buffers" record per activation buffer (its byte
 // offset in the arena and the ActDesc fields that place element (n, c, y, x)), and one "scratch" record per correlation's fp32
 // scratch [in1 | in2 | out], each NCHW.  A caller that finalizes into its own workspace can decode every buffer from these.
-static void describe_buffers(const v2v_plan* P, std::string& s) {
-  char t[512];
-  bool first = true;
+static void describe_buffers(const v2v_plan* P, Json& j) {
+  j.key("buffers").arr();
   for (size_t v = 0; v < P->values.size(); ++v)
-    for (size_t m = 0; m < P->values[v].bufs.size(); ++m) {
-      const int b = P->values[v].bufs[m];
+    for (int b : P->values[v].bufs) {
       const ActDesc& a = P->acts[b];
-      snprintf(t, sizeof(t),
-               "%s{\"value\":%zu,\"buf\":%d,\"off\":%zu,\"N\":%d,\"H\":%d,\"W\":%d,\"C\":%d,\"Cvalid\":%d,\"pads\":[%d,%d,%d,%d],"
-               "\"parity\":%d,\"P\":%d,\"Hp\":%d,\"Wp\":%d,\"split\":%d,\"mode\":%d}",
-               first ? "" : ",", v, b, P->act_off[b], a.N, a.H, a.W, a.C, a.Cvalid, a.pad_t, a.pad_l, a.pad_b, a.pad_r, a.parity, a.P,
-               a.Hp, a.Wp, a.split, P->act_pad_mode[b]);
-      s += t;
-      first = false;
+      j.obj().kv("value", v).kv("buf", b).kv("off", P->act_off[b]).kv("N", a.N).kv("H", a.H).kv("W", a.W).kv("C", a.C)
+          .kv("Cvalid", a.Cvalid).kv("pads", {a.pad_t, a.pad_l, a.pad_b, a.pad_r}).kv("parity", a.parity).kv("P", a.P)
+          .kv("Hp", a.Hp).kv("Wp", a.Wp).kv("split", a.split).kv("mode", P->act_pad_mode[b]).end();
     }
-  s += "],\"scratch\":[";
-  first = true;
+  j.end().key("scratch").arr();
   for (size_t i = 0; i < P->gops.size(); ++i) {
     const GOp& op = P->gops[i];
     if (op.kind != G_CORR) continue;
     const Value& a = P->values[op.value_in], &o = P->values[op.value_out];
-    snprintf(t, sizeof(t), "%s{\"gop\":%zu,\"off\":%zu,\"N\":%d,\"C\":%d,\"H\":%d,\"W\":%d,\"C_out\":%d,\"H_out\":%d,\"W_out\":%d}",
-             first ? "" : ",", i, P->corr_off[i], a.N, a.C, a.H, a.W, o.C, o.H, o.W);
-    s += t;
-    first = false;
+    j.obj().kv("gop", i).kv("off", P->corr_off[i]).kv("N", a.N).kv("C", a.C).kv("H", a.H).kv("W", a.W).kv("C_out", o.C)
+        .kv("H_out", o.H).kv("W_out", o.W).end();
   }
+  j.end();
 }
 
 // The record writers of the forward launch list, one per launch kind.  An import or export of a correlation (direct) moves its
 // fp32 scratch instead of a caller tensor.
-static void describe_import(const v2v_plan* P, const XOp& x, std::string& s) {
+static void describe_import(const v2v_plan* P, const XOp& x, Json& j) {
   const ImportParams& p = x.imp;
   const ActDesc& o = p.out;
-  char t[512];
-  snprintf(t, sizeof(t),
-           "{\"kind\":\"import\",\"gop\":%d,\"buf\":%d,\"slot\":%d,\"direct\":%d,\"C_src\":%d,\"c_off\":%d,\"act\":%d,\"pad_mode\":%d,"
-           "\"skip_lo\":%d,\"split\":%d,\"parity\":%d,\"N\":%d,\"H\":%d,\"W\":%d,\"C\":%d,\"Cvalid\":%d,\"Wpad\":%d,\"CT\":%d}",
-           x.gop, x.buf, p.slot, P->gops[x.gop].kind == G_CORR, p.C_src, p.c_off, p.act, p.pad_mode, p.skip_lo, o.split, o.parity,
-           o.N, o.H, o.W, o.C, o.Cvalid, o.W + o.pad_l + o.pad_r, import_tile_channels(o));
-  s += t;
+  j.obj().kv("kind", "import").kv("gop", x.gop).kv("buf", x.buf).kv("slot", p.slot).kv("direct", P->gops[x.gop].kind == G_CORR)
+      .kv("C_src", p.C_src).kv("c_off", p.c_off).kv("act", p.act).kv("pad_mode", p.pad_mode).kv("skip_lo", p.skip_lo)
+      .kv("split", o.split).kv("parity", o.parity).kv("N", o.N).kv("H", o.H).kv("W", o.W).kv("C", o.C).kv("Cvalid", o.Cvalid)
+      .kv("Wpad", o.W + o.pad_l + o.pad_r).kv("CT", import_tile_channels(o)).end();
 }
 
-static void describe_export(const v2v_plan* P, const XOp& x, std::string& s) {
+static void describe_export(const v2v_plan* P, const XOp& x, Json& j) {
   const ActDesc& a = x.exp.in;
-  char t[320];
-  snprintf(t, sizeof(t), "{\"kind\":\"export\",\"gop\":%d,\"buf\":%d,\"direct\":%d,\"split\":%d,\"N\":%d,\"H\":%d,\"W\":%d,\"C\":%d,\"Cvalid\":%d}",
-           x.gop, x.buf, P->gops[x.gop].kind == G_CORR, a.split, a.N, a.H, a.W, a.C, a.Cvalid);
-  s += t;
+  j.obj().kv("kind", "export").kv("gop", x.gop).kv("buf", x.buf).kv("direct", P->gops[x.gop].kind == G_CORR).kv("split", a.split)
+      .kv("N", a.N).kv("H", a.H).kv("W", a.W).kv("C", a.C).kv("Cvalid", a.Cvalid).end();
 }
 
-static void describe_copy(const XOp& x, std::string& s) {
+static void describe_copy(const XOp& x, Json& j) {
   const CopyParams& p = x.copy;
-  char t[320];
-  snprintf(t, sizeof(t), "{\"kind\":\"copy\",\"gop\":%d,\"in_buf\":%d,\"buf\":%d,\"c_off\":%d,\"Cvalid\":%d,\"pad_mode\":%d,"
-           "\"in_split\":%d,\"split\":%d,\"parity\":%d}",
-           x.gop, x.in_buf, x.buf, p.c_off, p.in.Cvalid, p.pad_mode, p.in.split, p.out.split, p.out.parity);
-  s += t;
-}
-
-static void describe_grad_layout(const char* kind, size_t i, const Value& v, int C_src, int c_off, std::string& s) {
-  char t[320];
-  const long long HW = (long long)v.H * v.W;
-  snprintf(t, sizeof(t), "{\"kind\":\"%s\",\"gop\":%zu,\"N\":%d,\"C\":%d,\"H\":%d,\"W\":%d,\"C_src\":%d,\"c_off\":%d,\"tiled\":%d}", kind,
-           i, v.N, v.C, v.H, v.W, C_src, c_off, grad_layout_tiled(v.N, v.C, HW));
-  s += t;
+  j.obj().kv("kind", "copy").kv("gop", x.gop).kv("in_buf", x.in_buf).kv("buf", x.buf).kv("c_off", p.c_off).kv("Cvalid", p.in.Cvalid)
+      .kv("pad_mode", p.pad_mode).kv("in_split", p.in.split).kv("split", p.out.split).kv("parity", p.out.parity).end();
 }
 
 static const char* kFinSite[] = {"tail0", "tail1", "standalone"};
@@ -514,34 +490,30 @@ struct FinRecord { int gop, site; const FinalizeParams* fp; };
 
 // stats: how conv_umma_kernel accumulates the statistics rows of a conv whose raw a norm layer reads (async_epi, MG, BN,
 // phases, units over ctas persistent CTAs) or raw_stats_kernel (SIMT), and where each of its slices is finalised
-static void describe_stats(const v2v_plan* P, const XOp& x, const std::string& sites, std::string& s) {
+static void describe_stats(const v2v_plan* P, const XOp& x, const std::vector<int>& sites, Json& j) {
   const GOp& op = P->gops[x.gop];
   const Raw& r = P->raws[op.raw];
   const ConvKernelParams& kp = x.kp;
-  char t[512];
-  snprintf(t, sizeof(t),
-           "{\"kind\":\"stats\",\"gop\":%d,\"raw\":%d,\"N\":%d,\"C\":%d,\"H\":%d,\"W\":%d,\"raw_f32\":%d,\"impl\":\"%s\","
-           "\"async_epi\":%d,\"MG\":%d,\"BN\":%d,\"phases\":%d,\"n_tiles\":%d,\"m_total\":%d,\"units\":%d,\"ctas\":%d,\"fin\":[",
-           x.gop, op.raw, r.N, r.C, r.H, r.W, r.desc.f32, P->impl == V2V_IMPL_UMMA ? "umma" : "simt", conv_umma_async_epilogue(kp),
-           kp.MG, kp.BN, kp.num_phases, kp.n_tiles, kp.m_total, kp.total_units, kp.grid);
-  s += t + sites + "]}";
+  j.obj().kv("kind", "stats").kv("gop", x.gop).kv("raw", op.raw).kv("N", r.N).kv("C", r.C).kv("H", r.H).kv("W", r.W)
+      .kv("raw_f32", r.desc.f32).kv("impl", P->impl == V2V_IMPL_UMMA ? "umma" : "simt").kv("async_epi", conv_umma_async_epilogue(kp))
+      .kv("MG", kp.MG).kv("BN", kp.BN).kv("phases", kp.num_phases).kv("n_tiles", kp.n_tiles).kv("m_total", kp.m_total)
+      .kv("units", kp.total_units).kv("ctas", kp.grid).key("fin").arr();
+  for (int q : sites) j.val(kFinSite[q]);
+  j.end().end();
 }
 
 // finalize: batch / instance / per-sample statistics, image flags, running buffers, conv bias, the saved mean / rstd of training
 // plans, the slice
-static void describe_finalize(const v2v_plan* P, const FinRecord& f, std::string& s) {
+static void describe_finalize(const v2v_plan* P, const FinRecord& f, Json& j) {
   const FinalizeParams& fp = *f.fp;
-  char t[512];
-  snprintf(t, sizeof(t),
-           "{\"kind\":\"finalize\",\"gop\":%d,\"raw\":%d,\"site\":\"%s\",\"stats\":\"%s\",\"N\":%d,\"flags\":%d,"
-           "\"running\":%d,\"bias\":%d,\"mean_rstd\":%d,\"c_off\":%d,\"C\":%d}",
-           f.gop, P->gops[f.gop].raw, kFinSite[f.site], fp.sample_running ? "sample" : (fp.instance ? "instance" : "batch"), fp.N,
-           fp.flags_slot >= 0, fp.running_mean != nullptr, fp.conv_bias != nullptr, P->train ? 1 : 0, fp.c_off, fp.C);
-  s += t;
+  j.obj().kv("kind", "finalize").kv("gop", f.gop).kv("raw", P->gops[f.gop].raw).kv("site", kFinSite[f.site])
+      .kv("stats", fp.sample_running ? "sample" : (fp.instance ? "instance" : "batch")).kv("N", fp.N).kv("flags", fp.flags_slot >= 0)
+      .kv("running", fp.running_mean != nullptr).kv("bias", fp.conv_bias != nullptr).kv("mean_rstd", P->train).kv("c_off", fp.c_off)
+      .kv("C", fp.C).end();
 }
 
 // apply: the norm_apply_launch choice of one normalise pass into one output layout, and what the kernel reads and writes
-static void describe_apply(const v2v_plan* P, const XOp& x, std::string& s) {
+static void describe_apply(const v2v_plan* P, const XOp& x, Json& j) {
   const GOp& op = P->gops[x.gop];
   const std::vector<int>& bufs = P->values[op.value_out].bufs;
   const size_t layout = std::find(bufs.begin(), bufs.end(), x.buf) - bufs.begin();
@@ -551,71 +523,55 @@ static void describe_apply(const v2v_plan* P, const XOp& x, std::string& s) {
   const NormApplyLaunch l = norm_apply_launch(ap);
   const ActDesc& o = ap.out;
   const int Wpad = o.W + o.pad_l + o.pad_r;
-  char t[768];
-  snprintf(t, sizeof(t),
-           "{\"kind\":\"apply\",\"gop\":%d,\"op\":\"%s\",\"raw\":%d,\"layout\":%zu,\"repeat\":%d,\"kernel\":\"%s\",\"prec\":%d,"
-           "\"nadd\":%d,\"vecs\":%d,\"ppb\":%d,\"xt\":%d,\"grid\":[%d,%d],\"idle\":%d,\"ragged\":%d,\"N\":%d,\"H\":%d,"
-           "\"W\":%d,\"C\":%d,\"Cvalid\":%d,\"raw_C\":%d,\"c_off\":%d,\"pad_mode\":%d,\"pads\":[%d,%d,%d,%d],\"parity\":%d,"
-           "\"split\":%d,\"scale\":\"%s\",\"act\":%d,\"adds\":[",
-           x.gop, op.kind == G_RAWIN ? "rawin" : "norm_act", op.raw, layout, x.repeat ? 1 : 0, l.rows ? "rows" : "grid_stride",
-           ap.raw.f32, ap.n_add, l.vecs, l.ppb, l.xt, l.grid[0], l.grid[1], l.rows && 256 % l.vecs != 0,
-           l.rows && Wpad % l.xt != 0, o.N, o.H, o.W, o.C, ap.raw.Cvalid, ap.raw.C, op.kind == G_RAWIN ? 0 : op.n_off,
-           ap.pad_mode, o.pad_t, o.pad_l, o.pad_b, o.pad_r, o.parity, o.split, scale, ap.act);
-  s += t;
-  for (int a = 0; a < ap.n_add; ++a) {
-    snprintf(t, sizeof(t), "%s{\"parity\":%d,\"split\":%d,\"C\":%d}", a ? "," : "", ap.add[a].parity, ap.add[a].split, ap.add[a].C);
-    s += t;
-  }
-  s += "]}";
+  j.obj().kv("kind", "apply").kv("gop", x.gop).kv("op", op.kind == G_RAWIN ? "rawin" : "norm_act").kv("raw", op.raw)
+      .kv("layout", layout).kv("repeat", x.repeat).kv("kernel", l.rows ? "rows" : "grid_stride").kv("prec", ap.raw.f32)
+      .kv("nadd", ap.n_add).kv("vecs", l.vecs).kv("ppb", l.ppb).kv("xt", l.xt).kv("grid", {l.grid[0], l.grid[1]})
+      .kv("idle", l.rows && 256 % l.vecs != 0).kv("ragged", l.rows && Wpad % l.xt != 0).kv("N", o.N).kv("H", o.H).kv("W", o.W)
+      .kv("C", o.C).kv("Cvalid", ap.raw.Cvalid).kv("raw_C", ap.raw.C).kv("c_off", op.kind == G_RAWIN ? 0 : op.n_off)
+      .kv("pad_mode", ap.pad_mode).kv("pads", {o.pad_t, o.pad_l, o.pad_b, o.pad_r}).kv("parity", o.parity).kv("split", o.split)
+      .kv("scale", scale).kv("act", ap.act).key("adds").arr();
+  for (int a = 0; a < ap.n_add; ++a)
+    j.obj().kv("parity", ap.add[a].parity).kv("split", ap.add[a].split).kv("C", ap.add[a].C).end();
+  j.end().end();
 }
 
 // The "layout" records of v2v_plan_describe, in launch order: every import (caller tensor or correlation scratch), export,
-// concat copy and the weight pack of every conv launch, with the fields that select its code path.  Training plans add the
-// gradient import of every export and the gradient export of every input (assuming the caller passes both gradients), and per
-// tensor-core backward unit its fold, dgrad pack and unstage (describe_backward_layout).
-static void describe_layout(const v2v_plan* P, const std::vector<XOp>& xops, std::string& s) {
-  bool first = true;
-  auto sep = [&]() { if (!first) s += ","; first = false; };
+// concat copy and the weight pack of every conv launch, with the fields that select its code path; training plans add their
+// backward's layout launches (describe_backward_layout).
+static void describe_layout(const v2v_plan* P, const std::vector<XOp>& xops, const std::vector<BwdUnit>& units, Json& j) {
+  j.key("layout").arr();
   for (const XOp& x : xops) {
     switch (x.kind) {
-      case X_IMPORT: sep(); describe_import(P, x, s); break;
-      case X_CONV: sep(); describe_pack(P, x.gop, s); break;
-      case X_EXPORT: sep(); describe_export(P, x, s); break;
-      case X_COPY: sep(); describe_copy(x, s); break;
+      case X_IMPORT: describe_import(P, x, j); break;
+      case X_CONV: describe_pack(P, x.gop, j); break;
+      case X_EXPORT: describe_export(P, x, j); break;
+      case X_COPY: describe_copy(x, j); break;
       default: break;
     }
   }
-  if (!P->train) return;
-  for (size_t i = 0; i < P->gops.size(); ++i) {
-    const GOp& op = P->gops[i];
-    if (!P->op_live[i]) continue;
-    if (op.kind == G_EXPORT) { const Value& v = P->values[op.value_in]; sep(); describe_grad_layout("grad_import", i, v, v.C, 0, s); }
-    if (op.kind == G_INPUT) { sep(); describe_grad_layout("grad_export", i, P->values[op.value_out], op.C_src, op.c_off, s); }
-  }
+  if (P->train) describe_backward_layout(P, units, j);
+  j.end();
 }
 
 // The "epilogue_forward" records of v2v_plan_describe: every stats record (in launch order), every finalize record (in the
 // order of the passes they serve) and every apply record (in launch order).
-static void describe_epilogue_forward(const v2v_plan* P, const std::vector<XOp>& xops, std::string& s) {
+static void describe_epilogue_forward(const v2v_plan* P, const std::vector<XOp>& xops, Json& j) {
   std::vector<FinRecord> fins;
   for (const XOp& x : xops) {
     if (x.kind == X_CONV) for (int q = 0; q < x.kp.n_fin; ++q) fins.push_back({x.fin_gop[q], q, &x.kp.fin[q]});
     if (x.kind == X_FINALIZE) fins.push_back({x.gop, 2, &x.fin});
   }
   std::sort(fins.begin(), fins.end(), [](const FinRecord& a, const FinRecord& b) { return a.gop < b.gop; });
-  std::vector<std::string> sites(P->raws.size());      // per raw: the sites of its slices, as its stats record lists them
-  for (const FinRecord& f : fins) {
-    std::string& l = sites[P->gops[f.gop].raw];
-    l += std::string(l.empty() ? "\"" : ",\"") + kFinSite[f.site] + "\"";
-  }
-  bool first = true;
-  auto sep = [&]() { if (!first) s += ","; first = false; };
+  std::vector<std::vector<int>> sites(P->raws.size());      // per raw: the sites of its slices, as its stats record lists them
+  for (const FinRecord& f : fins) sites[P->gops[f.gop].raw].push_back(f.site);
+  j.key("epilogue_forward").arr();
   for (const XOp& x : xops) {
     if (x.kind != X_CONV || P->gops[x.gop].kind != G_CONV || sites[P->gops[x.gop].raw].empty()) continue;
-    sep(); describe_stats(P, x, sites[P->gops[x.gop].raw], s);
+    describe_stats(P, x, sites[P->gops[x.gop].raw], j);
   }
-  for (const FinRecord& f : fins) { sep(); describe_finalize(P, f, s); }
-  for (const XOp& x : xops) if (x.kind == X_APPLY) { sep(); describe_apply(P, x, s); }
+  for (const FinRecord& f : fins) describe_finalize(P, f, j);
+  for (const XOp& x : xops) if (x.kind == X_APPLY) describe_apply(P, x, j);
+  j.end();
 }
 
 }  // namespace v2v
@@ -1072,69 +1028,43 @@ int64_t v2v_plan_describe(const v2v_plan* P_, char* buf, int64_t cap) {
   std::vector<XOp> emitted;                           // an unfinalized plan: the launch list finalize would run
   if (!P->finalized && emit_forward(P, emitted)) return -1;
   const std::vector<XOp>& xops = P->finalized ? P->xops : emitted;
-  std::string s = "{\"values\":[";
-  std::string bwd_layout;            // training plans: the backward units' layout records, appended to "layout"
-  char t[512];
+  // training plans: the backward unit of every live conv, as finalize built it, or as it would build it (the same host-only
+  // choice; the sub-plans chosen here are destroyed on return)
+  struct Chosen {
+    std::vector<BwdUnit> units;
+    ~Chosen() { for (BwdUnit& u : units) v2v_plan_destroy(u.child); }
+  } chosen;
+  if (P->train && !P->finalized && choose_backward_units(P, chosen.units)) return -1;
+  const std::vector<BwdUnit>& units = P->finalized ? P->bwd : chosen.units;
+  std::string s;
+  Json j(s);
+  j.obj().key("values").arr();
   for (size_t i = 0; i < P->values.size(); ++i) {
     const Value& v = P->values[i];
-    snprintf(t, sizeof(t), "%s{\"id\":%zu,\"N\":%d,\"C\":%d,\"H\":%d,\"W\":%d,\"layouts\":[", i ? "," : "", i, v.N, v.C, v.H, v.W);
-    s += t;
-    for (size_t m = 0; m < v.reqs.size(); ++m) {
-      const Req& r = v.reqs[m];
-      snprintf(t, sizeof(t), "%s{\"mode\":%d,\"pads\":[%d,%d,%d,%d],\"parity\":%d}", m ? "," : "", r.mode, r.pads[0], r.pads[1],
-               r.pads[2], r.pads[3], r.parity);
-      s += t;
-    }
-    s += "]}";
+    j.obj().kv("id", i).kv("N", v.N).kv("C", v.C).kv("H", v.H).kv("W", v.W).key("layouts").arr();
+    for (const Req& r : v.reqs)
+      j.obj().kv("mode", r.mode).kv("pads", {r.pads[0], r.pads[1], r.pads[2], r.pads[3]}).kv("parity", r.parity).end();
+    j.end().end();
   }
-  s += "],\"convs\":[";
-  bool first = true;
-  for (const GOp& op : P->gops) {
-    if (!(op.kind == G_CONV || op.kind == G_CONV_ACT || op.kind == G_HEAD)) continue;
-    if (!first) s += ",";
-    describe_conv(P, op, s);
-    first = false;
-  }
-  // training plans: the backward of every live conv, as finalize built it, or as it would build it (same host-only choice)
+  j.end().key("convs").arr();
+  for (const GOp& op : P->gops)
+    if (op.kind == G_CONV || op.kind == G_CONV_ACT || op.kind == G_HEAD) describe_conv(P, op, j);
+  j.end();
   if (P->train) {
-    s += "],\"backward\":[";
-    first = true;
-    if (P->finalized) {
-      for (const BwdUnit& u : P->bwd) {
-        if (!first) s += ",";
-        describe_backward_unit(u, s);
-        describe_backward_layout(P, u, bwd_layout);
-        first = false;
-      }
-    } else {
-      for (size_t i = 0; i < P->gops.size(); ++i) {
-        const GOp& op = P->gops[i];
-        if (!(op.kind == G_CONV || op.kind == G_CONV_ACT || op.kind == G_HEAD) || !P->op_live[i]) continue;
-        BwdUnit u;
-        const int rc = choose_backward_unit(P, (int)i, u);
-        if (!rc) { if (!first) s += ","; describe_backward_unit(u, s); describe_backward_layout(P, u, bwd_layout); first = false; }
-        if (u.child) v2v_plan_destroy(u.child);
-        if (rc) return -1;
-      }
-    }
-    s += "],\"epilogue_backward\":[";
-    describe_epilogue_backward(P, s);
+    j.key("backward").arr();
+    for (const BwdUnit& u : units) describe_backward_unit(u, j);
+    j.end();
+    describe_epilogue_backward(P, j);
   }
-  s += "],\"epilogue_forward\":[";
-  describe_epilogue_forward(P, xops, s);
-  s += "],\"buffers\":[";
-  describe_buffers(P, s);
-  s += "],\"layout\":[";
-  describe_layout(P, xops, s);
-  s += s.back() == '[' ? bwd_layout.substr(bwd_layout.empty() ? 0 : 1) : bwd_layout;
+  describe_epilogue_forward(P, xops, j);
+  describe_buffers(P, j);
+  describe_layout(P, xops, units, j);
   // ops the backward visits (0 for the forward-only branch of a feature L1 target) and values without a gradient buffer
   int bwd_ops = 0, detached = 0;
   for (char l : P->op_live) bwd_ops += l;
   for (const Value& v : P->values) detached += v.detached;
-  snprintf(t, sizeof(t), "],\"conv_macs\":%.0f,\"n_slots\":%d,\"ops\":%zu,\"backward_ops\":%d,\"detached_values\":%d,\"sample_stats\":%d,"
-           "\"image_flags\":%d}", P->conv_macs, P->n_slots, P->gops.size(), bwd_ops, detached, P->sample_stats ? 1 : 0,
-           P->flags_slot >= 0 ? 1 : 0);
-  s += t;
+  j.kv("conv_macs", P->conv_macs).kv("n_slots", P->n_slots).kv("ops", P->gops.size()).kv("backward_ops", bwd_ops)
+      .kv("detached_values", detached).kv("sample_stats", P->sample_stats).kv("image_flags", P->flags_slot >= 0).end();
   if (buf && cap > 0) {
     size_t n = std::min((size_t)cap - 1, s.size());
     memcpy(buf, s.data(), n);

@@ -79,8 +79,8 @@ static void wgrad_operands(const v2v_plan* P, const BwdUnit& u, const ActDesc** 
 
 // Host-only half of the backward of live conv op i: the data-gradient mode and its sub-plan (built and lowered, no device
 // memory), and the weight-gradient launch or the reason it stays on the SIMT kernel.  u.child, when set, belongs to the
-// caller.  The device half is build_backward_units; v2v_plan_describe reports the same choice without a device.
-int choose_backward_unit(v2v_plan* P, int i, BwdUnit& u) {
+// caller.
+static int choose_backward_unit(v2v_plan* P, int i, BwdUnit& u) {
   const GOp& op = P->gops[i];
   const v2v_conv_desc& c = op.conv;
   const Value& vin = P->values[op.value_in];
@@ -183,17 +183,24 @@ int choose_backward_unit(v2v_plan* P, int i, BwdUnit& u) {
   return 0;
 }
 
-// Device half: finalizes each unit's sub-plan, encodes the weight gradient's tensor maps and allocates its stage buffer.
-int build_backward_units(v2v_plan* P, cudaStream_t stream) {
-  P->bwd_of.assign(P->gops.size(), -1);
-  size_t stage_max = 0;
+int choose_backward_units(v2v_plan* P, std::vector<BwdUnit>& units) {
   for (size_t i = 0; i < P->gops.size(); ++i) {
     const GOp& op = P->gops[i];
     if (op.kind != G_CONV && op.kind != G_CONV_ACT && op.kind != G_HEAD) continue;
     if (!P->op_live[i]) continue;                 // forward-only branch: no backward
-    P->bwd.emplace_back();                        // owns the sub-plan from here on, also when a step below fails
-    BwdUnit& u = P->bwd.back();
-    int rc = choose_backward_unit(P, (int)i, u); if (rc) return rc;
+    units.emplace_back();                         // owns the sub-plan from here on, also when the choice fails
+    int rc = choose_backward_unit(P, (int)i, units.back()); if (rc) return rc;
+  }
+  return 0;
+}
+
+// Device half: finalizes each unit's sub-plan, encodes the weight gradient's tensor maps and allocates its stage buffer.
+int build_backward_units(v2v_plan* P, cudaStream_t stream) {
+  int rc = choose_backward_units(P, P->bwd); if (rc) return rc;
+  P->bwd_of.assign(P->gops.size(), -1);
+  size_t stage_max = 0;
+  for (size_t k = 0; k < P->bwd.size(); ++k) {
+    BwdUnit& u = P->bwd[k];
     if (!u.mode) continue;
     rc = v2v_plan_finalize(u.child, reinterpret_cast<v2v_stream_t>(stream)); if (rc) return rc;
     if (u.wgrad) {
@@ -203,7 +210,7 @@ int build_backward_units(v2v_plan* P, cudaStream_t stream) {
       rc = make_tmap_act(&u.tmIn, *a_in, u.wg.KP, 1, std::min(a_in->C, 64)); if (rc) return rc;
       stage_max = std::max(stage_max, wgrad_stage_bytes(u.wg));
     }
-    P->bwd_of[i] = (int)P->bwd.size() - 1;
+    P->bwd_of[u.gop] = (int)k;
   }
   if (stage_max) {
     V2V_CUDA(cudaMalloc(reinterpret_cast<void**>(&P->wg_stage), stage_max));
@@ -212,28 +219,108 @@ int build_backward_units(v2v_plan* P, cudaStream_t stream) {
   return 0;
 }
 
+// ------------------------------------------------------------------------------ training: launch parameters of the backward
+// What one backward is asked for: io and gio, the caller's tensors and gradient tensors per IO slot (a null gradient tensor
+// asks for none), and pg, each parameter's gradient buffer (a parameter it lacks asks for none).  kEveryGradient asks for
+// every gradient, as v2v_plan_describe reports the launches: the gradient pointers it yields stand for requested buffers and
+// are never launched.
+static float g_requested;
+struct BwdRequest {
+  void* const* io;
+  void* const* gio;
+  const std::unordered_map<const void*, void*>* pg;     // null: every gradient
+  float* grad_io(int slot) const { return pg ? reinterpret_cast<float*>(gio[slot]) : &g_requested; }
+  float* grad(const void* param) const {
+    if (!param || !pg) return param ? &g_requested : nullptr;
+    auto it = pg->find(param);
+    return it == pg->end() ? nullptr : reinterpret_cast<float*>(it->second);
+  }
+};
+static const BwdRequest kEveryGradient{nullptr, nullptr, nullptr};
+
+// The fp32 SIMT backward of a conv op: data, weight and bias gradients (a bias in front of a norm, G_CONV, has zero gradient).
+// A tensor-core unit takes the data and weight gradients over.
+static BwdConv conv_bwd_params(const v2v_plan* P, const GOp& op, const BwdRequest& q) {
+  const Value& vin = P->values[op.value_in];
+  const v2v_conv_desc& c = op.conv;
+  BwdConv b{};
+  b.N = vin.N; b.H = vin.H; b.W = vin.W; b.oh = op.geom.out_h; b.ow = op.geom.out_w;
+  b.Cin = c.Cin; b.Cout = c.Cout; b.kh = c.kh; b.kw = c.kw; b.stride = c.stride;
+  b.pad = c.pad; b.transposed = c.transposed; b.pad_mode = c.pad_mode;
+  b.x = P->acts[vin.bufs[op.req_index]];
+  if (op.kind == G_CONV) { b.dy = P->raws[op.raw].graw; b.dy_C = P->raws[op.raw].desc.C; }
+  else { b.dy = op.gdz; b.dy_C = round_up(c.Cout, 8); }
+  b.w = c.weight; b.w2 = c.Cout2 > 0 ? c.weight2 : nullptr; b.Cout1 = c.Cout - c.Cout2;
+  b.dx = (vin.input_slot < 0 || q.grad_io(vin.input_slot)) ? vin.gval : nullptr;
+  b.dw = q.grad(c.weight); b.dw2 = b.w2 ? q.grad(c.weight2) : nullptr;
+  if (op.kind != G_CONV) { b.dbias = q.grad(c.bias); b.dbias2 = b.w2 ? q.grad(c.bias2) : nullptr; }
+  return b;
+}
+
+// The head backward: dz of each head channel from the gradients of its IO slot (the caller's and the composite backward's)
+static HeadBwd head_bwd_params(const v2v_plan* P, const GOp& op, const BwdRequest& q) {
+  HeadBwd h{};
+  h.N = P->values[op.value_in].N; h.H = op.geom.out_h; h.W = op.geom.out_w; h.Cout = op.conv.Cout;
+  h.dz = op.gdz; h.dz_C = round_up(op.conv.Cout, 8);
+  for (int j = 0; j < op.conv.Cout; ++j) {
+    const int slot = op.head[j].slot;
+    h.out[j] = q.io ? reinterpret_cast<const float*>(q.io[slot]) : nullptr;
+    h.g_ext[j] = q.grad_io(slot);
+    h.g_int[j] = slot < (int)P->gslot.size() ? P->gslot[slot] : nullptr;
+    h.off[j] = op.kp.head_off[j]; h.bstride[j] = op.kp.head_bstride[j];
+    h.act[j] = op.head[j].act; h.scale[j] = op.head[j].scale;
+  }
+  return h;
+}
+
+// The norm backward of a G_NORM_ACT op: its slice of the raw tensor's saved statistics (set at finalize) and gradients
+static NormBwd norm_bwd_params(const v2v_plan* P, const GOp& op, const BwdRequest& q) {
+  const Raw& r = P->raws[op.raw];
+  const Value& vo = P->values[op.value_out];
+  auto slice = [&](const float* rows) { return rows ? rows + op.n_off : nullptr; };
+  NormBwd n{};
+  n.N = vo.N; n.H = vo.H; n.W = vo.W; n.C = op.cC; n.raw = r.desc; n.c_off = op.n_off;
+  n.has_norm = op.norm.kind != V2V_NORM_NONE; n.batch_stats = op.norm.kind == V2V_NORM_BATCH;
+  n.scale = slice(r.scale); n.shift = slice(r.shift); n.stat_stride = r.C;
+  n.mean = n.has_norm ? slice(r.mean) : nullptr; n.rstd = n.has_norm ? slice(r.rstd) : nullptr;
+  n.act = op.act; n.slope = op.slope; n.dy = vo.gval; n.draw = r.graw; n.draw_C = r.desc.C;
+  n.dadd0 = op.add[0] >= 0 ? P->values[op.add[0]].gval : nullptr;
+  n.dadd1 = op.add[1] >= 0 ? P->values[op.add[1]].gval : nullptr;
+  n.sums = P->gsums;
+  const v2v_conv_desc& c = P->gops[r.conv_op].conv;
+  if (n.has_norm) { n.dgamma = q.grad(op.norm.gamma); n.dbeta = q.grad(op.norm.beta); }
+  else { n.dgamma = nullptr; n.dbeta = q.grad(op.n_off == 0 ? c.bias : c.bias2); }
+  return n;
+}
+
+// The fold of a tensor-core unit's data gradient (its sub-plan's raw output) into dx
+static FoldParams fold_params(const v2v_plan* P, const BwdUnit& u, float* dx) {
+  const GOp& op = P->gops[u.gop];
+  const Value& vin = P->values[op.value_in];
+  const Raw& cr = u.child->raws[u.child_raw];
+  const int pad = u.mode == 1 ? op.conv.pad : 0;
+  return FoldParams{reinterpret_cast<const float*>(cr.desc.base), cr.desc.C, cr.H, cr.W, dx, vin.N, vin.H, vin.W, op.conv.Cin,
+                    pad, (op.conv.pad_mode == V2V_PAD_REFLECT && pad > 0) ? 1 : 0};
+}
+
+// The gradient import of a G_EXPORT (the caller's gradient of the output onto the value's) or the gradient export of a
+// G_INPUT (the value's gradient onto the caller's gradient of the input); g null: not requested
+static GradLayout grad_layout_params(const v2v_plan* P, const GOp& op, const BwdRequest& q) {
+  if (op.kind == G_EXPORT) {
+    const Value& v = P->values[op.value_in];
+    return GradLayout{q.grad_io(op.slot), v.gval, v.N, v.C, 0, v.C, v.H, v.W};
+  }
+  const Value& v = P->values[op.value_out];
+  return GradLayout{q.grad_io(op.slot), v.gval, v.N, op.C_src, op.c_off, v.C, v.H, v.W};
+}
+
 // Backward of one recorded forward (the plan's buffers still hold it).  Walks the graph ops in reverse.
 int run_backward(v2v_plan* P, void* const* io, void* const* gio, const std::unordered_map<const void*, void*>& pg,
                         cudaStream_t s) {
-  auto grad_of = [&](const void* param) -> float* {
-    if (!param) return nullptr;
-    auto it = pg.find(param);
-    return it == pg.end() ? nullptr : reinterpret_cast<float*>(it->second);
-  };
+  const BwdRequest q{io, gio, &pg};
   V2V_CUDA(cudaMemsetAsync(P->garena, 0, P->garena_bytes, s));
-  auto conv_bwd = [&](const GOp& op, const float* dy, int dy_C, bool bias_grad) -> int {
-    const Value& vin = P->values[op.value_in];
-    BwdConv b{};
-    b.N = vin.N; b.H = vin.H; b.W = vin.W; b.oh = op.geom.out_h; b.ow = op.geom.out_w;
-    b.Cin = op.conv.Cin; b.Cout = op.conv.Cout; b.kh = op.conv.kh; b.kw = op.conv.kw; b.stride = op.conv.stride;
-    b.pad = op.conv.pad; b.transposed = op.conv.transposed; b.pad_mode = op.conv.pad_mode;
-    b.x = P->acts[vin.bufs[op.req_index]];
-    b.dy = dy; b.dy_C = dy_C;
-    b.w = op.conv.weight; b.w2 = op.conv.Cout2 > 0 ? op.conv.weight2 : nullptr; b.Cout1 = op.conv.Cout - op.conv.Cout2;
-    const bool input_needs = vin.input_slot < 0 || (gio && gio[vin.input_slot] != nullptr);
-    b.dx = input_needs ? vin.gval : nullptr;
-    b.dw = grad_of(op.conv.weight); b.dw2 = b.w2 ? grad_of(op.conv.weight2) : nullptr;
-    if (bias_grad) { b.dbias = grad_of(op.conv.bias); b.dbias2 = b.w2 ? grad_of(op.conv.bias2) : nullptr; }
+  auto conv_bwd = [&](const GOp& op) -> int {
+    BwdConv b = conv_bwd_params(P, op, q);
     const int ui = P->bwd_of.empty() ? -1 : P->bwd_of[&op - P->gops.data()];
     if (ui >= 0) {
       // tensor-core path: dY -> the sub-plan's halo-padded split activation; data gradient = its conv (+ fold); weight gradient
@@ -247,12 +334,7 @@ int run_backward(v2v_plan* P, void* const* io, void* const* gio, const std::unor
           int rc = run_xop(C, x, s); if (rc) return rc;
         }
       }
-      if (b.dx) {
-        const Raw& cr = C->raws[u.child_raw];
-        const int pad = u.mode == 1 ? op.conv.pad : 0;
-        V2V_CUDA(launch_fold_add(reinterpret_cast<const float*>(cr.desc.base), cr.desc.C, cr.H, cr.W, b.dx, vin.N, vin.H, vin.W, op.conv.Cin, pad,
-                                 (op.conv.pad_mode == V2V_PAD_REFLECT && pad > 0) ? 1 : 0, s));
-      }
+      if (b.dx) V2V_CUDA(launch_fold_add(fold_params(P, u, b.dx), s));
       if (need_w && u.wgrad) {
         V2V_CUDA(launch_wgrad_umma(u.tmOut, u.tmIn, u.wg, u.M, u.M1, u.Nv, b.dw, b.dw2, s));
         b.dw = nullptr; b.dw2 = nullptr;
@@ -280,8 +362,8 @@ int run_backward(v2v_plan* P, void* const* io, void* const* gio, const std::unor
         break;
       }
       case G_EXPORT: {
-        const Value& v = P->values[op.value_in];
-        if (gio[op.slot]) V2V_CUDA(launch_grad_import(reinterpret_cast<const float*>(gio[op.slot]), v.gval, v.N, v.C, 0, v.C, v.H, v.W, s));
+        const GradLayout g = grad_layout_params(P, op, q);
+        if (g.g) V2V_CUDA(launch_grad_import(g, s));
         break;
       }
       case G_COMPOSITE: {
@@ -303,55 +385,31 @@ int run_backward(v2v_plan* P, void* const* io, void* const* gio, const std::unor
         break;
       }
       case G_HEAD: {
-        const Value& vin = P->values[op.value_in];
-        HeadBwd h{};
-        h.N = vin.N; h.H = op.geom.out_h; h.W = op.geom.out_w; h.Cout = op.conv.Cout; h.dz = op.gdz; h.dz_C = round_up(op.conv.Cout, 8);
-        for (int j = 0; j < op.conv.Cout; ++j) {
-          const int slot = op.head[j].slot;
-          h.out[j] = reinterpret_cast<const float*>(io[slot]);
-          h.g_ext[j] = reinterpret_cast<const float*>(gio[slot]);
-          h.g_int[j] = slot < (int)P->gslot.size() ? P->gslot[slot] : nullptr;
-          h.off[j] = op.kp.head_off[j]; h.bstride[j] = op.kp.head_bstride[j];
-          h.act[j] = op.head[j].act; h.scale[j] = op.head[j].scale;
-        }
-        V2V_CUDA(launch_head_bwd(h, s));
-        int rc = conv_bwd(op, op.gdz, round_up(op.conv.Cout, 8), true); if (rc) return rc;
+        V2V_CUDA(launch_head_bwd(head_bwd_params(P, op, q), s));
+        int rc = conv_bwd(op); if (rc) return rc;
         break;
       }
       case G_NORM_ACT: {
         const Raw& r = P->raws[op.raw];
-        const GOp& cop = P->gops[r.conv_op];
-        const Value& vo = P->values[op.value_out];
-        NormBwd n{};
-        n.N = vo.N; n.H = vo.H; n.W = vo.W; n.C = op.cC; n.raw = r.desc; n.c_off = op.n_off;
-        n.has_norm = op.norm.kind != V2V_NORM_NONE; n.batch_stats = op.norm.kind == V2V_NORM_BATCH;
-        n.scale = r.scale + op.n_off; n.shift = r.shift + op.n_off; n.stat_stride = r.C;
-        n.mean = n.has_norm ? r.mean + op.n_off : nullptr; n.rstd = n.has_norm ? r.rstd + op.n_off : nullptr;
-        if (!n.has_norm && !cop.conv.bias)     // plain activation of a bias-less conv: scale / shift arrays are unset
+        const NormBwd n = norm_bwd_params(P, op, q);
+        if (!n.has_norm && !P->gops[r.conv_op].conv.bias)     // plain activation of a bias-less conv: scale / shift arrays are unset
           V2V_CUDA(launch_bias_affine(r.scale, r.shift, nullptr, r.N, r.C, r.C, s));
-        n.act = op.act; n.slope = op.slope; n.dy = vo.gval; n.draw = r.graw; n.draw_C = r.desc.C;
-        n.dadd0 = op.add[0] >= 0 ? P->values[op.add[0]].gval : nullptr;
-        n.dadd1 = op.add[1] >= 0 ? P->values[op.add[1]].gval : nullptr;
-        n.sums = P->gsums;
-        if (n.has_norm) { n.dgamma = grad_of(op.norm.gamma); n.dbeta = grad_of(op.norm.beta); }
-        else { n.dgamma = nullptr; n.dbeta = grad_of(op.n_off == 0 ? cop.conv.bias : cop.conv.bias2); }
         V2V_CUDA(launch_norm_bwd(n, s));
         break;
       }
       case G_CONV: {
-        const Raw& r = P->raws[op.raw];
-        int rc = conv_bwd(op, r.graw, r.desc.C, false); if (rc) return rc;    // a bias in front of a norm has zero gradient
+        int rc = conv_bwd(op); if (rc) return rc;
         break;
       }
       case G_CONV_ACT: {
         const Value& vo = P->values[op.value_out];
         V2V_CUDA(launch_convact_bwd(vo.gval, P->acts[vo.bufs[0]], op.act, op.slope, op.gdz, op.conv.Cout, round_up(op.conv.Cout, 8), s));
-        int rc = conv_bwd(op, op.gdz, round_up(op.conv.Cout, 8), true); if (rc) return rc;
+        int rc = conv_bwd(op); if (rc) return rc;
         break;
       }
       case G_INPUT: {
-        const Value& v = P->values[op.value_out];
-        if (gio[op.slot]) V2V_CUDA(launch_grad_export(v.gval, reinterpret_cast<float*>(gio[op.slot]), v.N, op.C_src, op.c_off, v.C, v.H, v.W, s));
+        const GradLayout g = grad_layout_params(P, op, q);
+        if (g.g) V2V_CUDA(launch_grad_export(g, s));
         break;
       }
       case G_RAWIN: break;
@@ -365,53 +423,47 @@ int run_backward(v2v_plan* P, void* const* io, void* const* gio, const std::unor
 
 // One backward record: the data-gradient mode (0: SIMT, "simt" says why), the sub-plan's conv as a conv record, and the
 // weight-gradient launch (null: SIMT, "wgrad_simt" says why).
-void describe_backward_unit(const BwdUnit& u, std::string& s) {
-  char t[640];
-  snprintf(t, sizeof(t), "{\"gop\":%d,\"mode\":%d,\"simt\":\"%s\",\"wgrad_simt\":\"%s\",\"conv\":", u.gop, u.mode, u.simt.c_str(),
-           u.wg_simt.c_str());
-  s += t;
-  if (u.mode) describe_conv(u.child, u.child->gops[1], s);
-  else s += "null";
-  s += ",\"wgrad\":";
+void describe_backward_unit(const BwdUnit& u, Json& j) {
+  j.obj().kv("gop", u.gop).kv("mode", u.mode).kv("simt", u.simt).kv("wgrad_simt", u.wg_simt).key("conv");
+  if (u.mode) describe_conv(u.child, u.child->gops[1], j);
+  else j.null();
+  j.key("wgrad");
   if (u.wgrad) {
     const WgradParams& w = u.wg;
-    snprintf(t, sizeof(t),
-             "{\"swap\":%d,\"KP\":%d,\"BN\":%d,\"Mblocks\":%d,\"Nblocks\":%d,\"b_row\":%d,\"m_tiles\":%d,\"n_tiles\":%d,\"ntaps\":%d,"
-             "\"ksplit\":%d,\"chunks_per_unit\":%d,\"chunks_total\":%d,\"xsegs\":%d,\"gh\":%d,\"gw\":%d,\"stages\":%d,\"split\":%d,"
-             "\"Mp\":%d,\"Np\":%d}}",
-             w.swap, w.KP, w.BN, w.Mblocks, w.Nblocks, w.b_row, w.m_tiles, w.n_tiles, w.ntaps, w.ksplit, w.chunks_per_unit,
-             w.chunks_total, w.xsegs, w.gh, w.gw, w.stages, w.split, w.Mp, w.Np);
-    s += t;
+    j.obj().kv("swap", w.swap).kv("KP", w.KP).kv("BN", w.BN).kv("Mblocks", w.Mblocks).kv("Nblocks", w.Nblocks).kv("b_row", w.b_row)
+        .kv("m_tiles", w.m_tiles).kv("n_tiles", w.n_tiles).kv("ntaps", w.ntaps).kv("ksplit", w.ksplit)
+        .kv("chunks_per_unit", w.chunks_per_unit).kv("chunks_total", w.chunks_total).kv("xsegs", w.xsegs).kv("gh", w.gh)
+        .kv("gw", w.gw).kv("stages", w.stages).kv("split", w.split).kv("Mp", w.Mp).kv("Np", w.Np).end();
   } else {
-    s += "null}";
+    j.null();
   }
+  j.end();
 }
 
-// The layout launches of one tensor-core backward unit as run_backward makes them (each record with a leading comma): the
-// packing of the sub-plan's weights (the dgrad packing in mode 1), the fold of the data gradient into dX (crop: the sub-plan's
-// output extends past the padded input; overlap: a reflect halo so deep that the top and bottom, or left and right, mirrors
-// reach the same pixel) and the unstage of the weight gradient.
-void describe_backward_layout(const v2v_plan* P, const BwdUnit& u, std::string& s) {
-  if (!u.mode) return;
-  char t[512];
-  s += ",";
-  describe_pack(u.child, 1, s);
-  const GOp& op = P->gops[u.gop];
-  const Value& vin = P->values[op.value_in];
-  const Raw& cr = u.child->raws[u.child_raw];
-  const int pad = u.mode == 1 ? op.conv.pad : 0;
-  const int reflect = (op.conv.pad_mode == V2V_PAD_REFLECT && pad > 0) ? 1 : 0;
-  const int crop = cr.H > vin.H + 2 * pad || cr.W > vin.W + 2 * pad;
-  const int overlap = reflect && (pad >= vin.H - 1 - pad || pad >= vin.W - 1 - pad);
-  snprintf(t, sizeof(t),
-           ",{\"kind\":\"fold\",\"gop\":%d,\"mode\":%d,\"pad\":%d,\"reflect\":%d,\"crop\":%d,\"overlap\":%d,\"N\":%d,\"H\":%d,\"W\":%d,"
-           "\"C\":%d,\"PH\":%d,\"PW\":%d,\"Cs\":%d}",
-           u.gop, u.mode, pad, reflect, crop, overlap, vin.N, vin.H, vin.W, op.conv.Cin, cr.H, cr.W, cr.desc.C);
-  s += t;
-  if (u.wgrad) {
-    snprintf(t, sizeof(t), ",{\"kind\":\"unstage\",\"gop\":%d,\"swap\":%d,\"R\":%d,\"R1\":%d,\"Cc\":%d,\"taps\":%d,\"Mp\":%d,\"Np\":%d}",
-             u.gop, u.wg.swap, u.M, u.M1, u.Nv, u.wg.ntaps, u.wg.Mp, u.wg.Np);
-    s += t;
+// The layout launches of the backward as run_backward makes them, assuming the caller passes every gradient: the gradient
+// import of every export and the gradient export of every input, then per tensor-core unit the packing of its sub-plan's
+// weights (the dgrad packing in mode 1), the fold of the data gradient into dX (crop: the sub-plan's output extends past the
+// padded input; overlap: a reflect halo so deep that the top and bottom, or left and right, mirrors reach the same pixel)
+// and the unstage of the weight gradient.
+void describe_backward_layout(const v2v_plan* P, const std::vector<BwdUnit>& units, Json& j) {
+  for (size_t i = 0; i < P->gops.size(); ++i) {
+    const GOp& op = P->gops[i];
+    if (!P->op_live[i] || (op.kind != G_EXPORT && op.kind != G_INPUT)) continue;
+    const GradLayout g = grad_layout_params(P, op, kEveryGradient);
+    j.obj().kv("kind", op.kind == G_EXPORT ? "grad_import" : "grad_export").kv("gop", i).kv("N", g.N).kv("C", g.C).kv("H", g.H)
+        .kv("W", g.W).kv("C_src", g.C_src).kv("c_off", g.c_off).kv("tiled", grad_layout_tiled(g)).end();
+  }
+  for (const BwdUnit& u : units) {
+    if (!u.mode) continue;
+    describe_pack(u.child, 1, j);
+    const FoldParams f = fold_params(P, u, nullptr);
+    j.obj().kv("kind", "fold").kv("gop", u.gop).kv("mode", u.mode).kv("pad", f.pad).kv("reflect", f.reflect)
+        .kv("crop", f.PH > f.H + 2 * f.pad || f.PW > f.W + 2 * f.pad)
+        .kv("overlap", f.reflect && (f.pad >= f.H - 1 - f.pad || f.pad >= f.W - 1 - f.pad)).kv("N", f.N).kv("H", f.H)
+        .kv("W", f.W).kv("C", f.C).kv("PH", f.PH).kv("PW", f.PW).kv("Cs", f.Cs).end();
+    if (u.wgrad)
+      j.obj().kv("kind", "unstage").kv("gop", u.gop).kv("swap", u.wg.swap).kv("R", u.M).kv("R1", u.M1).kv("Cc", u.Nv)
+          .kv("taps", u.wg.ntaps).kv("Mp", u.wg.Mp).kv("Np", u.wg.Np).end();
   }
 }
 
@@ -419,48 +471,35 @@ void describe_backward_layout(const v2v_plan* P, const BwdUnit& u, std::string& 
 // assuming every parameter gradient (gamma, beta, bias) is requested.  Norm units: the norm_bwd_launch choice; conv_act and
 // head units: the dense dz buffer's channel stride, the stacked second bias (channels from C1 on go to dbias2) and the
 // bias_grad grid.
-void describe_epilogue_backward(const v2v_plan* P, std::string& s) {
-  char t[640];
-  bool first = true;
+void describe_epilogue_backward(const v2v_plan* P, Json& j) {
+  j.key("epilogue_backward").arr();
   for (size_t i = 0; i < P->gops.size(); ++i) {
     const GOp& op = P->gops[i];
     if (!P->op_live[i] || !(op.kind == G_NORM_ACT || op.kind == G_CONV_ACT || op.kind == G_HEAD)) continue;
-    if (!first) s += ",";
-    first = false;
     if (op.kind == G_NORM_ACT) {
-      const Raw& r = P->raws[op.raw];
-      const GOp& cop = P->gops[r.conv_op];
-      const Value& vo = P->values[op.value_out];
-      const int has_norm = op.norm.kind != V2V_NORM_NONE;
-      const int param = has_norm ? (op.norm.gamma || op.norm.beta) : ((op.n_off == 0 ? cop.conv.bias : cop.conv.bias2) != nullptr);
-      const NormBwdLaunch l = norm_bwd_launch(vo.N, vo.H, vo.W, op.cC, r.desc.C, op.n_off, has_norm, param);
-      snprintf(t, sizeof(t),
-               "{\"kind\":\"norm_act\",\"gop\":%zu,\"raw\":%d,\"C\":%d,\"N\":%d,\"H\":%d,\"W\":%d,\"c_off\":%d,\"raw_C\":%d,\"raw_f32\":%d,"
-               "\"has_norm\":%d,\"batch_stats\":%d,\"act\":%d,\"adds\":%d,\"reduce\":\"%s\",\"ppb\":%d,\"chunk\":%lld,\"grid\":[%d,%d,%d],"
-               "\"param\":%d}",
-               i, op.raw, op.cC, vo.N, vo.H, vo.W, op.n_off, r.desc.C, r.desc.f32, has_norm, op.norm.kind == V2V_NORM_BATCH ? 1 : 0,
-               op.act, (op.add[0] >= 0) + (op.add[1] >= 0), l.reduce == 1 ? "vec" : (l.reduce == 2 ? "scalar" : "none"), l.ppb,
-               l.chunk, l.grid[0], l.grid[1], l.grid[2], l.param);
-      s += t;
+      const NormBwd n = norm_bwd_params(P, op, kEveryGradient);
+      const NormBwdLaunch l = norm_bwd_launch(n);
+      j.obj().kv("kind", "norm_act").kv("gop", i).kv("raw", op.raw).kv("C", n.C).kv("N", n.N).kv("H", n.H).kv("W", n.W)
+          .kv("c_off", n.c_off).kv("raw_C", n.raw.C).kv("raw_f32", n.raw.f32).kv("has_norm", n.has_norm)
+          .kv("batch_stats", n.batch_stats).kv("act", n.act).kv("adds", (op.add[0] >= 0) + (op.add[1] >= 0))
+          .kv("reduce", l.reduce == 1 ? "vec" : (l.reduce == 2 ? "scalar" : "none")).kv("ppb", l.ppb).kv("chunk", l.chunk)
+          .kv("grid", {l.grid[0], l.grid[1], l.grid[2]}).kv("param", l.param).end();
       continue;
     }
-    const v2v_conv_desc& c = op.conv;
-    const Value& vin = P->values[op.value_in];
-    const long long npix = (long long)vin.N * op.geom.out_h * op.geom.out_w;
-    const int has_bias = c.bias != nullptr || (c.Cout2 > 0 && c.bias2 != nullptr);
-    snprintf(t, sizeof(t),
-             "{\"kind\":\"%s\",\"gop\":%zu,\"C\":%d,\"N\":%d,\"H\":%d,\"W\":%d,\"dz_C\":%d,\"bias\":%d,\"C1\":%d,\"bias_grid\":[%d,%d],"
-             "\"acts\":[",
-             op.kind == G_HEAD ? "head" : "conv_act", i, c.Cout, vin.N, op.geom.out_h, op.geom.out_w, round_up(c.Cout, 8), has_bias,
-             c.Cout2 > 0 ? c.Cout - c.Cout2 : c.Cout, has_bias ? c.Cout : 0, has_bias ? bias_grad_blocks(npix) : 0);
-    s += t;
-    const int nch = op.kind == G_HEAD ? c.Cout : 1;
-    for (int j = 0; j < nch; ++j) {
-      snprintf(t, sizeof(t), "%s%d", j ? "," : "", op.kind == G_HEAD ? op.head[j].act : op.act);
-      s += t;
+    const BwdConv b = conv_bwd_params(P, op, kEveryGradient);
+    const bool bias = b.dbias || b.dbias2;
+    j.obj().kv("kind", op.kind == G_HEAD ? "head" : "conv_act").kv("gop", i).kv("C", b.Cout).kv("N", b.N).kv("H", b.oh)
+        .kv("W", b.ow).kv("dz_C", b.dy_C).kv("bias", bias).kv("C1", b.w2 ? b.Cout1 : b.Cout)
+        .kv("bias_grid", {bias ? b.Cout : 0, bias ? bias_grad_blocks((long long)b.N * b.oh * b.ow) : 0}).key("acts").arr();
+    if (op.kind == G_HEAD) {
+      const HeadBwd h = head_bwd_params(P, op, kEveryGradient);
+      for (int c = 0; c < h.Cout; ++c) j.val(h.act[c]);
+    } else {
+      j.val(op.act);
     }
-    s += "]}";
+    j.end().end();
   }
+  j.end();
 }
 
 }  // namespace v2v

@@ -2,6 +2,8 @@
 // builders, lowering, arena layout, finalize, run / profile / repack), conv_lower.cu (conv geometry, tiling, tensor maps
 // and weight packing) and plan_backward.cu (gradient buffers and the tensor-core backward).
 #pragma once
+#include <iomanip>
+#include <sstream>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -35,6 +37,42 @@ static inline size_t round_up_sz(size_t a, size_t b) { return (a + b - 1) / b * 
 // padded channel count of an activation buffer: one K block of min(C,64) channels per shared-memory row (a plan's buffers
 // may be padded further: Value::Cp)
 static inline int pad_channels(int c) { return c <= 16 ? 16 : (c <= 32 ? 32 : round_up(c, 64)); }
+
+// The JSON writer of v2v_plan_describe: appends to s, placing every separator itself.  obj() / arr() open a container (as a
+// value: after key(), inside an array or at the top), end() closes the innermost one.  Integers print in full, a double as
+// %.0f, a string escaped.
+class Json {
+ public:
+  explicit Json(std::string& s) : s_(s) {}
+  Json& obj() { value(); s_ += '{'; open_.push_back('}'); first_ = true; return *this; }
+  Json& arr() { value(); s_ += '['; open_.push_back(']'); first_ = true; return *this; }
+  Json& end() { s_ += open_.back(); open_.pop_back(); first_ = false; return *this; }
+  Json& key(const char* k) { value(); str(k); s_ += ':'; keyed_ = true; return *this; }
+  Json& val(int v) { value(); s_ += std::to_string(v); return *this; }
+  Json& val(long long v) { value(); s_ += std::to_string(v); return *this; }
+  Json& val(size_t v) { value(); s_ += std::to_string(v); return *this; }
+  Json& val(double v) { value(); std::ostringstream o; o << std::fixed << std::setprecision(0) << v; s_ += o.str(); return *this; }
+  Json& val(const char* v) { value(); str(v); return *this; }
+  Json& val(const std::string& v) { return val(v.c_str()); }
+  Json& null() { value(); s_ += "null"; return *this; }
+  Json& val(std::initializer_list<int> v) { arr(); for (int x : v) val(x); return end(); }
+  template <class T> Json& kv(const char* k, const T& v) { return key(k).val(v); }
+  Json& kv(const char* k, std::initializer_list<int> v) { return key(k).val(v); }
+
+ private:
+  void value() {               // the separator in front of a key, or of a value that follows no key
+    if (!keyed_ && !first_) s_ += ',';
+    keyed_ = false; first_ = false;
+  }
+  void str(const char* v) {
+    s_ += '"';
+    for (; *v; ++v) { if (*v == '"' || *v == '\\') s_ += '\\'; s_ += *v; }
+    s_ += '"';
+  }
+  std::string& s_;
+  std::vector<char> open_;
+  bool first_ = true, keyed_ = false;
+};
 
 // ------------------------------------------------------------------------------ conv geometry
 struct ConvGeom {
@@ -214,8 +252,8 @@ int make_tmap_act(CUtensorMap* tm, const ActDesc& a, int box_w, int box_h, int k
 int make_tmap_w(CUtensorMap* tm, bf16* w, int Ktotal, int Cout, int BN, int kc);
 PackParams pack_params(const GOp& op);
 int pack_one(const GOp& op, cudaStream_t stream);
-void describe_conv(const v2v_plan* P, const GOp& op, std::string& s);
-void describe_pack(const v2v_plan* P, size_t i, std::string& s);
+void describe_conv(const v2v_plan* P, const GOp& op, Json& j);
+void describe_pack(const v2v_plan* P, size_t i, Json& j);
 
 // plan.cu
 int new_value(v2v_plan* p, int N, int H, int W, int C);
@@ -225,12 +263,14 @@ FeatL1Params featl1_params(const v2v_plan* P, const GOp& op);
 
 // plan_backward.cu
 int alloc_training(v2v_plan* P, cudaStream_t stream);
-int choose_backward_unit(v2v_plan* P, int i, BwdUnit& u);
+// the host half of the backward unit of every live conv, in graph order (build_backward_units finalizes them, v2v_plan_describe
+// reports them); units own their sub-plans, also after an error
+int choose_backward_units(v2v_plan* P, std::vector<BwdUnit>& units);
 int build_backward_units(v2v_plan* P, cudaStream_t stream);
 int run_backward(v2v_plan* P, void* const* io, void* const* gio, const std::unordered_map<const void*, void*>& pg,
                  cudaStream_t s);
-void describe_backward_unit(const BwdUnit& u, std::string& s);
-void describe_epilogue_backward(const v2v_plan* P, std::string& s);
-void describe_backward_layout(const v2v_plan* P, const BwdUnit& u, std::string& s);
+void describe_backward_unit(const BwdUnit& u, Json& j);
+void describe_epilogue_backward(const v2v_plan* P, Json& j);
+void describe_backward_layout(const v2v_plan* P, const std::vector<BwdUnit>& units, Json& j);
 
 }  // namespace v2v

@@ -258,11 +258,10 @@ __global__ void __launch_bounds__(256) fold_add_kernel(const float* __restrict__
   }
 }
 
-cudaError_t launch_fold_add(const float* src, int Cs, int PH, int PW, float* dx, int N, int H, int W, int C, int pad, int reflect,
-                            cudaStream_t s) {
-  const size_t total = (size_t)N * H * W * C;
+cudaError_t launch_fold_add(const FoldParams& p, cudaStream_t s) {
+  const size_t total = (size_t)p.N * p.H * p.W * p.C;
   const int blocks = (int)std::min<size_t>((total + 255) / 256, 132 * 16);
-  fold_add_kernel<<<blocks, 256, 0, s>>>(src, Cs, PH, PW, dx, N, H, W, C, pad, reflect);
+  fold_add_kernel<<<blocks, 256, 0, s>>>(p.src, p.Cs, p.PH, p.PW, p.dx, p.N, p.H, p.W, p.C, p.pad, p.reflect);
   return cudaGetLastError();
 }
 
