@@ -238,14 +238,12 @@ int v2v_plan_destroy(v2v_plan* plan);
 /* Select V2V_PREC_* (default V2V_PREC_BF16); must precede the first v2v_g_* call. */
 int v2v_plan_set_precision(v2v_plan* plan, int precision);
 
-/* Channels [c_off, c_off + C) of the fp32 NCHW tensor (N, C_src, H, W) bound to IO slot `slot`. */
-int v2v_g_input(v2v_plan* plan, int slot, int N, int C_src, int c_off, int C, int H, int W, int* value_out);
-/* As v2v_g_input with flags.  V2V_INPUT_EXACT_BF16: the caller promises that every element of the window is exactly
- * representable in bf16 (one-hot label maps, 0/1 edge maps -- what encode_input produces at full resolution,
- * models/vid2vid_model_G.py:93-105): precise plans then skip the all-zero lo half of that operand (2 MMAs per K block, no
- * change in results). */
+/* Channels [c_off, c_off + C) of the fp32 NCHW tensor (N, C_src, H, W) bound to IO slot `slot`.  flags:
+ * V2V_INPUT_EXACT_BF16: the caller promises that every element of the window is exactly representable in bf16 (one-hot
+ * label maps, 0/1 edge maps -- what encode_input produces at full resolution, models/vid2vid_model_G.py:93-105): precise
+ * plans then skip the all-zero lo half of that operand (2 MMAs per K block, no change in results). */
 #define V2V_INPUT_EXACT_BF16 1
-int v2v_g_input_ex(v2v_plan* plan, int slot, int N, int C_src, int c_off, int C, int H, int W, int flags, int* value_out);
+int v2v_g_input(v2v_plan* plan, int slot, int N, int C_src, int c_off, int C, int H, int W, int flags, int* value_out);
 /* Convolution of a value; result is a raw (pre-norm) tensor. */
 int v2v_g_conv(v2v_plan* plan, int value_in, const v2v_conv_desc* conv, int* raw_out);
 /* value = act(norm(raw)) + add0 + add1   (add ids may be -1).  Conv bias is folded into running_mean only.
@@ -277,15 +275,11 @@ int v2v_g_maxpool2(v2v_plan* plan, int value_in, int* value_out);
 int v2v_g_feature_l1(v2v_plan* plan, int value_x, int value_y, int slot, int index);
 /* Export a value as fp32 NCHW into the caller tensor bound to `slot`. */
 int v2v_g_export(v2v_plan* plan, int value, int slot);
-/* Fused warp / blend / fg composite on caller tensors (slots; -1 = absent).  s_raw is read (head output)
- * and, with a fg model, overwritten with the composited raw image; s_final is written. */
+/* Fused warp / blend / fg composite on caller tensors (slots; -1 = absent).  s_raw is read (head output); s_final is
+ * written.  With a fg model the composited raw image overwrites s_raw, or goes to IO slot s_raw_out when s_raw_out >= 0:
+ * training plans need the head output intact for the backward. */
 int v2v_g_composite(v2v_plan* plan, int s_raw, int s_flow, int s_weight, int s_prev, int prev_C, int s_fg, int s_mask,
-                    int s_final, int N, int H, int W, int use_warp, int align_corners);
-
-/* As v2v_g_composite, with the composited raw image written to IO slot s_raw_out (>= 0) instead of over s_raw: training
- * plans need the head output intact for the backward. */
-int v2v_g_composite_ex(v2v_plan* plan, int s_raw, int s_flow, int s_weight, int s_prev, int prev_C, int s_fg, int s_mask,
-                       int s_final, int s_raw_out, int N, int H, int W, int use_warp, int align_corners);
+                    int s_final, int s_raw_out, int N, int H, int W, int use_warp, int align_corners);
 
 /* Training plans (before finalize): keep the batch statistics and allocate dense fp32 gradient buffers. */
 int v2v_plan_set_training(v2v_plan* plan, int on);

@@ -118,22 +118,15 @@ class _GateFreeF:
 def gate_free(monkeypatch):
     """Gate-free generators and discriminators on both sides; yields the engine's remap count."""
     remaps = [0]
-    get_plan, plans = NW._Planned._get_plan, NW._Planned._plans
+    get_plan = NW._Planned._get_plan
 
     def _get_plan(self, key, device, build, train=False):
+        # gate-free plans are cached under a key of their own, so a plan built with real gates is never reused
         if isinstance(self, GATED):
-            return get_plan(self, key, device, lambda p: build(_GateFreePlan(p, remaps)), train)
+            return get_plan(self, ('gate_free',) + key, device, lambda p: build(_GateFreePlan(p, remaps)), train)
         return get_plan(self, key, device, build, train)
 
-    def _plans(self):
-        # gate-free plans live in a cache of their own, so a plan built with real gates is never reused (tagging the key
-        # instead would break MultiscaleDiscriminator, which reads its entry back under the key it passed)
-        if isinstance(self, GATED):
-            return self.__dict__.setdefault('_plan_cache_gate_free', {})
-        return plans(self)
-
     monkeypatch.setattr(NW._Planned, '_get_plan', _get_plan)
-    monkeypatch.setattr(NW._Planned, '_plans', _plans)
     monkeypatch.setattr(GO, 'F', _GateFreeF())
     monkeypatch.setattr(FD, 'F', _GateFreeF())
     return remaps

@@ -46,8 +46,8 @@ SYMBOLS = [
     'v2v_resample_forward', 'v2v_onehot_edges', 'v2v_avgpool3s2', 'v2v_fg_mask',
     'v2v_l1_loss_forward', 'v2v_l1_loss_backward', 'v2v_mse_const_forward', 'v2v_mse_const_backward', 'v2v_avgpool3s2_backward',
     'v2v_resample_backward', 'v2v_avgpool2', 'v2v_avgpool2_backward', 'v2v_face_region', 'v2v_instance_mean', 'v2v_face_features', 'v2v_face_features_per_image', 'v2v_ids_window_push', 'v2v_slots_window_push', 'v2v_tensor2im_u8', 'v2v_flownet_prep', 'v2v_resize', 'v2v_sub_channels', 'v2v_flow_conf',
-    'v2v_plan_create', 'v2v_plan_destroy', 'v2v_plan_set_precision', 'v2v_g_input', 'v2v_g_input_ex', 'v2v_g_conv', 'v2v_g_norm_act', 'v2v_g_norm_act_slice', 'v2v_g_conv_act',
-    'v2v_g_head', 'v2v_g_concat', 'v2v_g_correlation', 'v2v_g_maxpool2', 'v2v_g_feature_l1', 'v2v_g_export', 'v2v_g_composite', 'v2v_g_composite_ex', 'v2v_plan_set_training', 'v2v_plan_set_sample_stats', 'v2v_plan_set_image_flags', 'v2v_plan_backward', 'v2v_plan_finalize', 'v2v_plan_finalize_ws', 'v2v_plan_repack', 'v2v_plan_run',
+    'v2v_plan_create', 'v2v_plan_destroy', 'v2v_plan_set_precision', 'v2v_g_input', 'v2v_g_conv', 'v2v_g_norm_act', 'v2v_g_norm_act_slice', 'v2v_g_conv_act',
+    'v2v_g_head', 'v2v_g_concat', 'v2v_g_correlation', 'v2v_g_maxpool2', 'v2v_g_feature_l1', 'v2v_g_export', 'v2v_g_composite', 'v2v_plan_set_training', 'v2v_plan_set_sample_stats', 'v2v_plan_set_image_flags', 'v2v_plan_backward', 'v2v_plan_finalize', 'v2v_plan_finalize_ws', 'v2v_plan_repack', 'v2v_plan_run',
     'v2v_plan_profile', 'v2v_plan_num_kernels', 'v2v_plan_conv_macs', 'v2v_plan_workspace_bytes', 'v2v_plan_describe',
     'v2v_conv_tap_table',
 ]
@@ -69,8 +69,7 @@ def lib():
     l.v2v_plan_create.argtypes = [C.c_int, C.c_int, C.POINTER(C.c_void_p)]
     l.v2v_plan_destroy.argtypes = [C.c_void_p]
     l.v2v_plan_set_precision.argtypes = [C.c_void_p, C.c_int]
-    l.v2v_g_input.argtypes = [C.c_void_p] + [C.c_int] * 7 + [C.POINTER(C.c_int)]
-    l.v2v_g_input_ex.argtypes = [C.c_void_p] + [C.c_int] * 8 + [C.POINTER(C.c_int)]
+    l.v2v_g_input.argtypes = [C.c_void_p] + [C.c_int] * 8 + [C.POINTER(C.c_int)]
     l.v2v_g_conv.argtypes = [C.c_void_p, C.c_int, C.POINTER(ConvDesc), C.POINTER(C.c_int)]
     l.v2v_g_norm_act.argtypes = [C.c_void_p, C.c_int, C.POINTER(NormDesc), C.c_int, C.c_float, C.c_int, C.c_int,
                                  C.POINTER(C.c_int)]
@@ -83,10 +82,9 @@ def lib():
     l.v2v_g_feature_l1.argtypes = [C.c_void_p] + [C.c_int] * 4
     l.v2v_g_concat.argtypes = [C.c_void_p, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int)]
     l.v2v_g_correlation.argtypes = [C.c_void_p] + [C.c_int] * 8 + [C.c_float, C.POINTER(C.c_int)]
-    l.v2v_g_composite.argtypes = [C.c_void_p] + [C.c_int] * 13
     l.v2v_plan_finalize.argtypes = [C.c_void_p, C.c_void_p]
     l.v2v_plan_finalize_ws.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]
-    l.v2v_g_composite_ex.argtypes = [C.c_void_p] + [C.c_int] * 14
+    l.v2v_g_composite.argtypes = [C.c_void_p] + [C.c_int] * 14
     l.v2v_plan_set_training.argtypes = [C.c_void_p, C.c_int]
     l.v2v_plan_set_sample_stats.argtypes = [C.c_void_p, C.c_int]
     l.v2v_plan_set_image_flags.argtypes = [C.c_void_p, C.c_int]

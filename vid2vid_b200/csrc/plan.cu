@@ -650,19 +650,13 @@ int v2v_plan_destroy(v2v_plan* p) {
   return 0;
 }
 
-int v2v_g_input_ex(v2v_plan* p, int slot, int N, int C_src, int c_off, int C, int H, int W, int flags, int* value_out) {
-  int rc = v2v_g_input(p, slot, N, C_src, c_off, C, H, W, value_out);
-  if (rc) return rc;
-  p->values[*value_out].exact_bf16 = (flags & V2V_INPUT_EXACT_BF16) != 0;
-  return 0;
-}
-
-int v2v_g_input(v2v_plan* p, int slot, int N, int C_src, int c_off, int C, int H, int W, int* value_out) {
+int v2v_g_input(v2v_plan* p, int slot, int N, int C_src, int c_off, int C, int H, int W, int flags, int* value_out) {
   V2V_REQUIRE(p && !p->lowered && value_out, V2V_ERR_STATE, "plan already lowered or null");
   V2V_REQUIRE(slot >= 0 && N > 0 && C > 0 && c_off >= 0 && c_off + C <= C_src && H > 0 && W > 0, V2V_ERR_INVALID,
               "bad input description");
   GOp op; op.kind = G_INPUT; op.slot = slot; op.C_src = C_src; op.c_off = c_off;
   op.value_out = new_value(p, N, H, W, C);
+  p->values[op.value_out].exact_bf16 = (flags & V2V_INPUT_EXACT_BF16) != 0;
   p->values[op.value_out].input_slot = slot;
   p->n_slots = std::max(p->n_slots, slot + 1);
   p->gops.push_back(op);
@@ -815,12 +809,7 @@ int v2v_g_export(v2v_plan* p, int value, int slot) {
 }
 
 int v2v_g_composite(v2v_plan* p, int s_raw, int s_flow, int s_weight, int s_prev, int prev_C, int s_fg, int s_mask,
-                    int s_final, int N, int H, int W, int use_warp, int align_corners) {
-  return v2v_g_composite_ex(p, s_raw, s_flow, s_weight, s_prev, prev_C, s_fg, s_mask, s_final, -1, N, H, W, use_warp, align_corners);
-}
-
-int v2v_g_composite_ex(v2v_plan* p, int s_raw, int s_flow, int s_weight, int s_prev, int prev_C, int s_fg, int s_mask,
-                       int s_final, int s_raw_out, int N, int H, int W, int use_warp, int align_corners) {
+                    int s_final, int s_raw_out, int N, int H, int W, int use_warp, int align_corners) {
   V2V_REQUIRE(p && !p->lowered, V2V_ERR_STATE, "plan already lowered or null");
   V2V_REQUIRE(s_raw >= 0 && s_final >= 0, V2V_ERR_INVALID, "composite needs raw and final slots");
   V2V_REQUIRE(!use_warp || (s_flow >= 0 && s_weight >= 0 && s_prev >= 0 && prev_C >= 3), V2V_ERR_INVALID,

@@ -121,6 +121,7 @@ class FlowNetC(_Sub):
         c3 = self.u_conv(plan, 'conv3_1', plan.concat([self.u_conv(plan, 'conv_redir', c3a), corr]))
         t = self.tail(plan, c3)
         plan.export(self.refine(plan, {5: t[5], 4: t[4], 3: c3, 2: c2a}, t[6]), 1)
+        return {1: (N, 2, H // 4, W // 4)}
 
 
 class FlowNetS(_Sub):
@@ -143,6 +144,7 @@ class FlowNetS(_Sub):
         c3 = self.u_conv(plan, 'conv3_1', self.u_conv(plan, 'conv3', c2))
         t = self.tail(plan, c3)
         plan.export(self.refine(plan, {5: t[5], 4: t[4], 3: c3, 2: c2}, t[6]), 4)
+        return {4: (N, 2, H // 4, W // 4)}
 
 
 class FlowNetSD(_Sub):
@@ -166,6 +168,7 @@ class FlowNetSD(_Sub):
         c3 = self.u_conv(plan, 'conv3_1', self.u_conv(plan, 'conv3', c2))
         t = self.tail(plan, c3)
         plan.export(self.refine(plan, {5: t[5], 4: t[4], 3: c3, 2: c2}, t[6], inter=True), 1)
+        return {1: (N, 2, H // 4, W // 4)}
 
 
 class FlowNetFusion(_Sub):
@@ -193,6 +196,7 @@ class FlowNetFusion(_Sub):
         flow1 = self.u_predict(plan, 'predict_flow1', self.u_conv(plan, 'inter_conv1', cat1, act=False))
         cat0 = plan.concat([c0, self.u_deconv(plan, 'deconv0', cat1), self.u_upflow(plan, 'upsampled_flow1_to_0', flow1)])
         plan.export(self.u_predict(plan, 'predict_flow0', self.u_conv(plan, 'inter_conv0', cat0, act=False)), 7)
+        return {7: (N, 2, H, W)}
 
 
 def _p(t):
@@ -233,9 +237,18 @@ class FlowNet2(_Planned):
                     nn.init.uniform_(m.bias)
                 nn.init.xavier_uniform_(m.weight)
 
-    def _sub_plan(self, name, N, H, W, dev):
+    def _sub_key(self, name, N, H, W):
+        """Cache key and build closure of the plan of sub-network `name`."""
         sub = getattr(self, name)
-        return self._get_plan((name, N, H, W), dev, lambda p: sub.describe(p, N, H, W))
+        return (name, N, H, W), lambda p: sub.describe(p, N, H, W)
+
+    def _sub_plan(self, name, N, H, W, dev):
+        key, build = self._sub_key(name, N, H, W)
+        return self._get_plan(key, dev, build)
+
+    def _sub(self, name, io, N, H, W):
+        """Sub-network `name` on its inputs `io` (by slot); returns its flow (the plan's last slot)."""
+        return self._run_plan(*self._sub_key(name, N, H, W), io, range(len(io)), (), backward=False)[-1]
 
     def _evidence(self, x, x1, flow):
         """models.py:113-116: frame 1 warped towards frame 0 and the brightness-error magnitude."""
@@ -253,25 +266,18 @@ class FlowNet2(_Planned):
         x, x1, ws = new(6, H, W), new(3, H, W), torch.empty(B * 3, device=dev, dtype=torch.float32)
         ops._ck(L.lib().v2v_flownet_prep(_p(f0), _p(f1), bstride, cstride, _p(x), _p(x1), _p(ws), B, H, W, float(self.rgb_max),
                                          L.current_stream_ptr()))
-        q = (H // 4, W // 4)
-        flow2 = new(2, *q)
-        self._sub_plan('flownetc', B, H, W, dev).run([x, flow2], self.use_cuda_graph)
+        flow2 = self._sub('flownetc', [x], B, H, W)
         flow, flow_div = resize(flow2, H, W, 'bilinear', True, mul=self.div_flow, div=self.div_flow)     # models.py:106-107
         for name, mode in (('flownets_1', 'bilinear'), ('flownets_2', 'nearest')):
             warped, err = self._evidence(x, x1, flow)
-            flow2 = new(2, *q)
-            self._sub_plan(name, B, H, W, dev).run([x, warped, flow_div, err, flow2], self.use_cuda_graph)
+            flow2 = self._sub(name, [x, warped, flow_div, err], B, H, W)
             flow, flow_div = resize(flow2, H, W, mode, True, mul=self.div_flow, div=self.div_flow)       # :118-119 / :130-131
         flow_s = flow
-        flow2 = new(2, *q)
-        self._sub_plan('flownets_d', B, H, W, dev).run([x, flow2], self.use_cuda_graph)
-        flow_sd = resize(flow2, H, W, 'nearest', True, pre_div=self.div_flow)                            # :142-143
+        flow_sd = resize(self._sub('flownets_d', [x], B, H, W), H, W, 'nearest', True, pre_div=self.div_flow)   # :142-143
         _, err_s = self._evidence(x, x1, flow_s)
         _, err_sd = self._evidence(x, x1, flow_sd)
-        out = new(2, H, W)
-        self._sub_plan('flownetfusion', B, H, W, dev).run(
-            [x, flow_sd, flow_s, ops.channelnorm(flow_sd), ops.channelnorm(flow_s), err_sd, err_s, out], self.use_cuda_graph)
-        return out
+        return self._sub('flownetfusion', [x, flow_sd, flow_s, ops.channelnorm(flow_sd), ops.channelnorm(flow_s), err_sd, err_s],
+                         B, H, W)
 
     def forward(self, inputs):
         """inputs (B, 3, 2, H, W) -> flow (B, 2, H, W) in pixels (models.py:96-160, eval mode)."""
@@ -303,17 +309,17 @@ class FlowNet(nn.Module):
         return self
 
     def forward(self, input_A, input_B):
-        with torch.no_grad():
-            size = input_A.size()
-            assert len(size) in (4, 5)
-            if len(size) == 5:
-                b, n, c, h, w = size
-                flow, conf = self.compute_flow_and_conf(input_A.contiguous().view(-1, c, h, w), input_B.contiguous().view(-1, c, h, w))
-                return flow.view(b, n, 2, h, w), conf.view(b, n, 1, h, w)
-            return self.compute_flow_and_conf(input_A, input_B)
+        size = input_A.size()
+        assert len(size) in (4, 5)
+        if len(size) == 5:
+            b, n, c, h, w = size
+            flow, conf = self.compute_flow_and_conf(input_A.contiguous().view(-1, c, h, w), input_B.contiguous().view(-1, c, h, w))
+            return flow.view(b, n, 2, h, w), conf.view(b, n, 1, h, w)
+        return self.compute_flow_and_conf(input_A, input_B)
 
+    @torch.no_grad()
     def compute_flow_and_conf(self, im1, im2):
-        """flownet.py:43-58."""
+        """flownet.py:43-58 (detached, as the reference's FlowNet always is)."""
         assert im1.size()[1] == 3 and im1.size() == im2.size()
         im1, im2 = im1.contiguous().float(), im2.contiguous().float()
         old_h, old_w = im1.size()[2], im1.size()[3]

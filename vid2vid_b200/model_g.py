@@ -114,7 +114,8 @@ class Vid2VidModelG(HostScheduleMixin, nn.Module):
             if not os.path.exists(path):
                 raise FileNotFoundError('first-frame generator weights not found: %s' % path)
             net.load_state_dict(torch.load(path, map_location=self.device_))
-        return net.to(self.device_)
+        # pretrained and never trained here: with grad mode on, the first frames still run the inference plans
+        return net.requires_grad_(False).to(self.device_)
 
     def load_face_features(self, path='checkpoints/edge2face_single/features.npy', features=None):
         """The nearest-neighbour table of get_face_features: `features` ({label: (rows, feat_num + 1)}) if given, else the

@@ -10,10 +10,10 @@ There is no PyTorch/cuDNN fallback.
 Norm semantics (SURVEY App. B #1): Batch/InstanceNorm always use the statistics of the current
 tensor, as the reference does at inference because it never calls .eval() on G/D.
 """
+import collections
 import copy
 import functools
 import os
-import sys
 
 import torch
 import torch.nn as nn
@@ -239,6 +239,11 @@ def _can_pair(mods_a, mods_b):
             ca.kernel_size == cb.kernel_size and ca.stride == cb.stride and ca.out_channels % 8 == 0)
 
 
+# One plan call as _PlanFunction sees it: the plan, its IO tensors by slot, the slots whose tensors may take an input
+# gradient and the output slots (both restricted to the slots io fills), and the slots the caller filled (inputs, masks).
+_Call = collections.namedtuple('_Call', 'plan io in_slots out_slots fixed use_graph')
+
+
 class _PlanFunction(torch.autograd.Function):
     """Autograd node of one plan execution: forward = v2v_plan_run, backward = v2v_plan_backward (hand-written CUDA backward
     kernels over the plan's own buffers).  A plan holds the intermediates of its LAST run only: when another forward of the
@@ -246,53 +251,51 @@ class _PlanFunction(torch.autograd.Function):
     re-executes this node's forward (without the running-statistics side effect)."""
 
     @staticmethod
-    def forward(ctx, owner, plan, io, in_slots, out_slots, fixed_slots, *args):
-        # args = the input tensors that may need a gradient (slot order of in_slots) followed by the module parameters;
-        # fixed_slots = every slot the caller supplied (inputs incl. masks): all other slots are outputs / internal tensors
-        n_in = len(in_slots)
-        ctx.plan, ctx.in_slots, ctx.out_slots, ctx.n_in, ctx.fixed = plan, in_slots, out_slots, n_in, set(fixed_slots)
-        ctx.params = args[n_in:]
-        plan.run(io, owner.use_cuda_graph)
-        ctx.run_id = plan.run_id
+    def forward(ctx, call, *args):
+        # args = the tensors of call.in_slots followed by the module parameters the plan reads
+        io = call.io
+        call.plan.run(io, call.use_graph)
+        ctx.call, ctx.run_id = call._replace(io=None), call.plan.run_id
+        ctx.params = args[len(call.in_slots):]
         # The forward tensors the backward reads (inputs, masks AND the node's own outputs) go through save_for_backward: an
         # output kept as a plain ctx attribute is a reference cycle (output -> grad_fn -> ctx -> output) that only the cyclic
         # collector frees -- at cfg3 that held ~2.5 GB per training step until a generation-2 collection came by.
         ctx.n_slots = len(io)
         ctx.io_slots = [i for i, t_ in enumerate(io) if t_ is not None]
         ctx.save_for_backward(*[io[i] for i in ctx.io_slots])
-        return tuple(io[s] for s in out_slots)
+        return tuple(io[s] for s in call.out_slots)
 
     @staticmethod
     def backward(ctx, *gouts):
-        plan = ctx.plan
+        call, plan = ctx.call, ctx.call.plan
+        needs = ctx.needs_input_grad[1:]          # [0] is the call record
+        n_in = len(call.in_slots)
         io = [None] * ctx.n_slots
         for i, t_ in zip(ctx.io_slots, ctx.saved_tensors):
             io[i] = t_
         if plan.run_id != ctx.run_id:
             scratch = list(io)
             for s_ in range(len(scratch)):      # outputs of the re-execution go to scratch tensors (the originals are the user's)
-                if s_ not in ctx.fixed and scratch[s_] is not None:
+                if s_ not in call.fixed and scratch[s_] is not None:
                     scratch[s_] = torch.empty_like(scratch[s_])
             plan.run(scratch, False, recompute=True)
             io = scratch
         gio = [None] * len(io)
-        for s_, g in zip(ctx.out_slots, gouts):
+        for s_, g in zip(call.out_slots, gouts):
             if g is not None:
                 gio[s_] = g.contiguous().float()
         gin = []
-        for k, s_ in enumerate(ctx.in_slots):
-            if ctx.needs_input_grad[6 + k] and io[s_] is not None:
+        for k, s_ in enumerate(call.in_slots):
+            if needs[k]:
                 gio[s_] = torch.zeros_like(io[s_])
                 gin.append(gio[s_])
             else:
                 gin.append(None)
-        if os.environ.get('V2V_DEBUG_AUTOGRAD'):
-            print('plan backward: in_slots', ctx.in_slots, 'needs', ctx.needs_input_grad[6:6 + ctx.n_in], 'gin', [g is not None for g in gin])
         # Parameter gradients.  The kernels ACCUMULATE into the tensors they are given, so a parameter that already owns a
         # .grad (the trainer's flat all-reduce buffer, or a previous backward) receives its gradient in place and autograd gets
         # None for it: no per-parameter zero fill, no per-parameter accumulate kernel (~1000 of each per step otherwise).  The
         # others share ONE zero-filled buffer.
-        need = [bool(ctx.needs_input_grad[6 + ctx.n_in + j]) for j in range(len(ctx.params))]
+        need = [bool(needs[n_in + j]) for j in range(len(ctx.params))]
         direct = [need[j] and p.grad is not None and p.grad.is_contiguous() and p.grad.dtype == torch.float32 and
                   p.grad.device == p.device for j, p in enumerate(ctx.params)]
         fresh = [j for j, p in enumerate(ctx.params) if need[j] and not direct[j]]
@@ -308,7 +311,7 @@ class _PlanFunction(torch.autograd.Function):
             if direct[j]:
                 pgrads[j] = p.grad
         plan.backward(io, gio, ctx.params, pgrads)
-        return (None,) * 6 + tuple(gin) + tuple(ret)
+        return (None,) + tuple(gin) + tuple(ret)
 
 
 # Arithmetic of the conv stack (include/v2v_b200.h V2V_PREC_*): 'precise' = split-bf16 3-MMA, fp32-class -- the mode
@@ -362,17 +365,17 @@ class _Planned(nn.Module):
         return any(p.requires_grad for p in self.parameters()) or any(t is not None and t.requires_grad for t in tensors)
 
     def _get_plan(self, key, device, build, train=False):
+        """The plan cached under `key` + ('train',) + ('sample_stats',) + (precision,); a new plan keeps what build(plan)
+        returned as plan.outs."""
         ptrs, ver = self._signature()
         key = key + (('train',) if train else ()) + (('sample_stats',) if self.sample_stats else ()) + (self._precision(),)
         ent = self._plans().get(key)
         if ent is not None and ent['ptrs'] != ptrs:
             ent = None
         if ent is None:
-            if os.environ.get('V2V_LOG_PLANS'):
-                print('v2v: building plan %s for %s (cached: %d)' % (key, type(self).__name__, len(self._plans())), file=sys.stderr, flush=True)
             plan = Plan(device.index if device.index is not None else torch.cuda.current_device(),
                         precision=self._precision(), train=train, sample_stats=self.sample_stats)
-            build(plan)
+            plan.outs = build(plan)
             plan.finalize()
             ent = {'plan': plan, 'ptrs': ptrs, 'ver': ver}
             self._plans()[key] = ent
@@ -380,6 +383,33 @@ class _Planned(nn.Module):
             ent['plan'].repack()
             ent['ver'] = ver
         return ent['plan']
+
+    def _run_plan(self, key, build, io, grad_slots, out_slots, params=None, backward=True):
+        """One call of the plan cached under `key`.  build(plan) describes the plan and returns {slot: shape} of the fp32
+        tensors a run writes; they are allocated per call.  io: the caller's tensors by slot (inputs, masks, image flags;
+        io[0] is an input); grad_slots: the slots that may take an input gradient; out_slots: the outputs of the autograd
+        node; params: a function giving the parameters the plan reads (default: all of the module's).  Without autograd
+        this runs the inference plan; with it, the training plan through _PlanFunction, or NotImplementedError when the
+        caller has no backward (`backward` False).  Returns io with the written tensors filled in."""
+        train = self._wants_grad(*[io[s] for s in grad_slots])
+        if train and not backward:
+            raise NotImplementedError('%s.forward has no backward, so it passes no gradient: run it under torch.no_grad()'
+                                      % type(self).__name__)
+        dev = io[0].device
+        plan = self._get_plan(key, dev, build, train)
+        io = list(io) + [None] * (plan.n_slots - len(io))
+        fixed = frozenset(s for s, t in enumerate(io) if t is not None) if train else None
+        for s, shape in plan.outs.items():
+            io[s] = torch.empty(shape, device=dev, dtype=torch.float32)
+        if not train:
+            plan.run(io, self.use_cuda_graph)
+            return io
+        call = _Call(plan, io, tuple(s for s in grad_slots if io[s] is not None), tuple(s for s in out_slots if io[s] is not None),
+                     fixed, self.use_cuda_graph)
+        outs = _PlanFunction.apply(call, *[io[s] for s in call.in_slots], *(params or self.parameters)())
+        for s, t in zip(call.out_slots, outs):
+            io[s] = t
+        return io
 
     @staticmethod
     def _require_cuda(*ts):
@@ -476,14 +506,24 @@ class CompositeGenerator(_Planned):
             fg_feat = emit_seq(plan, self.indv_up, emit_seq(plan, self.indv_res, fgd))
             plan.export(fg_feat, S_FGF)                                                    # :225
             emit_head(plan, self.indv_final, fg_feat, (S_FG, self.output_nc, 1.0))         # :226
-        self._emit_composite(plan, N, H, W, use_raw_only)
+        return self._emit_composite(plan, N, H, W, use_raw_only)
 
     def _emit_composite(self, plan, N, H, W, use_raw_only):
+        """The composite, and {slot: shape} of every tensor the plan writes."""
         warp = not (use_raw_only or self.no_flow)
         # training plans keep the head output in S_RAW (the backward needs it) and write the composited raw image to S_RAWC
+        raw_out = S_RAWC if (plan.train and self.use_fg_model) else -1
         plan.composite(S_RAW, S_FLOW if warp else -1, S_W if warp else -1, S_PREV if warp else -1, self.prev_output_nc,
                        S_FG if self.use_fg_model else -1, S_MASK if self.use_fg_model else -1, S_FINAL, N, H, W, warp,
-                       self.align_corners, s_raw_out=S_RAWC if (plan.train and self.use_fg_model) else -1)   # :216-230
+                       self.align_corners, s_raw_out=raw_out)   # :216-230
+        c = {S_FINAL: self.output_nc, S_RAW: self.output_nc, S_IMGF: self._feat_c()}
+        if not self.no_flow:
+            c.update({S_FLOW: 2, S_W: 1, S_FLOWF: self._feat_c()})
+        if self.use_fg_model:
+            c.update({S_FGF: self._fg_feat_c(), S_FG: self.output_nc})
+        if raw_out >= 0:
+            c[S_RAWC] = self.output_nc
+        return {s: (N, c_, H, W) for s, c_ in c.items()}
 
     def _run(self, key, coarse, input, img_prev, mask, use_raw_only, image_flags=None):
         self._require_cuda(input, img_prev, mask, *coarse)
@@ -496,48 +536,28 @@ class CompositeGenerator(_Planned):
             raise ValueError('fg model needs a (N,1,H,W) mask')
         if self.output_nc != 3:
             raise NotImplementedError('the fused composite kernel handles 3 output channels')
-        train = self._wants_grad(input, img_prev, *coarse)
         build = lambda p: self._describe(p, N, H, W, use_raw_only)
         if image_flags is not None:
-            # slot plans: a per-sample plan that reads per-image flags (Plan.set_image_flags), cached under its own key
-            if train:
-                raise RuntimeError('per-image flags are for inference plans: a slot plan has no gradient')
+            # slot plans: a per-sample plan that reads per-image flags (Plan.set_image_flags), cached under its own key; they
+            # have no backward
             if not self.sample_stats:
                 raise ValueError('per-image flags need per-sample statistics (sample_stats = True)')
             if not image_flags.is_cuda or image_flags.dtype != torch.int32 or image_flags.numel() != N:
                 raise ValueError('image_flags must be an int32 CUDA tensor of %d elements' % N)
             key = key + ('image_flags',)
-            build = lambda p: (p.set_image_flags(S_FLAGS), self._describe(p, N, H, W, use_raw_only))
-        plan = self._get_plan(key + (N, H, W, bool(use_raw_only), bool(self.align_corners), bool(self.input_exact_bf16)), input.device,
-                              build, train=train)
-        new = lambda c: torch.empty((N, c, H, W), device=input.device, dtype=torch.float32)
+            build = lambda p: (p.set_image_flags(S_FLAGS), self._describe(p, N, H, W, use_raw_only))[1]
         io = [None] * 16
-        io[S_FLAGS] = image_flags
-        io[S_IN], io[S_PREV] = input, img_prev
-        io[S_FINAL], io[S_RAW], io[S_IMGF] = new(self.output_nc), new(self.output_nc), new(self._feat_c())
-        if not self.no_flow:
-            io[S_FLOW], io[S_W], io[S_FLOWF] = new(2), new(1), new(self._feat_c())
+        io[S_IN], io[S_PREV], io[S_FLAGS] = input, img_prev, image_flags
         if self.use_fg_model:
             io[S_MASK] = mask.contiguous()
-            io[S_FGF], io[S_FG] = new(self._fg_feat_c()), new(self.output_nc)
         for s, t in zip((S_CI, S_CF, S_CG), coarse):
             io[s] = t.contiguous() if t is not None else None
-        if not train:
-            plan.run(io, self.use_cuda_graph)
-            return io[S_FINAL], io[S_FLOW], io[S_W], io[S_RAW], io[S_IMGF], io[S_FLOWF], io[S_FGF]
-        raw_slot = S_RAW
-        if self.use_fg_model:
-            io[S_RAWC] = new(self.output_nc)
-            raw_slot = S_RAWC
-        in_slots = [s for s in (S_IN, S_PREV, S_CI, S_CF, S_CG) if io[s] is not None]
-        out_slots = [s for s in (S_FINAL, S_FLOW, S_W, raw_slot, S_IMGF, S_FLOWF, S_FGF) if io[s] is not None]
-        fixed = [s for s in (S_IN, S_PREV, S_MASK, S_CI, S_CF, S_CG) if io[s] is not None]
-        params = [p for p in self.parameters()]
-        outs = _PlanFunction.apply(self, plan, io, tuple(in_slots), tuple(out_slots), tuple(fixed),
-                                   *([io[s] for s in in_slots] + params))
-        res = dict(zip(out_slots, outs))
-        return (res.get(S_FINAL), res.get(S_FLOW), res.get(S_W), res.get(raw_slot), res.get(S_IMGF), res.get(S_FLOWF),
-                res.get(S_FGF))
+        io = self._run_plan(key + (N, H, W, bool(use_raw_only), bool(self.align_corners), bool(self.input_exact_bf16)), build, io,
+                            (S_IN, S_PREV, S_CI, S_CF, S_CG),
+                            (S_FINAL, S_FLOW, S_W, S_RAWC if self.use_fg_model else S_RAW, S_IMGF, S_FLOWF, S_FGF),
+                            backward=image_flags is None)
+        raw = io[S_RAWC] if io[S_RAWC] is not None else io[S_RAW]
+        return io[S_FINAL], io[S_FLOW], io[S_W], raw, io[S_IMGF], io[S_FLOWF], io[S_FGF]
 
     def _feat_c(self):
         return self.model_final_img[1].in_channels
@@ -610,7 +630,7 @@ class CompositeLocalGenerator(CompositeGenerator):
             fg_feat = emit_seq(plan, self.indv_up, fgd)                                                       # :319
             plan.export(fg_feat, S_FGF)
             emit_head(plan, self.indv_final, fg_feat, (S_FG, self.output_nc, 1.0))
-        self._emit_composite(plan, N, H, W, use_raw_only)
+        return self._emit_composite(plan, N, H, W, use_raw_only)
 
     def forward(self, input, img_prev, mask, img_feat_coarse, flow_feat_coarse, img_fg_feat_coarse, use_raw_only, image_flags=None):
         return self._run(('GL',), (img_feat_coarse, flow_feat_coarse, img_fg_feat_coarse), input, img_prev, mask,
@@ -642,6 +662,7 @@ class GlobalGenerator(_Planned):
         mods = list(self.model)
         v = emit_seq(plan, mods[:-3], v)
         emit_head(plan, mods[-3:], v, (1, self.output_nc, 1.0))
+        return {1: (N, self.output_nc, H, W)}
 
     def forward(self, input, feat=None):
         if feat is not None:
@@ -649,10 +670,7 @@ class GlobalGenerator(_Planned):
         self._require_cuda(input)
         input = input.contiguous()
         N, _, H, W = input.shape
-        plan = self._get_plan(('GG', N, H, W), input.device, lambda p: self._describe(p, N, H, W))
-        out = torch.empty((N, self.output_nc, H, W), device=input.device, dtype=torch.float32)
-        plan.run([input, out], self.use_cuda_graph)
-        return out
+        return self._run_plan(('GG', N, H, W), lambda p: self._describe(p, N, H, W), [input], (0,), (), backward=False)[1]
 
 
 class Global_with_z(_Planned):
@@ -697,12 +715,11 @@ class Global_with_z(_Planned):
         res = emit_seq(plan, self.model_resnet, plan.concat([down, v_zd]))              # :462
         up = emit_seq(plan, self.model_upsample, plan.concat([res, v_zd]))              # :463
         emit_head(plan, self.model_upsample_conv, plan.concat([up, v_z]), (2, self.output_nc, 1.0))   # :464
+        return {2: (N, self.output_nc, H, W)}
 
     def forward(self, x, z):
         from . import ops
         self._require_cuda(x, z)
-        if self._wants_grad(x, z):
-            raise NotImplementedError('Global_with_z has no backward (the first-frame generator runs under no_grad)')
         N, _, H, W = x.shape
         if x.shape[1] != self.input_nc or tuple(z.shape) != (N, self.nz, H, W) or H % 2 ** self.n_downsample_G or W % 2 ** self.n_downsample_G:
             raise ValueError('Global_with_z: x %s / z %s do not fit (%d + %d channels, sides divisible by %d)' % (
@@ -712,10 +729,7 @@ class Global_with_z(_Planned):
         for _ in range(self.n_downsample_G):
             z_down = ops.avgpool3s2(z_down)
         xz = torch.cat([x, z], dim=1)
-        plan = self._get_plan(('GZ', N, H, W), x.device, lambda p: self._describe(p, N, H, W))
-        out = torch.empty((N, self.output_nc, H, W), device=x.device, dtype=torch.float32)
-        plan.run([xz, z_down, out], self.use_cuda_graph)
-        return out
+        return self._run_plan(('GZ', N, H, W), lambda p: self._describe(p, N, H, W), [xz, z_down], (0, 1), (), backward=False)[2]
 
 
 class Encoder(_Planned):
@@ -741,17 +755,14 @@ class Encoder(_Planned):
         mods = list(self.model)
         v = emit_seq(plan, mods[:-3], plan.input(0, N, self.input_nc, 0, self.input_nc, H, W))
         emit_head(plan, mods[-3:], v, (1, self.output_nc, 1.0))
+        return {1: (N, self.output_nc, H, W)}
 
     def forward(self, input, inst):
         from . import ops
         self._require_cuda(input, inst)
-        if self._wants_grad(input):
-            raise NotImplementedError('Encoder has no backward (the face first frame runs under no_grad)')
         input = input.contiguous()
         N, _, H, W = input.shape
-        plan = self._get_plan(('E', N, H, W), input.device, lambda p: self._describe(p, N, H, W))
-        out = torch.empty((N, self.output_nc, H, W), device=input.device, dtype=torch.float32)
-        plan.run([input, out], self.use_cuda_graph)
+        out = self._run_plan(('E', N, H, W), lambda p: self._describe(p, N, H, W), [input], (0,), (), backward=False)[1]
         return ops.instance_mean(out, inst.contiguous(), self.n_ids, out=out)
 
 
@@ -829,6 +840,7 @@ class LocalEnhancer(_Planned):
                 emit_head(plan, mods[-3:], out, (L_ + 1, self.output_nc, 1.0))
             else:
                 out = emit_seq(plan, mods, x)
+        return {L_ + 1: (N, self.output_nc, H, W)}
 
     def forward(self, input, feat_map=None):
         from . import ops
@@ -839,10 +851,8 @@ class LocalEnhancer(_Planned):
         for _ in range(self.n_local_enhancers):
             pyr.append(ops.avgpool3s2(pyr[-1]))
         N, _, H, W = input.shape
-        plan = self._get_plan(('LE', N, H, W), input.device, lambda p: self._describe(p, N, H, W))
-        out = torch.empty((N, self.output_nc, H, W), device=input.device, dtype=torch.float32)
-        plan.run(pyr + [out], self.use_cuda_graph)
-        return out
+        return self._run_plan(('LE', N, H, W), lambda p: self._describe(p, N, H, W), pyr, range(len(pyr)), (),
+                              backward=False)[-1]
 
 
 # ------------------------------------------------------------------------------------ discriminators
@@ -906,9 +916,11 @@ class MultiscaleDiscriminator(_Planned):
         return [p for mods in self._tower_layers(d) for m in mods for p in m.parameters()]
 
     def _describe(self, plan, d, N, H, W):
+        """Tower d; returns {slot: shape} of the layer outputs it writes (every layer's with getIntermFeat, else the
+        logits')."""
         layers = self._tower_layers(d)
         v = plan.input(0, N, self.input_nc, 0, self.input_nc, H, W)
-        shapes = []
+        outs = {}
         for j, mods in enumerate(layers):
             last = j == len(layers) - 1
             conv = mods[0]
@@ -920,29 +932,18 @@ class MultiscaleDiscriminator(_Planned):
                 v = emit_seq(plan, mods, v)
                 if self.getIntermFeat:
                     plan.export(v, 1 + j)
-            shapes.append((conv.out_channels, oh, ow))
+            if last or self.getIntermFeat:
+                outs[1 + j] = (N, conv.out_channels, oh, ow)
             H, W = oh, ow
-        return shapes
+        return outs
 
     def _tower_forward(self, d, x):
         N, _, H, W = x.shape
-        key = ('D', d, N, H, W)
-        shapes_box = {}
-
-        def build(p):
-            shapes_box['s'] = self._describe(p, d, N, H, W)
-        train = self._wants_grad(x)
-        plan = self._get_plan(key, x.device, build, train=train)
-        shapes = self._plans()[key + (('train',) if train else ()) + (self._precision(),)].setdefault('shapes', shapes_box.get('s'))
-        outs = [torch.empty((N, c, h, w), device=x.device, dtype=torch.float32) for (c, h, w) in shapes]
-        io = [x] + [o if (self.getIntermFeat or j == len(outs) - 1) else None for j, o in enumerate(outs)]
-        if not train:
-            plan.run(io, self.use_cuda_graph)
-            return outs if self.getIntermFeat else [outs[-1]]
-        out_slots = tuple(s for s in range(1, len(io)) if io[s] is not None)
-        params = [p for p in self._tower_params(d)]
-        res = _PlanFunction.apply(self, plan, io, (0,), out_slots, (0,), *([x] + params))
-        return list(res)
+        n = self.n_layers + 2                    # layers per tower; slot 1 + j holds layer j's output
+        out_slots = tuple(range(1, n + 1)) if self.getIntermFeat else (n,)
+        io = self._run_plan(('D', d, N, H, W), lambda p: self._describe(p, d, N, H, W), [x], (0,), out_slots,
+                            params=functools.partial(self._tower_params, d))
+        return [io[s] for s in out_slots]
 
     def forward(self, input):
         from . import ops
@@ -1008,20 +1009,14 @@ class SequentialRunner(_Planned):
         self._require_cuda(x)
         x = x.contiguous()
         N, C, H, W = x.shape
-        key = ('SR', N, C, H, W, bool(self.input_exact_bf16))
-        plan = self._get_plan(key, x.device, lambda p: self._describe(p, N, C, H, W))
-        if self.head is not None:
-            oc, (oh, ow) = self._head_conv().out_channels, plan.describe()['convs'][-1]['out']
-        else:
-            last = plan.describe()['values'][-1]
-            oc, oh, ow = last['C'], last['H'], last['W']
-        out = torch.empty((N, oc, oh, ow), device=x.device, dtype=torch.float32)
-        if not self._wants_grad(x):
-            plan.run([x, out], self.use_cuda_graph)
-            return out
-        tplan = self._get_plan(key, x.device, lambda p: self._describe(p, N, C, H, W), train=True)
-        (res,) = _PlanFunction.apply(self, tplan, [x, out], (0,), (1,), (0,), *([x] + list(self.parameters())))
-        return res
+
+        def build(p):
+            self._describe(p, N, C, H, W)
+            d = p.describe()
+            if self.head is not None:
+                return {1: (N, self._head_conv().out_channels) + tuple(d['convs'][-1]['out'])}
+            return {1: tuple(d['values'][-1][k] for k in 'NCHW')}
+        return self._run_plan(('SR', N, C, H, W, bool(self.input_exact_bf16)), build, [x], (0,), (1,))[1]
 
 
 # ------------------------------------------------------------------------------------ VGG19 perceptual loss
@@ -1121,10 +1116,12 @@ class Vgg19(_Planned):
         fy = self._branch(plan, plan.input(1, N, 3, 0, 3, H, W))
         for k in range(5):
             plan.feature_l1(fx[k], fy[k], 2, k)
+        return {2: (5,)}
 
     def _describe_features(self, plan, N, H, W):
         for k, v in enumerate(self._branch(plan, plan.input(0, N, 3, 0, 3, H, W))):
             plan.export(v, 1 + k)
+        return {1 + k: (N,) + s for k, s in enumerate(self.feature_shapes(H, W))}
 
     @staticmethod
     def feature_shapes(H, W):
@@ -1137,14 +1134,10 @@ class Vgg19(_Planned):
     def forward(self, X):
         """The five feature maps (inference only: VGGLoss differentiates through feature_l1)."""
         self._require_cuda(X)
-        if self._wants_grad(X):
-            raise NotImplementedError('Vgg19.forward has no backward; VGGLoss differentiates through Vgg19.feature_l1')
         X = X.contiguous()
         N, _, H, W = X.shape
-        plan = self._get_plan(('VGGF', N, H, W), X.device, lambda p: self._describe_features(p, N, H, W))
-        outs = [torch.empty((N, c, h, w), device=X.device, dtype=torch.float32) for c, h, w in self.feature_shapes(H, W)]
-        plan.run([X] + outs, self.use_cuda_graph)
-        return outs
+        return self._run_plan(('VGGF', N, H, W), lambda p: self._describe_features(p, N, H, W), [X], (0,), (),
+                              backward=False)[1:6]
 
     def feature_l1(self, x, y):
         """(5,) fp32 tensor of mean |vgg(x)_k - vgg(y)_k.detach()|, k = relu1_1 .. relu5_1.  Differentiable in x only."""
@@ -1153,15 +1146,7 @@ class Vgg19(_Planned):
         if x.shape != y.shape or x.dim() != 4 or x.shape[1] != 3:
             raise ValueError('VGG inputs must be two (N, 3, H, W) tensors of the same shape, got %s and %s' % (tuple(x.shape), tuple(y.shape)))
         N, _, H, W = x.shape
-        train = self._wants_grad(x)
-        plan = self._get_plan(('VGGL', N, H, W), x.device, lambda p: self._describe(p, N, H, W), train=train)
-        out = torch.empty(5, device=x.device, dtype=torch.float32)
-        io = [x, y, out]
-        if not train:
-            plan.run(io, self.use_cuda_graph)
-            return out
-        (res,) = _PlanFunction.apply(self, plan, io, (0,), (2,), (0, 1), *([x] + list(self.parameters())))
-        return res
+        return self._run_plan(('VGGL', N, H, W), lambda p: self._describe(p, N, H, W), [x, y], (0,), (2,))[2]
 
 
 class AvgPool2(nn.Module):

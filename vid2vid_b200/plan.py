@@ -77,6 +77,7 @@ class Plan:
         self.finalized = False
         self.n_slots = 0
         self._graph_ok = False
+        self.outs = None        # {slot: shape} of the tensors a run writes, as the module that described the plan reports it
 
     def __del__(self):
         try:
@@ -96,7 +97,7 @@ class Plan:
     # ---- description
     def input(self, slot, N, C_src, c_off, Cn, H, W, exact_bf16=False):
         v = C.c_int()
-        L.check(L.lib().v2v_g_input_ex(self._h, slot, N, C_src, c_off, Cn, H, W, 1 if exact_bf16 else 0, C.byref(v)))
+        L.check(L.lib().v2v_g_input(self._h, slot, N, C_src, c_off, Cn, H, W, 1 if exact_bf16 else 0, C.byref(v)))
         self.n_slots = max(self.n_slots, slot + 1)
         return v.value
 
@@ -163,8 +164,8 @@ class Plan:
 
     def composite(self, s_raw, s_flow, s_weight, s_prev, prev_C, s_fg, s_mask, s_final, N, H, W, use_warp,
                   align_corners, s_raw_out=-1):
-        L.check(L.lib().v2v_g_composite_ex(self._h, s_raw, s_flow, s_weight, s_prev, prev_C, s_fg, s_mask, s_final, s_raw_out,
-                                           N, H, W, int(use_warp), int(align_corners)))
+        L.check(L.lib().v2v_g_composite(self._h, s_raw, s_flow, s_weight, s_prev, prev_C, s_fg, s_mask, s_final, s_raw_out,
+                                        N, H, W, int(use_warp), int(align_corners)))
         self.n_slots = max(self.n_slots, s_raw + 1, s_flow + 1, s_weight + 1, s_prev + 1, s_fg + 1, s_mask + 1,
                            s_final + 1, s_raw_out + 1)
 
@@ -224,11 +225,7 @@ class Plan:
 
     def profile(self, io=None):
         """Eager run with a CUDA event after every kernel -> list of (kind, ms, conv_macs)."""
-        io = io if io is not None else self.last_io
-        arr = (C.c_void_p * self.n_slots)()
-        for i in range(self.n_slots):
-            t = io[i] if i < len(io) else None
-            arr[i] = t.data_ptr() if t is not None else None
+        arr = self._io_array(io if io is not None else self.last_io)
         n = self.num_kernels + 4
         kinds, ms, macs, cnt = (C.c_int * n)(), (C.c_float * n)(), (C.c_double * n)(), C.c_int()
         L.check(L.lib().v2v_plan_profile(self._h, arr, self.n_slots, self._stream(), n, kinds, ms, macs,
